@@ -16,20 +16,19 @@ __device__ void linearize(Phase& ph, Ctx& c) {
   ph.lap2(23);
 }
 
-// Schur complement set-up for a damping value; returns the buffer index of A_c^-1
 // Schur complement set-up for a damping value.  Hll^-1 (part of the operator) is always rebuilt; the two-level
 // preconditioner (dense diagonal blocks + coarse Galerkin inverse) only when `rebuild` -- a stale
-// preconditioner changes the PCG iteration count, never the solution.  Returns the buffer index of A_c^-1.
+// preconditioner changes the PCG iteration count, never the solution.
 __device__ __forceinline__ bool G_levels3(const Phase&) { return G.levels == 3; }
-__device__ int schur_setup(Phase& ph, Ctx& c, double lambda, Timer& ft, bool rebuild, int acinv_prev) {
+__device__ void schur_setup(Phase& ph, Ctx& c, double lambda, Timer& ft, bool rebuild) {
   ft.sync();
   ph.plane_inverse(lambda);
   team_barrier(c);
   ft.lap(8);
-  if (!rebuild && !G.prm.blocks_always) return acinv_prev;
+  if (!rebuild && !G.prm.blocks_always) return;
   ph.build_blocks(lambda);
   ft.lap(9);
-  if (!rebuild) { team_barrier(c); return acinv_prev; }   // level 1 refreshed for this linearisation, coarse level kept
+  if (!rebuild) { team_barrier(c); return; }   // level 1 refreshed for this linearisation, coarse level kept
   ph.coarse_wc();
   team_barrier(c);
   ft.lap(10);
@@ -37,9 +36,8 @@ __device__ int schur_setup(Phase& ph, Ctx& c, double lambda, Timer& ft, bool reb
   if (G_levels3(ph)) ph.build_groups(lambda);   // level 2: needs Wc2 / Yc2 (behind the barrier above) only
   team_barrier(c);
   ft.lap(11);
-  int r = ph.coarse_invert();
+  ph.coarse_invert();
   ft.lap(12);
-  return r;
 }
 
 // Solve (Hpp_d - W Hll_d^-1 W^T) x = -gp + W Hll_d^-1 gl by preconditioned CG, then back-substitute the
@@ -51,7 +49,7 @@ __device__ __forceinline__ void span_view(Ctx& c, bool global) {
   else { c.rank = c.lrank; c.tsize = c.ltsize; c.mirror = 0; }
 }
 
-__device__ double schur_solve(Phase& ph, Ctx& c, double lambda, int acinv, int* its, Timer& ft, bool warm) {
+__device__ double schur_solve(Phase& ph, Ctx& c, double lambda, int* its, Timer& ft, bool warm) {
   // spanning solve: the PCG phases are split over the CTAs of all ranks (every rank keeps full copies of the vectors)
   span_view(c, true);
   const bool resident = G.prm.resident && !c.use_tma && !c.mirror;   // block-resident loop (pcg_resident): loads its own caches
@@ -63,7 +61,7 @@ __device__ double schur_solve(Phase& ph, Ctx& c, double lambda, int acinv, int* 
   team_barrier(c);
   double v[2];
   int rcb = 0, cur = 0, it = 0;
-  v[0] = ph.precondition(0.0, nullptr, acinv, G.rcpart[0], G.rcpart[1], true);
+  v[0] = ph.precondition(0.0, nullptr, G.rcpart[0], G.rcpart[1], true);
   team_reduce<1>(c, G.red, v);
   rcb = 1;
   const double rz0 = v[0];
@@ -77,14 +75,14 @@ __device__ double schur_solve(Phase& ph, Ctx& c, double lambda, int acinv, int* 
     if (c.use_tma) { ph.solve_heavy(); team_barrier(c); }
     ph.pose_phase(false, G.xprev, lambda, G.q, G.qcpart);
     team_barrier(c);
-    v[0] = ph.precondition(1.0, G.xprev, acinv, G.rcpart[rcb], G.rcpart[rcb ^ 1], false);
+    v[0] = ph.precondition(1.0, G.xprev, G.rcpart[rcb], G.rcpart[rcb ^ 1], false);
     team_reduce<1>(c, G.red, v);
     rcb ^= 1;
     rz = v[0];
     if (!(rz > tol2 * rz0)) done = true;
   }
   if (rz0 > 0.0 && !done && resident) {
-    it = ph.pcg_resident(lambda, acinv, rcb, rz0, rz, tol2, ft);
+    it = ph.pcg_resident(lambda, rcb, rz0, rz, tol2, ft);
   } else if (rz0 > 0.0 && !done) {
     c.light = c.mirror ? 0 : 1;   // every value the loop exchanges between CTAs is read through L2 (ld.global.cg / bulk copies)
     while (it < G.prm.pcg_max_iter) {
@@ -105,7 +103,7 @@ __device__ double schur_solve(Phase& ph, Ctx& c, double lambda, int acinv, int* 
       const double pq = v[0];
       if (!(pq > 0.0)) break;  // breakdown (not SPD / exhausted precision)
       const double alpha = rz / pq;
-      v[0] = ph.precondition(alpha, G.pv[cur ^ 1], acinv, G.rcpart[rcb], G.rcpart[rcb ^ 1], false);
+      v[0] = ph.precondition(alpha, G.pv[cur ^ 1], G.rcpart[rcb], G.rcpart[rcb ^ 1], false);
       team_reduce<1>(c, G.red, v);
       ft.lap(20);
       rcb ^= 1;
@@ -179,11 +177,10 @@ __device__ void run_graph_impl(Ctx& c) {
     linearize(ph, c);
     if (lead) res->relin = 1;
     if (P.debug_stage >= 1) {
-      int acinv = schur_setup(ph, c, P.debug_lambda, ft, true, 0);
-      if (lead) res->status = acinv;
+      schur_setup(ph, c, P.debug_lambda, ft, true);
       if (P.debug_stage >= 2) {
         int its = 0;
-        double dn = schur_solve(ph, c, P.debug_lambda, acinv, &its, ft, false);
+        double dn = schur_solve(ph, c, P.debug_lambda, &its, ft, false);
         if (lead) { res->pcg_iters = its; res->chi2_final = dn; }
       }
     }
@@ -202,10 +199,10 @@ __device__ void run_graph_impl(Ctx& c) {
   if (P.mode == MODE_BATCH) { err = ph.chi2(false); nchi++; }
   tm.lap(4);
   const double err0 = err;
-  int acinv = schur_setup(ph, c, lambda, ft, true, 0);
+  schur_setup(ph, c, lambda, ft, true);
   int prec_builds = 1;
   tm.lap(1);
-  double dnorm = schur_solve(ph, c, lambda, acinv, &its, ft, false);
+  double dnorm = schur_solve(ph, c, lambda, &its, ft, false);
   pcg_total += its;
   int its_ref = its;  // PCG iterations right after the last preconditioner build
   tm.lap(2);
@@ -257,9 +254,9 @@ __device__ void run_graph_impl(Ctx& c) {
         // refresh the preconditioner only when the last solve needed clearly more iterations than the one right
         // after the previous build (deterministic rule, identical on every CTA)
         const bool rebuild = (P.prec_refresh == 0) || (last_pcg > its_ref * P.refresh_pct / 100 + P.refresh_add);
-        acinv = schur_setup(ph, c, lambda, ft, rebuild, acinv);
+        schur_setup(ph, c, lambda, ft, rebuild);
         tm.lap(1);
-        dnorm = schur_solve(ph, c, lambda, acinv, &its, ft, rejected && P.warm_start);
+        dnorm = schur_solve(ph, c, lambda, &its, ft, rejected && P.warm_start);
         if (rebuild) { its_ref = its; prec_builds++; }
       }
       last_pcg = its;
@@ -292,9 +289,9 @@ __device__ void run_graph_impl(Ctx& c) {
       err = err_new;
       {
         const bool rebuild = (P.prec_refresh == 0) || (last_pcg > its_ref * P.refresh_pct / 100 + P.refresh_add);
-        acinv = schur_setup(ph, c, 0.0, ft, rebuild, acinv);
+        schur_setup(ph, c, 0.0, ft, rebuild);
         tm.lap(1);
-        dnorm = schur_solve(ph, c, 0.0, acinv, &its, ft, false);
+        dnorm = schur_solve(ph, c, 0.0, &its, ft, false);
         if (rebuild) { its_ref = its; prec_builds++; }
       }
       last_pcg = its;
@@ -353,6 +350,7 @@ __global__ void __launch_bounds__(kThreads, 1) lm_kernel(const DevGraph* graphs,
     mbar_init(gbar, 1);
     mbar_init(gbar + 1, 1);
     mbar_init(gbar + 2, 1);
+    mbar_init(gbar + 3, 1);
   }
   if ((threadIdx.x & 31) == 0) {
     unsigned long long* bar = reinterpret_cast<unsigned long long*>(smem + kSmBar) + (threadIdx.x >> 5) * 2;

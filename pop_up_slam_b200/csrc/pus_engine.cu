@@ -96,7 +96,6 @@ struct Solver {
   pus_stats stats;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int num_sms = 0;
-  int last_acinv = 0;
 
   Solver() {
     std::memset(&prop, 0, sizeof(prop));
@@ -249,7 +248,7 @@ static int upload(Solver* s) {
     AL(Hpp, N * 36, "Hpp"); AL(gp, N * 6, "gp"); AL(Hll, M * 9, "Hll"); AL(gl, M * 3, "gl"); AL(Hinv, M * 9, "Hinv");
     AL(ypart, 8, "ypart"); AL(upartb, (size_t)std::max(1, c.ngrp) * 3, "upartb"); AL(hpart, (size_t)std::max(1, c.n_atask) * 9, "hpart");
     AL(Binv, (size_t)c.nblk * kPackedBlock, "Binv"); AL(Wc, (size_t)c.nce * 18, "Wc"); AL(Yc, (size_t)c.nce * 18, "Yc");
-    AL(Ac[0], ac_doubles(6 * c.nc_pad), "Ac0"); AL(Ac[1], ac_doubles(6 * c.nc_pad), "Ac1");
+    AL(Ac, ac_doubles(6 * c.nc_pad), "Ac"); AL(Atri, ac_tri_doubles(6 * c.nc_pad), "Atri"); AL(Apan, ac_panel_doubles(6 * c.nc_pad), "Apan");
     AL(Wc2, (size_t)c.nce2 * 18, "Wc2"); AL(Yc2, (size_t)c.nce2 * 18, "Yc2"); AL(D2inv, (size_t)c.ng2 * kBlockDim * kBlockDim, "D2inv");
 #undef AL
     {
@@ -354,7 +353,7 @@ static int auto_team(const Solver* s, int limit) {
   if (s->opt.team_ctas > 0) return std::min(std::max(1, s->opt.team_ctas), limit);
   int need = std::max((s->c.ntile + kWarps - 1) / kWarps, (s->c.nblk + kSlots - 1) / kSlots);
   need = std::max(need, (6 * s->c.nc + kWarps - 1) / kWarps);  // one warp per row of the coarse inverse
-  need = std::max(need, (6 * s->c.nc_pad + 15) / 16);           // <= two 8-row MMA tiles per CTA in the coarse inversion
+  need = std::max(need, (6 * s->c.nc_pad + 15) / 16);           // about 16 rows of A_c per CTA: a few tiles each in its inversion
   // a CTA per 16-pose block when the device has room: the phases of the PCG loop are latency-bound, so fewer owned blocks per
   // CTA shorten every phase
   if (s->c.nblk <= limit) return std::min(std::max(std::max(need, s->c.nblk), 1), limit);
@@ -396,15 +395,12 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
       for (int t = 1; t <= std::min(need, max_ctas); t++) {
         const int teams_t = std::min(n, max_ctas / t), waves = (n + teams_t - 1) / teams_t;
         double worst = 0;
-        bool ok = true;
-        for (int i = 0; i < n && ok; i++) {
+        for (int i = 0; i < n; i++) {
           const Compiled& cc = ss[i]->c;
-          if (kSmWork + gj_smem_bytes(6 * cc.nc_pad, t) > (size_t)kSmemBytes) { ok = false; break; }
           const int b = (cc.nblk + t - 1) / t;
           const bool res = resident_fits(cc, t) && !(ss[i]->opt.reserved[2] & 32);
           worst = std::max(worst, res ? 3.0 + 0.2 * b : 4.3 + 4.2 * ((b + kSlots - 1) / kSlots));
         }
-        if (!ok) continue;
         const double cost = waves * worst;
         if (cost <= best) { best = cost; best_t = t; }   // (ties: the larger team)
       }
@@ -433,8 +429,6 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
       int t = 0;
       if (cl == team) t = cl;
       else if (n == 1 && s0->opt.team_ctas <= 0 && s0->c.levels == 2 && s0->c.nblk <= 2 * cl) t = cl;
-      for (int i = 0; i < n && t; i++)
-        if (kSmWork + gj_smem_bytes(6 * ss[i]->c.nc_pad, t) > (size_t)kSmemBytes) t = 0;
       if (t > 1) {
         if (t > 8) cudaFuncSetAttribute(kplain::lm_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
         const int teams = (n == 1) ? 1 : std::min(n, max_ctas / t);
@@ -457,14 +451,6 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
           cudaGetLastError();
         }
       }
-    }
-  }
-  // the coarse inversion stages a 48x48 pivot block, the band's coefficient rows and a 48x256 panel chunk in shared memory
-  for (int i = 0; i < n; i++) {
-    const int ldmc = 6 * ss[i]->c.nc_pad;
-    if (kSmWork + gj_smem_bytes(ldmc, team) > (size_t)kSmemBytes) {
-      g_err = "team of " + std::to_string(team) + " CTAs is too small for a coarse operator of order " + std::to_string(ldmc);
-      return -1;
     }
   }
   // per-graph parameter blocks
@@ -548,7 +534,6 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
     st.n_pose_prior = npr; st.n_odometry = s->c.Epf - npr; st.n_plane_prior = s->c.Elp;
     st.gpu_launches = 1; st.grid_ctas = grid; st.block_threads = kThreads;
     for (int k = 0; k < 24; k++) st.phase_ms[k] = s->res.phase_ns[k] * 1e-6;
-    if (mode == MODE_DEBUG) s->last_acinv = s->res.status;
     st.gpu_launches = 1;
   }
   return 0;
@@ -1398,12 +1383,11 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
         for (int k = 0; k < 18; k++) out[e * 18 + k] = tmp[(e >> 5) * kWStride + k * 32 + (e & 31)];
     return cnt;
   }
-  if (nm == "Acinv") nm = s->last_acinv ? "Ac1" : "Ac0";
-  if (nm == "Ac0" || nm == "Ac1") {  // de-tiled: row-major ldm x ldm
+  if (nm == "Acinv") {  // de-tiled: row-major ldm x ldm
     const int ldm = 6 * c.nc_pad;
     const size_t n = ac_doubles(ldm);
     std::vector<double> tmp(n);
-    if (cudaMemcpy(tmp.data(), s->hd.Ac[nm == "Ac1"], n * 8, cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
+    if (cudaMemcpy(tmp.data(), s->hd.Ac, n * 8, cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
     long long cnt = (long long)ldm * ldm;
     if (cnt <= cap)
       for (int r = 0; r < ldm; r++)

@@ -8,7 +8,8 @@
 //   Schur       Hll^-1 (3x3); dense 96x96 diagonal blocks of S = Hpp - W Hll^-1 W^T built by pose-pair ownership and
 //               inverted in shared memory (blocked Gauss-Jordan, rank-8 updates on the FP64 tensor cores);
 //               Galerkin coarse operator on piecewise-linear trajectory modes, assembled output-stationary and
-//               inverted in HBM (48-wide pivots, panel chunks staged by bulk async copies, rank-48 DMMA updates)
+//               inverted in place by a symmetric block sweep of its lower triangle (48x48 tiles split over the team,
+//               pivot-column snapshots staged by bulk async copies, DMMA tile updates, look-ahead pivot inversion)
 //   PCG         implicit-Schur operator: plane-major sweep (W^T p), plane solve, pose-major sweep (W v),
 //               two-level additive preconditioner, deterministic segmented reductions; on large graphs the W / Wt
 //               tiles and the dense preconditioner blocks stream through shared memory by cp.async.bulk + mbarrier
@@ -103,7 +104,8 @@ struct DevGraph {
   double *W, *Wt, *JP, *JL, *PF, *LP;
   double *Hpp, *gp, *Hll, *gl, *Hinv, *vl, *dl;
   double *upart, *ypart;
-  double *Binv, *Wc, *Yc, *Ac[2];
+  double *Binv, *Wc, *Yc;
+  double *Ac, *Atri, *Apan;     // A_c^-1 for the applies (ac_index); the triangle and panel buffers of its inversion
   double *x, *r, *z, *q, *b, *pv[2], *xprev, *zc;
   double *rcpart[2], *qcpart;
   double *red;
@@ -134,7 +136,7 @@ struct Ctx {
   int l3_local;          // three-level mode, small level 3: every CTA applies A_3^-1 itself (no exchange of its result)
   int use_tma;           // this graph streams its W / Wt tiles through the per-warp TMA staging buffers
   unsigned tma_par;      // phase parity of this warp's two staging mbarriers (bit s = stage s)
-  unsigned gj_par;       // phase parity of the coarse inversion's two panel mbarriers
+  unsigned gj_par;       // phase parity of the coarse inversion's four mbarriers (bit s = mbarrier s)
   // spanning mode: the team seen by the split PCG phases covers the CTAs of all ranks (rank = span_r * ltsize + lrank);
   // the replicated phases (linearise, Schur set-up, update) use the local view.  `mirror` = stores to the shared PCG
   // vectors are repeated into every peer's arena.
@@ -343,21 +345,44 @@ __device__ __forceinline__ void dmma884(double* cacc, double a, double b) {
                : "d"(a), "d"(b));
 }
 
-// blocked Gauss-Jordan inversion of A_c: chunk width and padded shared-memory strides, rows per CTA
-constexpr int kGjChunk = 128, kGjLdT = 52, kGjLdR = kGjChunk + 4, kGjLdP = 52, kGjLdQ = 12;
-// A_c (and its inverse) live in HBM as 48-row x 128-column tiles, each stored with the padded row stride the MMA
-// fragment loads want, so that one bulk copy brings a whole pivot-panel chunk into shared memory ready to use
+// A_c^-1 as the PCG applies read it: full rows, stored as 48-row x 128-column tiles with a padded row stride
+constexpr int kGjChunk = 128, kGjLdR = kGjChunk + 4;
 constexpr int kGjTile = 48 * kGjLdR;   // doubles per tile
 __host__ __device__ inline int ac_chunks(int ldm) { return (ldm + kGjChunk - 1) / kGjChunk; }
 __host__ __device__ inline size_t ac_index(int ldm, int row, int col) {
   return ((size_t)(row / 48) * ac_chunks(ldm) + (col / kGjChunk)) * kGjTile + (size_t)(row % 48) * kGjLdR + (col % kGjChunk);
 }
 __host__ __device__ inline size_t ac_doubles(int ldm) { return (size_t)(ldm / 48) * ac_chunks(ldm) * kGjTile; }
-__host__ __device__ inline int gj_band_rows(int ldm, int team) { return 8 * ((ldm / 8 + team - 1) / team); }
-__host__ __device__ inline size_t gj_smem_bytes(int ldm, int team) {
-  const size_t R = gj_band_rows(ldm, team);
-  return (2 * 48 * kGjLdP + 48 * kGjLdQ + R * 48 + R * kGjLdT + 2 * 48 * (size_t)kGjLdR) * 8;   // two panel buffers
+// A_c while it is assembled and inverted: the lower triangle only, as 48x48 tiles (I, J), I >= J, each stored with a
+// padded row stride (conflict-free DMMA fragment loads; one bulk copy moves a tile).  Tiles are numbered band by band
+// (bands of two tile rows), column by column inside a band: (0,0) (1,0) (1,1) | (2,0) (3,0) (2,1) (3,1) (2,2) (3,2) (3,3) | ...
+// so that a contiguous range of tile numbers is a compact patch (few tile rows, few tile columns).
+constexpr int kAcLd = 52, kAcTile = 48 * kAcLd;
+__host__ __device__ inline int ac_ntri(int ldm) { const int nb = ldm / 48; return nb * (nb + 1) / 2; }
+__host__ __device__ inline int tri_index(int nb, int i, int j) {
+  const int b = i >> 1;
+  const int p = (2 * b + 1 < nb) ? (j <= 2 * b ? 2 * j + (i - 2 * b) : 4 * b + 2) : j;
+  return b * (2 * b + 1) + p;
 }
+__host__ __device__ inline void tri_tile(int nb, int t, int& i, int& j) {
+  int b = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.25);
+  while (b > 0 && b * (2 * b + 1) > t) b--;
+  while ((b + 1) * (2 * b + 3) <= t) b++;
+  const int p = t - b * (2 * b + 1);
+  if (2 * b + 1 < nb) {
+    if (p < 4 * b + 2) { j = p >> 1; i = 2 * b + (p & 1); }
+    else { i = j = 2 * b + 1; }
+  } else {
+    i = 2 * b; j = p;
+  }
+}
+// device buffers of the inversion: the triangle, the pivot-column snapshots [2 step parities][nb tiles] and the pivot
+// inverses [2 step parities] (one allocation: snapshots, then inverses)
+__host__ __device__ inline size_t ac_tri_doubles(int ldm) { return (size_t)ac_ntri(ldm) * kAcTile; }
+__host__ __device__ inline size_t ac_panel_doubles(int ldm) { return (size_t)(2 * (ldm / 48) + 2) * kAcTile; }
+// A diagonal tile counts as this many tile updates when the triangle is split over the team: its owner updates it first
+// in the step before it becomes the pivot, inverts it and publishes the inverse while the other CTAs update their tiles
+constexpr int kPivotWeight = 10;
 
 // shared-memory carve-up (bytes)
 constexpr int kSmRed = 0;                            // [kWarps][4] + [4] doubles
@@ -397,12 +422,15 @@ static_assert(kSmPoseEnd <= kSmCache, "pose-phase buffers overlap the block cach
 // TMA staging (large graphs; replaces the block cache): per warp two 4608-byte W / Wt tiles, filled by
 // cp.async.bulk and signalled through one mbarrier per stage
 constexpr int kSmBar = 768;                           // [kWarps][2] mbarriers (u64)
-constexpr int kSmGjBar = 1024;                        // mbarriers of the coarse inversion's panel pipeline (2) / the block ring (3)
+constexpr int kSmGjBar = 1024;                        // mbarriers of the coarse inversion (4) / the block ring (3)
 constexpr int kSmTma = kSmCache;
 constexpr int kTileBytes = 18 * 32 * 8;
 constexpr int kSmTmaEnd = kSmTma + kWarps * 2 * kTileBytes;
 static_assert(kSmBar + kWarps * 2 * 8 <= kSmGjBar && kSmGjBar + 32 <= kSmWork, "mbarriers overlap the work area");
 static_assert(kSmTmaEnd <= 227 * 1024, "TMA staging buffers");
+// coarse inversion: eight 48x48 tiles (P, two T rows, three snapshot tiles, two staging tiles), the coefficient columns of the pivot
+// inversion and the owned tile range -- the same for every team size
+static_assert(kSmWork + (8 * kAcTile + 48 * 12 + 2) * 8 <= kSmemBytes, "coarse inversion buffers");
 static_assert(kSmemBytes <= 227 * 1024, "dynamic shared memory");
 
 
@@ -741,6 +769,28 @@ __device__ __forceinline__ double* gj_invert_smem(double* Mc, double* Mn, double
     double* t = Mc; Mc = Mn; Mn = t;
   }
   return Mc;
+}
+
+// acc += A B for 48x48 tiles in shared memory (row stride kAcLd) on the FP64 tensor cores; B is read as Bm^T (BT) or Bm.
+// Warp w owns the 8x8 output tiles q = w, w + 16, w + 32 (< 36): acc[s] = rows 8 (q / 6) + lane / 4, columns
+// 8 (q % 6) + 2 (lane % 4) + {0, 1}.  Three accumulator chains per output tile (the MMA latency is long, the chain short).
+template <bool BT>
+__device__ __forceinline__ void mma48(double (&acc)[3][2], const double* A, const double* Bm) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, fr = lane >> 2, fc = lane & 3;
+#pragma unroll
+  for (int s = 0; s < 3; s++) {
+    const int q = warp + 16 * s;
+    if (q < 36) {
+      const int m = q / 6, n = q - 6 * m;
+      const double* a = A + (8 * m + fr) * kAcLd + fc;
+      const double* b = BT ? Bm + (8 * n + fr) * kAcLd + fc : Bm + fc * kAcLd + 8 * n + fr;
+      double x[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
+#pragma unroll
+      for (int k = 0; k < 12; k++) dmma884(k % 3 == 0 ? acc[s] : x[k % 3 - 1], a[4 * k], BT ? b[4 * k] : b[4 * k * kAcLd]);
+      acc[s][0] += x[0][0] + x[1][0];
+      acc[s][1] += x[0][1] + x[1][1];
+    }
+  }
 }
 
 // Pose3d_Plane3d_Factor2 edges are rare (disabled in the shipped demo): keep their extra arithmetic out of the
@@ -1363,18 +1413,18 @@ struct Phase {
     __syncthreads();
   }
 
-  // -------- Schur setup, part 4: A_c = P^T S P, one warp per coarse row panel --------
-  // Output-stationary: every thread owns entries (i, j) of A_c = P^T S P and writes each exactly once
-  // (coalesced along j, tiled layout):  pose part (supports of the two nodes overlap: |a-b| <= 1), pose-pose factors
+  // -------- Schur setup, part 4: A_c = P^T S P, lower triangle of 48x48 tiles --------
+  // Output-stationary: every thread owns entries (i, j) of the triangle of A_c = P^T S P and writes each exactly once
+  // (coalesced along j inside a tile row):  pose part (supports of the two nodes overlap: |a-b| <= 1), pose-pose factors
   // coupling the supports (host-built per-pair list), light planes (host-built per-pair list of (Yc, Wc) products),
   // heavy planes (Yc / Wc rows of the plane staged per node in shared memory: dense rank-3 update, one pass each).
+  // Tile column 0 also goes to the step-0 pivot-column snapshot of coarse_invert().
   __device__ void coarse_assemble(double lambda) {
-    const int ldm = G.ldmc, nc = G.nc, n6 = 6 * nc;
-    double* A = G.Ac[0];
+    const int ldm = G.ldmc, nc = G.nc, n6 = 6 * nc, nb = ldm / 48;
     double* Yh = reinterpret_cast<double*>(g_smem + kSmWork);   // [nc][18]
     double* Wh = Yh + (size_t)nc * 18;                          // [nc][18]
     const int npass = max(1, G.n_hv);
-    const long long total = (long long)ldm * ldm;
+    const long long total = (long long)ac_ntri(ldm) * 48 * 48;
     for (int pass = 0; pass < npass; pass++) {
       if (G.n_hv > 0) {
         __syncthreads();
@@ -1388,11 +1438,19 @@ struct Phase {
         }
         __syncthreads();
       }
+      int tprev = -1, ti = 0, tj = 0;
       for (long long idx = tid_team(); idx < total; idx += nthr_team()) {
-        const int i = (int)(idx / ldm), j = (int)(idx - (long long)i * ldm);
-        double* out = A + ac_index(ldm, i, j);
+        const int t = (int)(idx / 2304), e = (int)(idx - (long long)t * 2304), er = e / 48, ec = e - er * 48;
+        if (t != tprev) { tri_tile(nb, t, ti, tj); tprev = t; }
+        const int i = 48 * ti + er, j = 48 * tj + ec;
+        double* out = G.Atri + (size_t)t * kAcTile + er * kAcLd + ec;
+        double* snap = (tj == 0) ? G.Apan + (size_t)ti * kAcTile + er * kAcLd + ec : nullptr;
         if (i >= n6 || j >= n6) {   // padding: identity
-          if (pass == 0) *out = (i == j) ? 1.0 : 0.0;
+          if (pass == 0) {
+            const double v = (i == j) ? 1.0 : 0.0;
+            *out = v;
+            if (snap) *snap = v;
+          }
           continue;
         }
         const int a = i / 6, r = i - a * 6, b = j / 6, cc = j - b * 6;
@@ -1428,162 +1486,239 @@ struct Phase {
           v -= y[0] * w[0] + y[1] * w[1] + y[2] * w[2];
         }
         *out = v;
+        if (snap) *snap = v;
       }
     }
-    fence_proxy_async();  // A_c is read back by bulk copies in coarse_invert()
+    fence_proxy_async();  // the snapshot is read by bulk copies in coarse_invert()
   }
 
-  // -------- Schur setup, part 5: invert A_c in HBM: blocked Gauss-Jordan with 48-wide pivot blocks ---------
-  // Step k (pivot block K = 48 rows/cols): every CTA inverts A_KK in shared memory (P), forms T = A[band,K]*P for
-  // the band of rows it owns, then streams the pivot row panel A[K,:] through shared memory in 256-column chunks
-  // and writes   (K,K): P ; (K,j): P A_Kj ; (i,K): -T ; (i,j): A_ij - T A_Kj   to the other buffer.
-  // One team barrier per step; ldm/48 steps.  Returns the index of the buffer holding A_c^-1.
-  __device__ int coarse_invert() {
-    constexpr int PW = 6 * kPivotNodes;   // 48
-    constexpr int CW = kGjChunk;          // columns of the pivot row panel staged at a time
-    constexpr int LDT = kGjLdT, LDR = kGjLdR;  // padded strides: the DMMA fragment loads are bank-conflict free
-    const int ldm = G.ldmc, nsteps = ldm / PW;
-    constexpr int LDP = kGjLdP, LDQ = kGjLdQ;
-    double* Pa = reinterpret_cast<double*>(g_smem + kSmWork);  // [PW][LDP] pivot block (ping)
-    double* Pb = Pa + PW * LDP;                                // [PW][LDP] (pong); ends up holding the inverse
-    double* TQ = Pb + PW * LDP;                                // [PW][LDQ] coefficient columns of the inner block step
-    const int R = gj_band_rows(ldm, c.tsize);                  // rows per CTA (whole 8-row MMA tiles)
-    double* Ab = TQ + PW * LDQ;                                // [band][PW] the band's slice of the pivot column block
-    double* Tn = Ab + (size_t)R * PW;                          // [band][LDT]  -(A[band,K] * P)   (+P in pivot rows)
-    double* Rc = Tn + (size_t)R * LDT;                         // [2][PW][LDR] chunks of the pivot row panel
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int r0 = min(ldm, c.rank * R), r1 = min(ldm, r0 + R);
-    const int band = r1 - r0, mtiles = band / 8;
-    const int fr = lane >> 2, fc = lane & 3;   // MMA fragment coordinates
-    int cur = 0;
-    for (int k = 0; k < nsteps; k++) {
-      const double* src = G.Ac[cur];
-      double* dst = G.Ac[cur ^ 1];
-      const int k0 = k * PW;
+  // -------- Schur setup, part 5: A_c^-1 by an in-place symmetric block sweep of the triangle ---------
+  // Step K (pivot block K, P = A_KK^-1):  A_KK <- -P,  A_iK <- A_iK P,  A_ij <- A_ij - A_iK P A_Kj  (i, j != K).  The
+  // matrix stays symmetric, so only the tiles (i, j), i >= j, are kept; after the last step they hold -A_c^-1.  SPD: no
+  // pivoting.  Every CTA owns a contiguous range of tile numbers (a compact patch, see tri_index) for the whole inversion.
+  // Step K overwrites pivot column K, so it reads only a snapshot of that column (C_i = A_iK, taken by the owners of
+  // those tiles at the end of step K-1; double-buffered by step parity), P and the CTA's own tiles:  T_i = -C_i P once per
+  // tile row of a band, then, column by column, the snapshot tile C_j streams in by bulk copy (two more in flight)
+  // and every owned tile of the column gets  (i,j): A_ij + T_i C_j^T,  (K,j): P C_j^T,  (i,K): -T_i,  (K,K): -P
+  // on the FP64 tensor cores.  Look-ahead: the owner of diagonal tile K+1 updates that tile first, inverts it and
+  // publishes P_{K+1} before it updates the rest, so no CTA inverts a pivot redundantly (kPivotWeight gives it fewer
+  // tiles).  One team barrier per step.  The last step writes -(its result), mirrored, into the full layout of G.Ac.
+  __device__ void coarse_invert() {
+    const int ldm = G.ldmc, nb = ldm / 48, nt = ac_ntri(ldm);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3;
+    double* Ps = reinterpret_cast<double*>(g_smem + kSmWork);   // P_K
+    double* Tr = Ps + kAcTile;                                  // [2] T_i of the two tile rows of the current band
+    double* Cb = Tr + 2 * kAcTile;                              // [3] snapshot tiles C_j (ring)
+    double* Sb = Cb + 3 * kAcTile;                              // [2] C_i while T_i is formed; pivot inversion
+    double* TQ = Sb + 2 * kAcTile;                              // [48][12] coefficient columns of gj_invert_smem
+    int* rng = reinterpret_cast<int*>(TQ + 48 * 12);            // owned tile numbers [rng[0], rng[1])
+    unsigned long long* mb = reinterpret_cast<unsigned long long*>(g_smem + kSmGjBar);   // [0..2]: Cb; [3]: Ps, Sb
+    double* piv = G.Apan + (size_t)2 * nb * kAcTile;            // [2] P_K by step parity
+
+    // owner(t): the CTA whose share of the total weight holds the middle of tile t (a diagonal tile weighs 1 + kPivotWeight)
+    if (tid < 2) rng[tid] = nt;
+    __syncthreads();
+    {
+      const long long T = c.tsize, W2 = 2ll * (nt + (long long)kPivotWeight * nb);
+      auto owner = [&](int t) {
+        int i, j;
+        tri_tile(nb, t, i, j);
+        const int b = i >> 1;
+        const long long before = t + (long long)kPivotWeight * (2 * b + ((i == 2 * b + 1 && j >= 2 * b) ? 1 : 0));
+        return (int)min(T - 1, (2 * before + 1 + (i == j ? kPivotWeight : 0)) * T / W2);
+      };
+      for (int t = tid; t < nt; t += kThreads) {
+        const int o = owner(t), op = t > 0 ? owner(t - 1) : -1;
+        if (o >= c.rank && op < c.rank) rng[0] = t;
+        if (o > c.rank && op <= c.rank) rng[1] = t;
+      }
+    }
+    __syncthreads();
+    const int t0 = rng[0], t1 = rng[1];
+
+    // bulk copies of up to three tiles on one mbarrier phase (the CTA's last accesses of dst are behind a barrier)
+    auto fetch = [&](int bar, int n, double* d0, const double* s0, double* d1 = nullptr, const double* s1 = nullptr,
+                     double* d2 = nullptr, const double* s2 = nullptr) {
+      if (tid == 0) {
+        fence_proxy_async();
+        mbar_expect_tx(mb + bar, (unsigned)(n * kAcTile * 8));
+        tma_copy_1d(d0, s0, (unsigned)(kAcTile * 8), mb + bar);
+        if (n > 1) tma_copy_1d(d1, s1, (unsigned)(kAcTile * 8), mb + bar);
+        if (n > 2) tma_copy_1d(d2, s2, (unsigned)(kAcTile * 8), mb + bar);
+      }
+    };
+    auto wait = [&](int bar) {
+      mbar_wait(mb + bar, (c.gj_par >> bar) & 1u);
+      c.gj_par ^= 1u << bar;
+    };
+    auto frag = [&](int s, int& r, int& cc) {   // position of accumulator s of mma48 in the 48x48 tile
+      const int q = warp + 16 * s;
+      r = 8 * (q / 6) + fr;
+      cc = 8 * (q % 6) + 2 * fc;
+      return q < 36;
+    };
+    auto form_T = [&](double* dst, const double* Ci) {   // dst = -Ci P
+      double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+      mma48<false>(acc, Ci, Ps);
+      int r, cc;
+#pragma unroll
+      for (int s = 0; s < 3; s++)
+        if (frag(s, r, cc)) *reinterpret_cast<double2*>(dst + r * kAcLd + cc) = make_double2(-acc[s][0], -acc[s][1]);
+    };
+    auto group_end = [&](int t) {   // one past the column group that starts at owned tile t (the tiles of one column in one band)
+      int i, j, i2, j2;
+      tri_tile(nb, t, i, j);
+      if (t + 1 < t1) {
+        tri_tile(nb, t + 1, i2, j2);
+        if (j2 == j && (i2 >> 1) == (i >> 1)) return t + 2;
+      }
+      return t + 1;
+    };
+    auto load_base = [&](int t, double (&acc)[3][2]) {
+      const double* tile = G.Atri + (size_t)t * kAcTile;
+      int r, cc;
+#pragma unroll
+      for (int s = 0; s < 3; s++)
+        if (frag(s, r, cc)) {
+          const double2 v = __ldcg(reinterpret_cast<const double2*>(tile + r * kAcLd + cc));
+          acc[s][0] = v.x;
+          acc[s][1] = v.y;
+        }
+    };
+
+    for (int K = 0; K < nb; K++) {
+      const bool last = (K == nb - 1);
+      const double* snap = G.Apan + (size_t)(K & 1) * nb * kAcTile;    // C_i = snap + i kAcTile
+      double* snapn = G.Apan + (size_t)((K + 1) & 1) * nb * kAcTile;   // the snapshot for step K + 1
+      auto tile_col = [&](int t) { int i, j; tri_tile(nb, t, i, j); return j; };
+      auto issue_col = [&](int t, int slot) {   // the snapshot tile of the column group starting at t, unless it is column K
+        if (t < t1 && tile_col(t) != K) fetch(slot, 1, Cb + slot * kAcTile, snap + (size_t)tile_col(t) * kAcTile);
+      };
+      issue_col(t0, 0);
+      if (t0 < t1) issue_col(group_end(t0), 1);
+      const int d = K + 1;
+      const bool ahead = !last && tri_index(nb, d, d) >= t0 && tri_index(nb, d, d) < t1;   // this CTA inverts the next pivot
+      // P_K (for K = 0 nobody has published it: every CTA inverts A_00, snapshot tile 0), and C_{K+1} for the look-ahead
+      if (K == 0) fetch(3, ahead ? 2 : 1, Sb + kAcTile, snap, Sb, snap + (size_t)d * kAcTile);
+      else fetch(3, ahead ? 2 : 1, Ps, piv + (size_t)(K & 1) * kAcTile, Sb, snap + (size_t)d * kAcTile);
+      wait(3);
+      if (K == 0) {
+        const double* inv = gj_invert_smem<6, kAcLd>(Sb + kAcTile, Ps, TQ);
+        if (inv != Ps)
+          for (int e = tid; e < 48 * 48; e += kThreads) Ps[(e / 48) * kAcLd + e % 48] = inv[(e / 48) * kAcLd + e % 48];
+      }
       __syncthreads();
-      for (int i = tid; i < PW * PW; i += kThreads) Pa[(i / PW) * LDP + i % PW] = ldc(src + ac_index(ldm, k0 + i / PW, k0 + i % PW));
-      for (int i = tid; i < band * PW; i += kThreads) Ab[i] = ldc(src + ac_index(ldm, r0 + i / PW, k0 + i % PW));
-      __syncthreads();
+      lap1(7);
+      // look-ahead: diagonal tile K+1 first, then P_{K+1} = its inverse for the next step
+      if (ahead) {
+        form_T(Tr, Sb);
+        __syncthreads();
+        double acc[3][2];
+        load_base(tri_index(nb, d, d), acc);
+        mma48<true>(acc, Tr, Sb);
+        double* Md = Tr + kAcTile;
+        int r, cc;
+#pragma unroll
+        for (int s = 0; s < 3; s++)
+          if (frag(s, r, cc)) *reinterpret_cast<double2*>(Md + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+        __syncthreads();
+        const double* inv = gj_invert_smem<6, kAcLd>(Md, Sb + kAcTile, TQ);
+        double* out = piv + (size_t)(d & 1) * kAcTile;
+        for (int e = tid; e < 48 * 48; e += kThreads) out[(e / 48) * kAcLd + e % 48] = inv[(e / 48) * kAcLd + e % 48];
+        __syncthreads();
+      }
       lap1(6);
-      // inversion of the 48x48 pivot block (SPD: no pivoting), see gj_invert_smem()
-      const double* Pm = gj_invert_smem<PW / 8, LDP>(Pa, Pb, TQ);
-      lap(7);
-      // coefficient rows (negated): Tn = -(A[band,K] * P) for ordinary rows, +P for the rows of the pivot block
-      // itself, so that every entry outside the pivot columns is  base + sum_t Tn[row][t] * A[K][col]
-      // (base = A_ij, or 0 in pivot rows), and the pivot columns of the result are Tn itself
-      for (int i = tid; i < band * PW; i += kThreads) {
-        int lr = i / PW, t = i - lr * PW;
-        const int row = r0 + lr;
-        double acc;
-        if (row >= k0 && row < k0 + PW) {
-          acc = Pm[(row - k0) * LDP + t];
-        } else {
-          acc = 0;
-#pragma unroll 8
-          for (int sx = 0; sx < PW; sx++) acc -= Ab[lr * PW + sx] * Pm[sx * LDP + t];
+      // the owned tiles, column group by column group (a group: the tiles of one column inside one band, at most two)
+      int band = -1, g = 0;
+      for (int t = t0; t < t1;) {
+        int i0, j;
+        tri_tile(nb, t, i0, j);
+        const int b = i0 >> 1, te = group_end(t);
+        if (b != band) {   // T_i of the band's rows that the owned tiles need
+          band = b;
+          bool need[2] = {false, false};
+          for (int u = t; u < min(t1, (b + 1) * (2 * b + 3)); u++) {
+            int iu, ju;
+            tri_tile(nb, u, iu, ju);
+            if (iu != K) need[iu - 2 * b] = true;
+          }
+          if (need[0] || need[1]) {
+            const int r0 = need[0] ? 0 : 1;
+            fetch(3, need[0] && need[1] ? 2 : 1, Sb + r0 * kAcTile, snap + (size_t)(2 * b + r0) * kAcTile, Sb + kAcTile,
+                  snap + (size_t)(2 * b + 1) * kAcTile);
+            wait(3);
+            for (int r = 0; r < 2; r++)
+              if (need[r]) form_T(Tr + r * kAcTile, Sb + r * kAcTile);
+            __syncthreads();
+          }
+          lap1(7);
         }
-        Tn[lr * LDT + t] = acc;
-        dst[ac_index(ldm, row, k0 + t)] = acc;
-      }
-      __syncthreads();
-      lap(21);
-      // rank-48 update of the band on the FP64 tensor cores.  The pivot row panel A[K,:] streams through two
-      // shared-memory buffers in 128-column chunks (one bulk async copy per row, mbarrier-signalled, the next chunk
-      // in flight while this one is multiplied); warp w owns the chunk's w-th 8-column tile and up to two 8-row
-      // tiles of the band per pass: mma.m8n8k4 with A = Tn fragment, B = panel fragment, C = base (prefetched).
-      const int nchunk = (ldm + CW - 1) / CW;
-      unsigned long long* gbar = reinterpret_cast<unsigned long long*>(g_smem + kSmGjBar);
-      auto issue = [&](int ci) {   // one bulk copy per chunk: tile (k, ci) of the source, padded stride included
-        if (tid == 0) {
-          double* buf = Rc + (ci & 1) * PW * LDR;
-          tma_load_1d(buf, src + ((size_t)k * nchunk + ci) * kGjTile, (unsigned)(kGjTile * 8), gbar + (ci & 1));
+        if (te < t1) issue_col(group_end(te), (g + 2) % 3);
+        // the tiles' own values are read while the snapshot tile is still in flight
+        double acc[2][3][2];
+#pragma unroll
+        for (int k = 0; k < 2; k++) {
+          int i, jj;
+          if (t + k < te) tri_tile(nb, t + k, i, jj);
+#pragma unroll
+          for (int s = 0; s < 3; s++) acc[k][s][0] = acc[k][s][1] = 0.0;
+          if (t + k < te && i != K && j != K) load_base(t + k, acc[k]);
         }
-      };
-      auto loadC = [&](int ci, int m0, double (*cc)[2]) {
-        const int col = ci * CW + 8 * warp + 2 * fc;
+        if (j != K) wait(g % 3);
+        const double* Cj = Cb + (g % 3) * kAcTile;
 #pragma unroll
-        for (int mi = 0; mi < 2; mi++) {
-          const int row = r0 + 8 * (m0 + mi) + fr;
-          const bool ok = (m0 + mi < mtiles) && (ci * CW + 8 * warp < ldm) && !(row >= k0 && row < k0 + PW);
-          double2 v2 = make_double2(0.0, 0.0);
-          if (ok) v2 = __ldcg(reinterpret_cast<const double2*>(src + ac_index(ldm, row, col)));
-          cc[mi][0] = v2.x;
-          cc[mi][1] = v2.y;
-        }
-      };
-      // first tile pair (all there is when the team is large enough): offsets without the per-chunk index math
-      size_t rowoff[2];
-      bool rowld[2];
+        for (int k = 0; k < 2; k++) {
+          const int u = t + k;
+          if (u >= te) continue;
+          int i, jj;
+          tri_tile(nb, u, i, jj);
+          if (!last && i == d && j == d) continue;   // done by the look-ahead
+          const double* Ti = Tr + (i - 2 * b) * kAcTile;
+          int r, cc;
+          if (j == K) {   // (K,K): -P;  (i,K): -T_i
+            const double* src = (i == K) ? Ps : Ti;
 #pragma unroll
-      for (int mi = 0; mi < 2; mi++) {
-        const int row = r0 + 8 * mi + fr;
-        rowoff[mi] = (size_t)(min(row, ldm - 1) / 48) * nchunk * kGjTile + (size_t)(min(row, ldm - 1) % 48) * LDR + 8 * warp + 2 * fc;
-        rowld[mi] = (mi < mtiles) && !(row >= k0 && row < k0 + PW);
-      }
-      auto loadC0 = [&](int ci, double (*cc)[2]) {
+            for (int s = 0; s < 3; s++)
+              if (frag(s, r, cc)) { acc[k][s][0] = -src[r * kAcLd + cc]; acc[k][s][1] = -src[r * kAcLd + cc + 1]; }
+          } else if (i == K) {
+            mma48<true>(acc[k], Ps, Cj);
+          } else {
+            mma48<true>(acc[k], Ti, Cj);
+          }
 #pragma unroll
-        for (int mi = 0; mi < 2; mi++) {
-          double2 v2 = make_double2(0.0, 0.0);
-          if (rowld[mi] && (ci * CW + 8 * warp < ldm)) v2 = __ldcg(reinterpret_cast<const double2*>(src + rowoff[mi] + (size_t)ci * kGjTile));
-          cc[mi][0] = v2.x;
-          cc[mi][1] = v2.y;
-        }
-      };
-      double cn[2][2];
-      issue(0);
-      loadC0(0, cn);
-      for (int ci = 0; ci < nchunk; ci++) {
-        if (ci + 1 < nchunk) issue(ci + 1);
-        double acc[2][2] = {{cn[0][0], cn[0][1]}, {cn[1][0], cn[1][1]}};
-        if (ci + 1 < nchunk) loadC0(ci + 1, cn);
-        mbar_wait(gbar + (ci & 1), (c.gj_par >> (ci & 1)) & 1u);
-        c.gj_par ^= (1u << (ci & 1));
-        const double* buf = Rc + (ci & 1) * PW * LDR;
-        const int col = ci * CW + 8 * warp + 2 * fc;
-        const bool nlive = (ci * CW + 8 * warp < ldm);
-        const bool colK = (col >= k0 && col < k0 + PW);   // pivot columns were written from Tn (whole tiles)
-        for (int m0 = 0; m0 < mtiles; m0 += 2) {
-          if (m0 > 0) loadC(ci, m0, acc);
-          if (nlive) {
-            const bool m1ok = (m0 + 1 < mtiles);
-            const double* ta0 = Tn + (8 * m0 + fr) * LDT + fc;
-            const double* ta1 = Tn + (8 * (m1ok ? m0 + 1 : m0) + fr) * LDT + fc;
-            const double* rbp = buf + fc * LDR + 8 * warp + fr;
-            // three independent accumulator chains per tile (the MMA latency is long, the chain short)
-            double ax[2][2][2] = {{{0, 0}, {0, 0}}, {{0, 0}, {0, 0}}};
-#pragma unroll
-            for (int ks = 0; ks < PW / 12; ks++) {
-#pragma unroll
-              for (int g3 = 0; g3 < 3; g3++) {
-                const int kk = 4 * (ks + g3 * (PW / 12));
-                const double b0 = rbp[kk * LDR];
-                dmma884(g3 == 0 ? acc[0] : ax[g3 - 1][0], ta0[kk], b0);
-                dmma884(g3 == 0 ? acc[1] : ax[g3 - 1][1], ta1[kk], b0);
-              }
-            }
-#pragma unroll
-            for (int mi = 0; mi < 2; mi++)
-#pragma unroll
-              for (int q = 0; q < 2; q++) acc[mi][q] += ax[0][mi][q] + ax[1][mi][q];
-            if (!colK) {
-              if (m0 == 0) {
-                *reinterpret_cast<double2*>(dst + rowoff[0] + (size_t)ci * kGjTile) = make_double2(acc[0][0], acc[0][1]);
-                if (m1ok) *reinterpret_cast<double2*>(dst + rowoff[1] + (size_t)ci * kGjTile) = make_double2(acc[1][0], acc[1][1]);
+          for (int s = 0; s < 3; s++) {
+            if (!frag(s, r, cc)) continue;
+            if (last) {   // -(result) into the apply layout, mirrored; a diagonal tile contributes its lower half only
+              const int R = 48 * i + r, C = 48 * j + cc;
+              const double v0 = -acc[k][s][0], v1 = -acc[k][s][1];
+              if (i != j) {
+                *reinterpret_cast<double2*>(G.Ac + ac_index(ldm, R, C)) = make_double2(v0, v1);
+                G.Ac[ac_index(ldm, C, R)] = v0;
+                G.Ac[ac_index(ldm, C + 1, R)] = v1;
               } else {
-                *reinterpret_cast<double2*>(dst + ac_index(ldm, r0 + 8 * m0 + fr, col)) = make_double2(acc[0][0], acc[0][1]);
-                if (m1ok)
-                  *reinterpret_cast<double2*>(dst + ac_index(ldm, r0 + 8 * (m0 + 1) + fr, col)) = make_double2(acc[1][0], acc[1][1]);
+                if (r >= cc) { G.Ac[ac_index(ldm, R, C)] = v0; G.Ac[ac_index(ldm, C, R)] = v0; }
+                if (r >= cc + 1) { G.Ac[ac_index(ldm, R, C + 1)] = v1; G.Ac[ac_index(ldm, C + 1, R)] = v1; }
+              }
+            } else {
+              *reinterpret_cast<double2*>(G.Atri + (size_t)u * kAcTile + r * kAcLd + cc) = make_double2(acc[k][s][0], acc[k][s][1]);
+              if (i == d) {   // C_j = A_{j,K+1} = A_{K+1,j}^T
+                snapn[(size_t)j * kAcTile + cc * kAcLd + r] = acc[k][s][0];
+                snapn[(size_t)j * kAcTile + (cc + 1) * kAcLd + r] = acc[k][s][1];
+              } else if (j == d) {
+                *reinterpret_cast<double2*>(snapn + (size_t)i * kAcTile + r * kAcLd + cc) = make_double2(acc[k][s][0], acc[k][s][1]);
               }
             }
           }
         }
-        __syncthreads();   // the buffer is free for chunk ci + 2
+        __syncthreads();   // Cb[g % 3] is free for group g + 3
+        g++;
+        t = te;
       }
-      fence_proxy_async();  // the other CTAs' bulk copies read these rows in the next step
+      lap1(21);
+      fence_proxy_async();   // the snapshot and P_{K+1} are read by bulk copies in the next step
       team_barrier(c);
-      cur ^= 1;
+      lap1(22);
     }
-    return cur;
   }
 
   // -------- plane-major sweep: upart = segmented sums of Wt^T * (va + beta*vb)[pose] --------
@@ -2028,7 +2163,7 @@ struct Phase {
   // -------- three-level preconditioner, coarse part: level-3 residual from the level-2 partials; level-3 rows (distributed
   // over the team, or applied by every CTA when the level is small); level-2 nodes: one warp per node = its 6 rows of the
   // group's 96 x 96 inverse.  Publishes zc2 (and zc when level 3 is distributed); returns the partial of r.z it owns.
-  __device__ double coarse_three_level(double alpha, int acinv, const double* rc_old, bool first) {
+  __device__ double coarse_three_level(double alpha, const double* rc_old, bool first) {
     double* src = reinterpret_cast<double*>(g_smem + kSmRc);   // level-3 residual [6 nc]
     double* z3s = reinterpret_cast<double*>(g_smem + kSmZc);   // level-3 solution when it is applied locally (<= kL3Local rows)
     const int tid = threadIdx.x, lane = tid & 31;
@@ -2083,7 +2218,7 @@ struct Phase {
     }
     __syncthreads();
     lap(13);
-    const double* Ai = G.Ac[acinv];
+    const double* Ai = G.Ac;
     double dot = 0.0;
     if (c.l3_local) {
       for (int i = tid >> 5; i < ldm; i += kWarps) {
@@ -2150,7 +2285,7 @@ struct Phase {
 
   // -------- PCG: x += alpha p ; r -= alpha q ; z = M^-1 r (dense block + coarse) ; returns partial r.z ----
   // rc_old / rc_new: ping-pong buffers of per-block coarse restrictions of r
-  __device__ double precondition(double alpha, const double* pvec, int acinv, const double* rc_old, double* rc_new,
+  __device__ double precondition(double alpha, const double* pvec, const double* rc_old, double* rc_new,
                                  bool first) {
     double* sA = reinterpret_cast<double*>(g_smem + kSmA);   // r_new per slot
     double* src = reinterpret_cast<double*>(g_smem + kSmRc); // coarse residual, 6*nc
@@ -2159,7 +2294,7 @@ struct Phase {
     const int bpn = G.SP / kBlockPoses;  // blocks per coarse interval
     double dot = 0;
     if (G.levels == 3) {
-      dot = coarse_three_level(alpha, acinv, rc_old, first);
+      dot = coarse_three_level(alpha, rc_old, first);
     } else {
       // full coarse residual rc = sum_k rc_old[k] - alpha * sum_k qcpart[k]  (linear in r)
       __syncthreads();
@@ -2224,7 +2359,7 @@ struct Phase {
       }
       __syncthreads();
       lap(13);
-      const double* Ai = G.Ac[acinv];
+      const double* Ai = G.Ac;
       // coarse part, distributed over the team: one warp per row of A_c^-1.  z is never formed with its coarse
       // part; r.z = r.z_local + rc.zc (rc = P^T r), and the consumers of z add P*zc on the fly.
       {
@@ -2403,7 +2538,7 @@ struct Phase {
   //   C  coarse residual (linear update) ; A_c^-1 rows -> zc ; x, r updated in registers ; z = Binv r from smem ; r.z -> reduction
   // r, x, z, p, q of a row live in the registers of its thread for the whole solve.  Entry state (from the common prologue):
   // G.r, G.x, G.z (local part), G.zc, rcpart[rcb] ; exit: G.x.  Returns the iteration count.
-  __device__ int pcg_resident(double lambda, int acinv, int rcb, const double rz0, double rz, const double tol2, Timer& tmr) {
+  __device__ int pcg_resident(double lambda, int rcb, const double rz0, double rz, const double tol2, Timer& tmr) {
     const int ldm = 6 * G.nc;
     const int nown_max = (G.nblk + c.tsize - 1) / c.tsize;
     const ResLay L = res_layout(G.res_nt, G.res_ng, G.res_np, ldm, nown_max);
@@ -2530,7 +2665,7 @@ struct Phase {
     int wpe = kWarps;   // warps per listed plane (power of two)
     while (wpe > 1 && wpe * nh > kWarps) wpe >>= 1;
     double* hvp = reinterpret_cast<double*>(g_smem + L.hdr + 64 + kResHeavy * 16);   // [kResHeavy][kWarps][3] partial sums
-    const double* Ai = G.Ac[acinv];
+    const double* Ai = G.Ac;
     double* pvec = G.pv[0];
     int it = 0;
     double beta = 0.0;
