@@ -27,9 +27,6 @@
  *   There is NO CPU fallback: if no CUDA device / kernel image is usable, calls fail.
  *
  * Limits (a solve fails with a message instead of producing a wrong answer):
- *   - any 16 consecutive poses (in insertion order) may observe at most 256 distinct planes and produce at most 64
- *     (32-edge tile, pose) runs, i.e. about 96 plane observations per pose -- fixed shared-memory sizes of the fused
- *     pose phase; upstream iSAM has no such limit (the reference's own graphs: <= 10 planes per key-frame);
  *   - Slam::update() only with mod_batch = 1 (what PPS sets); relative-parameterised plane factors, anchor nodes,
  *     dog-leg and covariance recovery are not provided.
  */

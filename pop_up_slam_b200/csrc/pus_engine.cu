@@ -233,6 +233,7 @@ static int upload(Solver* s) {
     UP(blk_grp_ptr); UP(grp_plane); UP(grp_mem_ptr); UP(grp_mem); UP(blk_simple); UP(grp_info); UP(grp_info2); UP(at_plane); UP(at_lo); UP(at_hi); UP(at_ptr); UP(as_plane);
     d.n_atask = c.n_atask; d.n_asplit = c.n_asplit;
     d.res_nt = c.res_nt; d.res_ng = c.res_ng; d.res_np = c.res_np;
+    UP(blk_ovf); d.n_ovf_blk = c.n_ovf_blk;
     UP(ce_ptr); UP(ce_node); UP(ce_plane); UP(ce_lo); UP(ce_hi); UP(n2ce_ptr); UP(n2ce);
     UP(hv_plane); UP(lp_ptr); UP(lp_cea); UP(lp_ceb); UP(fp_ptr); UP(fp_f);
     d.n_hv = c.n_hv;
@@ -247,6 +248,7 @@ static int upload(Solver* s) {
     AL(PF, (size_t)c.Epf * 120, "PF"); AL(LP, (size_t)c.Elp * 12, "LP");
     AL(Hpp, N * 36, "Hpp"); AL(gp, N * 6, "gp"); AL(Hll, M * 9, "Hll"); AL(gl, M * 3, "gl"); AL(Hinv, M * 9, "Hinv");
     AL(ypart, 8, "ypart"); AL(upartb, (size_t)std::max(1, c.ngrp) * 3, "upartb"); AL(hpart, (size_t)std::max(1, c.n_atask) * 9, "hpart");
+    AL(ovf, c.n_ovf, "ovf");
     AL(Binv, (size_t)c.nblk * kPackedBlock, "Binv"); AL(Wc, (size_t)c.nce * 18, "Wc"); AL(Yc, (size_t)c.nce * 18, "Yc");
     AL(Ac, ac_doubles(6 * c.nc_pad), "Ac"); AL(Atri, ac_tri_doubles(6 * c.nc_pad), "Atri"); AL(Apan, ac_panel_doubles(6 * c.nc_pad), "Apan");
     AL(Wc2, (size_t)c.nce2 * 18, "Wc2"); AL(Yc2, (size_t)c.nce2 * 18, "Yc2"); AL(D2inv, (size_t)c.ng2 * kBlockDim * kBlockDim, "D2inv");
@@ -342,10 +344,11 @@ static void fill_params(Solver* s, LmParams& p, int mode, int restore_init, int 
 }
 
 // block-resident PCG loop: two levels with one hat node per pose block, every CTA's owned blocks in one round, and the per-CTA
-// layout (W tiles + packed preconditioner block + records per owned block) within the shared memory of an SM
+// layout (W tiles + packed preconditioner block + records per owned block) within the shared memory of an SM.  Graphs with a
+// pose block over the shared-memory limits of the general loop's pose phase (kMaxGrp / kMaxPart) run in the general loop.
 static bool resident_fits(const Compiled& cc, int team) {
   const int nown = (cc.nblk + team - 1) / team;
-  return cc.levels == 2 && cc.SP == kBlockPoses && nown >= 1 && nown <= kSlots && cc.res_ng <= 511 && cc.res_np <= 8191 &&
+  return cc.levels == 2 && cc.SP == kBlockPoses && cc.n_ovf_blk == 0 && nown >= 1 && nown <= kSlots && cc.res_ng <= 511 && cc.res_np <= 8191 &&
          res_layout(cc.res_nt, cc.res_ng, cc.res_np, 6 * cc.nc, nown).total <= (size_t)kSmemBytes;
 }
 
@@ -1364,6 +1367,8 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
   if (nm == "grp_mem") return ints(c.grp_mem);
   if (nm == "grp_mem_ptr") return ints(c.grp_mem_ptr);
   if (nm == "blk_grp_ptr") return ints(c.blk_grp_ptr);
+  if (nm == "blk_part_ptr") return ints(c.blk_part_ptr);
+  if (nm == "blk_ovf") return ints(c.blk_ovf);   // (empty: no pose block over the pose phase's shared-memory limits)
   if (nm == "dims") {
     double d[12] = {(double)c.N, (double)c.M, (double)c.Epl, (double)c.Epf, (double)c.Elp, (double)c.ntile, (double)c.nblk, (double)c.nc, (double)c.nce, (double)c.ngrp, (double)c.nslot, (double)c.ntile_pl};
     if (cap >= 12) std::memcpy(out, d, sizeof(d));

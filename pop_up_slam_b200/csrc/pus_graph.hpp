@@ -40,8 +40,8 @@ constexpr int kHeavyCoarse = 16;           // planes touching more coarse nodes 
 constexpr int kPivotNodes = 8;             // coarse nodes per pivot block of the blocked Gauss-Jordan inversion (48 scalars)
 constexpr int kTile = 32;                  // edges per warp tile
 constexpr int kWStride = 18 * kTile;       // doubles per W tile
-constexpr int kMaxGrp = 256;               // plane groups per 16-pose block held in shared memory
-constexpr int kMaxPart = 64;               // (tile, pose) partial sums per block held in shared memory
+constexpr int kMaxGrp = 256;               // plane groups per 16-pose block held in shared memory (more: global overflow scratch)
+constexpr int kMaxPart = 64;               // (tile, pose) partial sums per block held in shared memory (more: global overflow scratch)
 constexpr int kAsmChunk = 128;             // plane-major edge slots per Hll / gl assembly task (one warp)
 
 struct HNode {
@@ -203,6 +203,12 @@ struct Compiled {
   // res_* = largest tile / group / (tile, pose)-run count of any pose block (uniform shared-memory strides)
   std::vector<int> grp_info2;
   int res_nt = 0, res_ng = 0, res_np = 0;
+  // fused PCG pose phase, blocks over kMaxGrp plane groups or kMaxPart (tile, pose) runs: per block the offset (doubles) of its
+  // group vectors [ng][3] and run sums [npart][6] in the global overflow scratch, -1 for a block that keeps them in shared
+  // memory.  Empty when no block is over a limit (n_ovf = total doubles of the scratch, n_ovf_blk = blocks over a limit).
+  std::vector<int> blk_ovf;
+  size_t n_ovf = 0;
+  int n_ovf_blk = 0;
   // Hll / gl assembly tasks: the plane-major slots of every plane cut into chunks of kAsmChunk (a plane seen from thousands of
   // poses is gathered by many warps instead of one); at_* per task, at_ptr per plane, as_plane = planes with more than one task
   std::vector<int> at_plane, at_lo, at_hi, at_ptr, as_plane;
@@ -471,10 +477,14 @@ inline bool compile_graph(const Graph& g, Compiled& c, std::string& err) {
         if (c.pp_plane[es[i]] == c.pp_plane[es[i - 1]] && c.pp_pose[es[i]] == c.pp_pose[es[i - 1]]) simple = false;
       c.blk_simple[k] = simple ? 1 : 0;
     }
-    if (c.blk_grp_ptr[k + 1] - g0 > kMaxGrp || c.blk_part_ptr[k + 1] - c.blk_part_ptr[k] > kMaxPart) {
-      err = "pose block " + std::to_string(k) + " observes too many planes (limits: " + std::to_string(kMaxGrp) +
-            " distinct planes / " + std::to_string(kMaxPart) + " tile runs per 16 poses)";
-      return false;
+    {  // a block over either shared-memory limit of the fused pose phase keeps its vectors in the overflow scratch
+      const int ng = c.blk_grp_ptr[k + 1] - g0, npart = c.blk_part_ptr[k + 1] - c.blk_part_ptr[k];
+      if (ng > kMaxGrp || npart > kMaxPart) {
+        if (c.blk_ovf.empty()) c.blk_ovf.assign(c.nblk, -1);
+        c.blk_ovf[k] = (int)c.n_ovf;
+        c.n_ovf += (size_t)ng * 3 + (size_t)npart * 6;
+        c.n_ovf_blk++;
+      }
     }
   }
   c.grp_mem_ptr.push_back((int)c.grp_mem.size());

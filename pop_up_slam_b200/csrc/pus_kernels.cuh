@@ -89,6 +89,9 @@ struct DevGraph {
   const int *blk_grp_ptr, *grp_plane, *grp_mem_ptr, *grp_mem, *blk_simple, *grp_info;
   const int* grp_info2;         // block-resident PCG: {plane, first per-block partial, number of partials, own slot} per group
   int res_nt, res_ng, res_np;   // largest tile / group / (tile, pose)-run count of any pose block
+  int n_ovf_blk;                // pose blocks over kMaxGrp / kMaxPart (0: blk_ovf is a dummy)
+  const int* blk_ovf;           // per block: offset of its pose-phase vectors in `ovf`, -1 = shared memory
+  double* ovf;                  // overflow scratch of the fused pose phase (group vectors, then run sums, per block)
   double* upartb;               // [ngrp][3] per-(block, plane) partial sums of W^T p
   const int *at_plane, *at_lo, *at_hi, *at_ptr, *as_plane;   // Hll / gl assembly tasks (chunks of a plane's edges), split planes
   int n_atask, n_asplit;
@@ -1930,6 +1933,9 @@ struct Phase {
   //   2. y    = segmented sums over the block's pose-major tiles of W_e * v_{g(e)}        (shared memory)
   //   3. apply: q = (Hpp + lambda diag) p + (pose-pose blocks) p_other - y ; qc = P^T q ; returns partial p.q
   //      rhs  : b = -gp + y ; x = 0, r = b, p = z = q = 0 ; rcpart[0] = P^T b
+  // A block with more than kMaxGrp plane groups or kMaxPart (tile, pose) runs keeps v_g and the run sums in its own range of
+  // the global overflow scratch (offset blk_ovf[k], written and read only by the owning CTA, through L2) instead of shared
+  // memory; the sums and their order are the same.
   __device__ double pose_phase(bool rhs, const double* pvec, double lambda, double* qout, double* qc) {
     double* sA = reinterpret_cast<double*>(g_smem + kSmA);
     double* vg = reinterpret_cast<double*>(g_smem + kSmVg);
@@ -1941,15 +1947,16 @@ struct Phase {
     double dot = 0;
     const int nrounds = rounds();
     // plane-group record of this thread for the coming round (static data, read one round ahead)
-    int g0N = 0, ngN = 0;
+    int g0N = 0, ngN = 0, ovN = -1;
     int4 giN = make_int4(0, 0, 0, 0);
     auto next_groups = [&](int rd) {
       const int k = c.rank + c.tsize * (slot + kSlots * rd);
-      g0N = 0; ngN = 0;
+      g0N = 0; ngN = 0; ovN = -1;
       if (rd < nrounds && slot < kSlots && k < G.nblk) {
         g0N = G.blk_grp_ptr[k];
         ngN = G.blk_grp_ptr[k + 1] - g0N;
         if (u < ngN) giN = *reinterpret_cast<const int4*>(G.grp_info + (size_t)(g0N + u) * 4);
+        if (G.n_ovf_blk) ovN = G.blk_ovf[k];
       }
     };
     next_groups(0);
@@ -1961,6 +1968,8 @@ struct Phase {
       const bool on = live && (p < G.N);
       const int g0 = g0N, ng = ngN;
       const int4 gi0 = giN;
+      // over-limit block: v_g at ovf[ov + 3 g], the run sums at ovf[ov + 3 ng + 6 (part - part0)]  (uniform per slot)
+      const int ov = ovN;
       __syncthreads();
       next_groups(rd + 1);
       if (slot < kSlots) sA[slot * kBlockDim + u] = 0.0;
@@ -1984,9 +1993,10 @@ struct Phase {
         for (int g = u; g < ng; g += kBlockDim) {
           const int4 gi = (g == u) ? gi0 : *reinterpret_cast<const int4*>(G.grp_info + (size_t)(g0 + g) * 4);
           const int l = gi.x;
-          double* vo = vg + (slot * kMaxGrp + g) * 3;
+          double vv[3];
+          bool set = true;
           if (rhs) {
-            for (int b = 0; b < 3; b++) vo[b] = ldc(G.vl + (size_t)l * 3 + b);
+            for (int b = 0; b < 3; b++) vv[b] = ldc(G.vl + (size_t)l * 3 + b);
           } else {
             const int t0 = gi.y, n = gi.z;
             if (n <= 8) {
@@ -2003,9 +2013,18 @@ struct Phase {
 #pragma unroll
                 for (int b = 0; b < 3; b++) uu[b] += pr[t][b];
 #pragma unroll
-              for (int b = 0; b < 3; b++) vo[b] = Hi[b * 3] * uu[0] + Hi[b * 3 + 1] * uu[1] + Hi[b * 3 + 2] * uu[2];
+              for (int b = 0; b < 3; b++) vv[b] = Hi[b * 3] * uu[0] + Hi[b * 3 + 1] * uu[1] + Hi[b * 3 + 2] * uu[2];
             } else if (c.use_tma) {   // large graph: solve_heavy() already reduced this plane
-              for (int b = 0; b < 3; b++) vo[b] = ldc(G.vl + (size_t)l * 3 + b);
+              for (int b = 0; b < 3; b++) vv[b] = ldc(G.vl + (size_t)l * 3 + b);
+            } else {
+              set = false;            // heavy plane: summed by a warp below
+            }
+          }
+          if (set) {
+            if (ov < 0) {
+              for (int b = 0; b < 3; b++) vg[(slot * kMaxGrp + g) * 3 + b] = vv[b];
+            } else {
+              for (int b = 0; b < 3; b++) __stcg(G.ovf + ov + g * 3 + b, vv[b]);
             }
           }
         }
@@ -2027,10 +2046,12 @@ struct Phase {
                 for (int b = 0; b < 3; b++) uu[b] += pr[t][b];
             }
             for (int b = 0; b < 3; b++) uu[b] = warp_sum(uu[b]);
-            if (lane < 3)
-              vg[(slot * kMaxGrp + g) * 3 + lane] = ldc(G.Hinv + (size_t)l * 9 + lane * 3) * uu[0] +
-                                                    ldc(G.Hinv + (size_t)l * 9 + lane * 3 + 1) * uu[1] +
-                                                    ldc(G.Hinv + (size_t)l * 9 + lane * 3 + 2) * uu[2];
+            if (lane < 3) {
+              const double v = ldc(G.Hinv + (size_t)l * 9 + lane * 3) * uu[0] + ldc(G.Hinv + (size_t)l * 9 + lane * 3 + 1) * uu[1] +
+                               ldc(G.Hinv + (size_t)l * 9 + lane * 3 + 2) * uu[2];
+              if (ov < 0) vg[(slot * kMaxGrp + g) * 3 + lane] = v;
+              else __stcg(G.ovf + ov + g * 3 + lane, v);
+            }
           }
         }
       }
@@ -2051,8 +2072,13 @@ struct Phase {
           double y[6] = {0, 0, 0, 0, 0, 0};
           double v0 = 0, v1 = 0, v2 = 0;
           if (key >= 0) {
-            const double* v = vg + (slot * kMaxGrp + gos) * 3;
-            v0 = v[0]; v1 = v[1]; v2 = v[2];
+            if (ov < 0) {
+              const double* v = vg + (slot * kMaxGrp + gos) * 3;
+              v0 = v[0]; v1 = v[1]; v2 = v[2];
+            } else {
+              const double* v = G.ovf + ov + gos * 3;
+              v0 = __ldcg(v); v1 = __ldcg(v + 1); v2 = __ldcg(v + 2);
+            }
           }
           if (c.use_tma) {
             mbar_wait(tbar + st, (c.tma_par >> st) & 1u);
@@ -2070,8 +2096,13 @@ struct Phase {
           seg_suffix_sum<6>(key, y);
           int pk = __shfl_up_sync(0xffffffffu, key, 1);
           if (key >= 0 && (lane == 0 || pk != key)) {
-            double* o = yp + (slot * kMaxPart + (part - part0)) * 6;
-            for (int a = 0; a < 6; a++) o[a] = y[a];
+            if (ov < 0) {
+              double* o = yp + (slot * kMaxPart + (part - part0)) * 6;
+              for (int a = 0; a < 6; a++) o[a] = y[a];
+            } else {
+              double* o = G.ovf + ov + ng * 3 + (part - part0) * 6;
+              for (int a = 0; a < 6; a++) __stcg(o + a, y[a]);
+            }
           }
           __syncwarp();  // stage consumed by every lane before it is refilled
         }
@@ -2081,7 +2112,12 @@ struct Phase {
       if (on) {
         const int part0 = G.blk_part_ptr[k];
         double ysum = 0;
-        for (int t = G.ypart_ptr[p]; t < G.ypart_ptr[p + 1]; t++) ysum += yp[(slot * kMaxPart + (t - part0)) * 6 + row];
+        if (ov < 0) {
+          for (int t = G.ypart_ptr[p]; t < G.ypart_ptr[p + 1]; t++) ysum += yp[(slot * kMaxPart + (t - part0)) * 6 + row];
+        } else {
+          const double* ys = G.ovf + ov + ng * 3 + row;
+          for (int t = G.ypart_ptr[p]; t < G.ypart_ptr[p + 1]; t++) ysum += __ldcg(ys + (t - part0) * 6);
+        }
         const size_t o = (size_t)p * 6 + row;
         if (rhs) {
           double v = -ldc(G.gp + o) + ysum;

@@ -291,6 +291,58 @@ def make_corridor(seed=0, n_poses=5000, n_planes=500, obs_per_pose=10, step=0.1,
                    outlier_frac, outlier_mag, robust_kind, robust_b, max_iterations, init_mode)
 
 
+def make_dense(seed=0, n_poses=48, walls=40, advance=20, dense_blocks=None, sparse_walls=6, sparse_advance=3,
+               sigma_mode="consistent", plane_noise=0.01, odo_noise=(0.01, 0.005), max_iterations=10, name="dense"):
+    """Dense plane observations, as front ends give them that extract 20-40 planes per RGB-D frame, that add a new landmark
+    for every observation (no data association) or that take key-frames at a high rate while the camera turns on the spot.
+    Poses on the 2 m circle of make_room; each observes the ground plane plus `walls` consecutive vertical walls of a running
+    sequence that advances by `advance` walls per pose, so every wall is seen from about walls / advance poses.  With
+    `dense_blocks` (16-pose block numbers) only those blocks observe that densely; the other poses see `sparse_walls` walls
+    advancing by `sparse_advance`.
+    A dense 16-pose block observes about 15 advance + walls + 1 distinct planes in about 16 (walls + 1) / 32 + 16 (tile, pose)
+    runs: walls=40, advance=20 passes 256 distinct planes per block (with about 37 runs); walls=110, advance=6 passes 64 runs
+    (with about 200 distinct planes)."""
+    rng = np.random.default_rng(seed)
+    T = []
+    for i in range(n_poses):
+        ang = 2 * np.pi * i / n_poses
+        R = geo.euler_to_R(ang + np.pi, 0.02 * np.sin(3 * ang), 0.02 * np.cos(2 * ang)) @ R_BASE
+        Ti = np.eye(4)
+        Ti[:3, :3] = R
+        Ti[:3, 3] = [2 * np.cos(ang), 2 * np.sin(ang), 1.0]
+        T.append(Ti)
+    dense = [dense_blocks is None or (i // 16) in dense_blocks for i in range(n_poses)]
+    start, s = [], 0
+    for i in range(n_poses):
+        start.append(s)
+        s += advance if dense[i] else sparse_advance
+    n_walls = max(start[i] + (walls if dense[i] else sparse_walls) for i in range(n_poses))
+    planes = [np.array([0.0, 0.0, -1.0, 0.0])]
+    anchors = [np.zeros(3)]
+    for _ in range(n_walls):
+        phi = rng.uniform(0, 2 * np.pi)
+        rho = rng.uniform(3.0, 6.0)
+        planes.append(geo.plane_normalize([np.cos(phi), np.sin(phi), 0.0, -rho]))
+        anchors.append(np.array([rho * np.cos(phi), rho * np.sin(phi), 0.0]))
+    planes = np.array(planes)
+    obs_pose, obs_plane, dist = [], [], []
+    for i in range(n_poses):
+        for k in [0] + list(range(1 + start[i], 1 + start[i] + (walls if dense[i] else sparse_walls))):
+            obs_pose.append(i)
+            obs_plane.append(k)
+            dist.append(T[i][2, 3] if k == 0 else np.linalg.norm(anchors[k][:2] - T[i][:2, 3]))
+    return _finish(name, seed, T, planes, np.array(obs_pose), np.array(obs_plane), np.array(dist), rng, sigma_mode,
+                   plane_noise, odo_noise, 0.0, (0.2, 1.0), 0, 1.0, max_iterations)
+
+
+# dense-plane graphs over each per-block limit of the fused PCG pose phase (DESIGN.md section 6), and a mix
+DENSE_CASES = {
+    "planes": dict(n_poses=48, walls=40, advance=20),                          # > 256 distinct planes in every block
+    "runs": dict(n_poses=48, walls=110, advance=6),                            # > 64 (tile, pose) runs, < 256 planes
+    "mixed": dict(n_poses=96, walls=40, advance=20, dense_blocks=(1, 4)),      # two of six blocks over a limit
+}
+
+
 def make_config(config, seed=0, **kw):
     """BASELINE.json configs by number (SURVEY.md 8, table of sizes)."""
     if config == 1:   # 10 poses, 20 planes, 100 edges

@@ -4,15 +4,28 @@
 //   g++ -O2 -std=c++17 -DHDR='"<old checkout>/pop_up_slam_b200/csrc/pus_graph.hpp"' -x c++ tools/compile_graph_hash.cpp -o /tmp/h_old
 //   g++ -O2 -std=c++17 -DHDR='"pop_up_slam_b200/csrc/pus_graph.hpp"'               -x c++ tools/compile_graph_hash.cpp -o /tmp/h_new
 //   for a in "40 6 1" "300 8 2" "2000 12 3" "20000 20 5"; do /tmp/h_old $a; /tmp/h_new $a; done      (args: poses, edges/pose, seed [, force_levels])
+// With `--file <graph.txt> [force_levels]` it reads the graph instead, one Graph call per line in insertion order (node ids
+// are the running node count), so that generated or dataset graphs can be hashed too:
+//   pose - | pose x y z qw qx qy qz          plane - | plane a b c d
+//   prior <pose> m[6] sinf[21]   odo <pose> <pose> m[6] sinf[21]   pp <pose> <plane> m[4] sinf[6]   lprior <plane> m[4] sinf[6]
 #include <chrono>
 #include <cstdio>
 #include <cstdint>
+#include <cstring>
+#include <fstream>
 #include <random>
+#include <sstream>
 #include HDR
 using namespace pus;
 static uint64_t H = 1469598103934665603ull;
 template <typename T> void hv(const std::vector<T>& v) { const unsigned char* p = (const unsigned char*)v.data(); for (size_t i = 0; i < v.size() * sizeof(T); i++) { H ^= p[i]; H *= 1099511628211ull; } H ^= v.size(); H *= 1099511628211ull; }
 void hi(int x) { H ^= (uint64_t)(uint32_t)x; H *= 1099511628211ull; }
+// the overflow scratch layout of over-limit pose blocks: hashed when the header has it and a block uses it, so the hash of
+// a graph within the limits is the same as from a header that predates it
+template <typename C> auto hash_overflow(const C& c, int) -> decltype(c.blk_ovf, void()) {
+  if (!c.blk_ovf.empty()) { hv(c.blk_ovf); hi((int)c.n_ovf); hi(c.n_ovf_blk); }
+}
+template <typename C> void hash_overflow(const C&, long) {}
 static uint64_t image_hash(const Compiled& c) {
   H = 1469598103934665603ull;
   for (int x : {c.N, c.M, c.Epl, c.Epf, c.Elp, c.SP, c.nc_pad, c.ntile, c.nslot, c.nblk, c.nc, c.n_upart, c.n_ypart, c.nce, c.ngrp, c.n_hv, c.n_heavy, c.n_huge, c.n_f2, c.ntile_pl}) hi(x);
@@ -29,9 +42,47 @@ static uint64_t image_hash(const Compiled& c) {
   for (int x : {c.res_nt, c.res_ng, c.res_np, c.n_atask, c.n_asplit, c.levels, c.nc2, c.nce2, c.ng2}) hi(x);
   hv(c.grp_info2); hv(c.at_plane); hv(c.at_lo); hv(c.at_hi); hv(c.at_ptr); hv(c.as_plane);
   hv(c.ce2_ptr); hv(c.ce2_node); hv(c.ce2_plane); hv(c.ce2_lo); hv(c.ce2_hi); hv(c.g2_ptr); hv(c.g2_ce);
+  hash_overflow(c, 0);
   return H;
 }
+static bool read_graph(const char* path, Graph& g) {
+  std::ifstream in(path);
+  std::string line, op;
+  auto vals = [](std::istringstream& ss, double* v, int n) { for (int i = 0; i < n; i++) if (!(ss >> v[i])) return false; return true; };
+  while (std::getline(in, line)) {
+    std::istringstream ss(line);
+    if (!(ss >> op)) continue;
+    double v[27];
+    int a = -1, b = -1, r = 0;
+    if (op == "pose" || op == "plane") {
+      const int n = op == "pose" ? 7 : 4;
+      std::string first;
+      if (!(ss >> first)) return false;
+      const bool init = first != "-";
+      if (init) { v[0] = std::stod(first); if (!vals(ss, v + 1, n - 1)) return false; }
+      r = g.add_node(op == "pose" ? NODE_POSE : NODE_PLANE, init ? v : nullptr);
+    } else if (op == "prior") { if (!(ss >> a) || !vals(ss, v, 27)) return false; r = g.add_pose_prior(a, v, v + 6); }
+    else if (op == "odo") { if (!(ss >> a >> b) || !vals(ss, v, 27)) return false; r = g.add_odometry(a, b, v, v + 6); }
+    else if (op == "pp") { if (!(ss >> a >> b) || !vals(ss, v, 10)) return false; r = g.add_pose_plane(a, b, v, v + 4); }
+    else if (op == "lprior") { if (!(ss >> a) || !vals(ss, v, 10)) return false; r = g.add_plane_prior(a, v, v + 4); }
+    else return false;
+    if (r < 0) return false;
+  }
+  return true;
+}
+
 int main(int argc, char** argv) {
+  if (argc > 2 && !strcmp(argv[1], "--file")) {
+    Graph g;
+    if (!read_graph(argv[2], g)) { printf("ok=0 cannot read %s: %s\n", argv[2], g.err.c_str()); return 1; }
+    if (argc > 3) g.force_levels = atoi(argv[3]);
+    Compiled c; std::string err;
+    bool ok = compile_graph(g, c, err);
+    const uint64_t h1 = ok ? image_hash(c) : 0;
+    ok = compile_graph(g, c, err) && ok && image_hash(c) == h1;
+    printf("file=%s ok=%d E=%d hash=%016llx %s\n", argv[2], ok, c.Epl, (unsigned long long)H, err.c_str());
+    return ok ? 0 : 1;
+  }
   int N = atoi(argv[1]), per = atoi(argv[2]), seed = atoi(argv[3]);
   int M = std::max(3, N / 10);
   Graph g; std::mt19937 rng(seed);
