@@ -69,7 +69,7 @@ typedef struct pus_solver_options {
                         *   [2]      bit 0: sub-phase timers in pus_stats.phase_ms[13..23]; bit 1: always stage W / Wt
                         *            tiles by bulk async copy (the large-graph data path); bit 2: never; bit 3: force the
                         *            three-level preconditioner (default: graphs > 5120 poses); bit 4: force two levels;
-                        *            bit 5: no block-resident PCG loop; bit 6 / 7: other timer sets; bits 8-15: the CTA of the
+                        *            bit 5: no block-resident PCG loop; bit 6: another timer set; bits 8-15: the CTA of the
                         *            team that keeps the timers; bit 16: never run a team as a thread-block cluster (global-
                         *            memory barrier only; the environment variable PUS_CLUSTER=0 does the same process-wide)
                         *   [3] > 0  lazy-refresh threshold in percent of the post-build iteration count (default 130, three

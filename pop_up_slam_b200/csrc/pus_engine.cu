@@ -336,7 +336,7 @@ static void fill_params(Solver* s, LmParams& p, int mode, int restore_init, int 
   // large graphs is dearer per build and wants 200 % (tools/refresh_sweep.py re-measures both)
   p.refresh_pct = s->opt.reserved[3] > 0 ? s->opt.reserved[3] : (s->c.levels == 3 ? 200 : 130);
   p.refresh_add = 8;
-  p.fine_timers = (s->opt.reserved[2] & 128) ? 3 : (s->opt.reserved[2] & 64) ? 2 : ((s->opt.reserved[2] & 1) ? 1 : 0);   // bit 6: sub-phases of linearize instead     // reserved[2] bit 0: sub-phase timers inside the PCG phases
+  p.fine_timers = (s->opt.reserved[2] & 64) ? 2 : ((s->opt.reserved[2] & 1) ? 1 : 0);   // bit 6: sub-phases of linearize instead     // reserved[2] bit 0: sub-phase timers inside the PCG phases
   p.timer_rank = (s->opt.reserved[2] >> 8) & 0xff;   // bits 8-15: the CTA that keeps the phase timers
   p.tma_mode = (s->opt.reserved[2] & 2) ? 1 : ((s->opt.reserved[2] & 4) ? 2 : 0);  // bit 1: always stage tiles by TMA, bit 2: never
   p.warm_start = s->opt.reserved[1] == 1 ? 0 : 1;      // reserved[1] = 1: never warm-start PCG after a rejected step  // reserved[0] = 1: rebuild the preconditioner every solve

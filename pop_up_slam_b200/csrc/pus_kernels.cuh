@@ -619,9 +619,9 @@ __device__ __forceinline__ double team_reduce_flag(Ctx& c, double v) {
 }
 
 // segmented (by sorted key) suffix sums inside a warp: afterwards the first lane of every run of equal
-// keys holds the run's total, accumulated in a fixed order
+// keys holds the run's total, accumulated in a fixed order.  Returns true on that lane when the key is valid (>= 0).
 template <int K>
-__device__ __forceinline__ void seg_suffix_sum(int key, double* v) {
+__device__ __forceinline__ bool seg_suffix_sum(int key, double* v) {
   const int lane = threadIdx.x & 31;
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) {
@@ -631,6 +631,187 @@ __device__ __forceinline__ void seg_suffix_sum(int key, double* v) {
     for (int k = 0; k < K; k++) {
       double o = __shfl_down_sync(0xffffffffu, v[k], d);
       if (take) v[k] += o;
+    }
+  }
+  const int pk = __shfl_up_sync(0xffffffffu, key, 1);
+  return key >= 0 && (lane == 0 || pk != key);
+}
+
+// ---- arithmetic shared by the general PCG loop (schur_solve) and the block-resident one (pcg_resident) ----
+// Each helper fixes one summation order and expression shape for all its callers.  Loads stay with the
+// callers wherever they are issued early for latency; the loader argument (LdS: shared memory or registers, LdL2:
+// ld.global.cg) only selects the load instruction of the operands the helper reads itself.
+struct LdS {
+  __device__ __forceinline__ double operator()(const double* p) const { return *p; }
+};
+struct LdL2 {
+  __device__ __forceinline__ double operator()(const double* p) const { return __ldcg(p); }
+};
+
+// h[0..2] . u[0..2]: one row of a 3x3 product (Hll^-1 u)
+template <class Ld = LdS>
+__device__ __forceinline__ double dot3(const double* h, const double* u) {
+  const Ld ld;
+  return ld(h) * u[0] + ld(h + 1) * u[1] + ld(h + 2) * u[2];
+}
+// v = H u, H a row-major 3x3 already in registers
+__device__ __forceinline__ void mat3_vec(const double* H, const double* u, double* v) {
+#pragma unroll
+  for (int b = 0; b < 3; b++) v[b] = dot3(H + b * 3, u);
+}
+
+// sum of the 3-vector partials part[a0 .. a1) by one warp: 8 strided partials per lane in flight, then a fixed-order tree;
+// every lane gets the sums
+__device__ __forceinline__ void warp_sum_partials(const double* part, int a0, int a1, int lane, double* uu) {
+  uu[0] = 0; uu[1] = 0; uu[2] = 0;
+  for (int tb = a0 + lane; tb < a1; tb += 256) {
+    double pr[8][3];
+#pragma unroll
+    for (int t = 0; t < 8; t++)
+#pragma unroll
+      for (int b = 0; b < 3; b++) pr[t][b] = (tb + 32 * t < a1) ? ldc(part + (size_t)(tb + 32 * t) * 3 + b) : 0.0;
+#pragma unroll
+    for (int t = 0; t < 8; t++)
+#pragma unroll
+      for (int b = 0; b < 3; b++) uu[b] += pr[t][b];
+  }
+#pragma unroll
+  for (int b = 0; b < 3; b++) uu[b] = warp_sum(uu[b]);
+}
+
+// v = Hll^-1 of plane l times the sum of its n <= 8 partials part[t0 .. t0 + n), by one thread (all 33 loads in one batch)
+__device__ __forceinline__ void plane_vec_small(const double* part, int t0, int n, int l, double* v) {
+  double pr[8][3], Hi[9];
+#pragma unroll
+  for (int t = 0; t < 8; t++)
+#pragma unroll
+    for (int b = 0; b < 3; b++) pr[t][b] = (t < n) ? ldc(part + (size_t)(t0 + t) * 3 + b) : 0.0;
+#pragma unroll
+  for (int t = 0; t < 9; t++) Hi[t] = ldc(G.Hinv + (size_t)l * 9 + t);
+  double uu[3] = {0, 0, 0};
+#pragma unroll
+  for (int t = 0; t < 8; t++)
+#pragma unroll
+    for (int b = 0; b < 3; b++) uu[b] += pr[t][b];
+  mat3_vec(Hi, uu, v);
+}
+
+// W_e^T x (6 -> 3) of one lane's edge in an [18][32] warp tile (w = tile + lane), accumulated into u
+template <class Ld>
+__device__ __forceinline__ void tile_wt_x(const double* w, const double* x, double* u) {
+  const Ld ld;
+#pragma unroll
+  for (int a = 0; a < 6; a++) {
+    const double xa = x[a];
+#pragma unroll
+    for (int b = 0; b < 3; b++) u[b] += ld(w + (a * 3 + b) * 32) * xa;
+  }
+}
+// y = W_e v (3 -> 6) of one lane's edge in an [18][32] warp tile
+template <class Ld>
+__device__ __forceinline__ void tile_w_v(const double* w, double v0, double v1, double v2, double* y) {
+  const Ld ld;
+#pragma unroll
+  for (int a = 0; a < 6; a++) y[a] = ld(w + (a * 3) * 32) * v0 + ld(w + (a * 3 + 1) * 32) * v1 + ld(w + (a * 3 + 2) * 32) * v2;
+}
+
+// coefficients of row `row` of the pose-pose blocks towards the first two neighbours of a pose (the odometry chain), from its
+// pnbr record {f0 * 2 + side0, neighbour0, f1 * 2 + side1, neighbour1} (f < 0: none) into a[n * 6 + col]; returns the number of
+// such neighbours
+__device__ __forceinline__ int nbr_coeffs(int4 nb, int row, double* a) {
+  const int nf = (nb.x >= 0) + (nb.z >= 0);
+  const double* Ab[2] = {G.PF + (size_t)(max(nb.x, 0) >> 1) * 120 + 72, G.PF + (size_t)(max(nb.z, 0) >> 1) * 120 + 72};
+  const int sd[2] = {nb.x & 1, nb.z & 1};
+#pragma unroll
+  for (int n2 = 0; n2 < 2; n2++)
+#pragma unroll
+    for (int cc = 0; cc < 6; cc++) a[n2 * 6 + cc] = (n2 < nf) ? (sd[n2] ? ldc(Ab[n2] + cc * 6 + row) : ldc(Ab[n2] + row * 6 + cc)) : 0.0;
+  return nf;
+}
+// v + row `row` of the further pose-pose blocks (loop closures, incidences pinc[k0 .. k1)) times pvec
+__device__ __forceinline__ double pose_pose_tail(int k0, int k1, int row, const double* pvec, double v) {
+  for (int kk = k0; kk < k1; kk++) {
+    const int inc = G.pinc[kk], f = inc >> 1, side = inc & 1;
+    const int j = G.pf_j[f];
+    if (j < 0) continue;
+    const int oth = side ? G.pf_i[f] : j;
+    const double* A12 = G.PF + (size_t)f * 120 + 72;
+    for (int cc = 0; cc < 6; cc++) {
+      const double a = side ? ldc(A12 + cc * 6 + row) : ldc(A12 + row * 6 + cc);
+      v += a * ldc(pvec + (size_t)oth * 6 + cc);
+    }
+  }
+  return v;
+}
+
+// row i of a packed upper triangle of a symmetric kBlockDim block: packed_row(B, i)[j] = (i, j) for j >= i
+template <typename T>
+__device__ __forceinline__ T* packed_row(T* B, int i) { return B + i * kBlockDim - (i * (i - 1)) / 2 - i; }
+// row u of the packed symmetric block B times rv, one thread per row: rows j < u give (j, u), rows j >= u give (u, j)
+template <class Ld>
+__device__ __forceinline__ double packed_row_dot(const double* B, int u, const double* rv) {
+  const Ld ld;
+  double acc = 0;
+  for (int j = 0; j < u; j++) acc += ld(packed_row(B, j) + u) * rv[j];
+  const double* bu = packed_row(B, u);
+  for (int j = u; j < kBlockDim; j++) acc += ld(bu + j) * rv[j];
+  return acc;
+}
+
+// row of A_c^-1 (arow = its first element in the tiled layout) times the coarse residual src[0 .. ldm), one warp per row:
+// 128-bit loads, a lane owns column pairs (2 lane + 64 t), so a 1 884-wide row is two batches of 16 loads in flight (pairs never
+// straddle a 128-column tile: tile rows are 16-byte aligned, stride 132).  Returns the row sum on every lane.
+__device__ __forceinline__ double coarse_row_dot(const double* arow, const double* src, int ldm, int lane) {
+  double acc = 0;
+  int j = 2 * lane;
+  for (; j + 64 * 15 < ldm; j += 64 * 16) {
+    double2 av[16];
+#pragma unroll
+    for (int t = 0; t < 16; t++) {
+      const int jj = j + 64 * t;
+      av[t] = __ldcg(reinterpret_cast<const double2*>(arow + (size_t)(jj / kGjChunk) * kGjTile + (jj % kGjChunk)));
+    }
+#pragma unroll
+    for (int t = 0; t < 16; t++) acc += av[t].x * src[j + 64 * t] + av[t].y * src[j + 64 * t + 1];
+  }
+  {
+    double2 av[16];
+#pragma unroll
+    for (int t = 0; t < 16; t++) {
+      const int jj = j + 64 * t;
+      av[t] = (jj < ldm) ? __ldcg(reinterpret_cast<const double2*>(arow + (size_t)(jj / kGjChunk) * kGjTile + (jj % kGjChunk))) : make_double2(0.0, 0.0);
+    }
+#pragma unroll
+    for (int t = 0; t < 16; t++) {
+      const int jj = j + 64 * t;
+      if (jj < ldm) acc += av[t].x * src[jj] + av[t].y * src[jj + 1];   // (ldm = 6 nc is even)
+    }
+  }
+  return warp_sum(acc);
+}
+
+// coarse residual src[i] = rc_old + rc_old' - alpha (qcpart + qcpart') when every coarse interval is one pose block (graphs up
+// to 5120 poses): block `node` feeds the node through its slot 0, block `node-1` through slot 1.  Four outputs per thread, so
+// that all 16 loads are in flight together.  (first: no q yet, rc_old only.)
+__device__ __forceinline__ void coarse_residual(const double* rc_old, double alpha, bool first, double* src) {
+  const int ldm = 6 * G.nc;
+  for (int i0 = threadIdx.x; i0 < ldm; i0 += 4 * kThreads) {
+    double va[4][2], vq[4][2];
+#pragma unroll
+    for (int m = 0; m < 4; m++) {
+      const int i = i0 + m * kThreads, node = i / 6, row = i - node * 6;
+#pragma unroll
+      for (int side = 0; side < 2; side++) {
+        const int k = node - side;
+        const bool ok = (i < ldm) && (k >= 0) && (k < G.nblk);
+        va[m][side] = ok ? ldc(rc_old + (size_t)k * 12 + side * 6 + row) : 0.0;
+        vq[m][side] = (ok && !first) ? ldc(G.qcpart + (size_t)k * 12 + side * 6 + row) : 0.0;
+      }
+    }
+#pragma unroll
+    for (int m = 0; m < 4; m++) {
+      const int i = i0 + m * kThreads;
+      if (i < ldm) src[i] = (0.0 + (va[m][0] - alpha * vq[m][0])) + (va[m][1] - alpha * vq[m][1]);
     }
   }
 }
@@ -1254,7 +1435,7 @@ struct Phase {
       // inversion above, so stores of rows 0-10 were dropped at random.)
       double* out = G.Binv + (size_t)k * kPackedBlock;
       for (int i = tid >> 5; i < kBlockDim; i += kWarps) {
-        double* orow = out + i * kBlockDim - (i * (i - 1)) / 2 - i;   // orow[j] = packed (i, j)
+        double* orow = packed_row(out, i);
         for (int j = i + (tid & 31); j < kBlockDim; j += 32) orow[j] = inv[i * LD + j];
       }
     }
@@ -1762,16 +1943,8 @@ struct Phase {
         double u[3] = {0, 0, 0};
         mbar_wait(bar + st, (c.tma_par >> st) & 1u);
         c.tma_par ^= (1u << st);
-        if (keyC >= 0) {
-          const double* wt = buf + st * kWStride + lane;
-#pragma unroll
-          for (int a = 0; a < 6; a++)
-#pragma unroll
-            for (int b = 0; b < 3; b++) u[b] += wt[(a * 3 + b) * 32] * x[a];
-        }
-        seg_suffix_sum<3>(keyC, u);
-        const int pk = __shfl_up_sync(0xffffffffu, keyC, 1);
-        if (keyC >= 0 && (lane == 0 || pk != keyC)) {
+        if (keyC >= 0) tile_wt_x<LdS>(buf + st * kWStride + lane, x, u);
+        if (seg_suffix_sum<3>(keyC, u)) {
           double* o = G.upart + (size_t)G.pl_part[tile * 32 + lane] * 3;
           put(c, o, u[0]); put(c, o + 1, u[1]); put(c, o + 2, u[2]);
         }
@@ -1802,15 +1975,9 @@ struct Phase {
             for (int a = 0; a < 6; a++) x[a] += coarse_z(p, a);
           }
         }
-        const double* wt = G.Wt + (size_t)tile * kWStride + lane;
-#pragma unroll
-        for (int a = 0; a < 6; a++)
-#pragma unroll
-          for (int b = 0; b < 3; b++) u[b] += ldc(wt + (a * 3 + b) * 32) * x[a];
+        tile_wt_x<LdL2>(G.Wt + (size_t)tile * kWStride + lane, x, u);
       }
-      seg_suffix_sum<3>(key, u);
-      int pk = __shfl_up_sync(0xffffffffu, key, 1);
-      if (key >= 0 && (lane == 0 || pk != key)) {
+      if (seg_suffix_sum<3>(key, u)) {
         double* o = G.upart + (size_t)G.pl_part[s] * 3;
         put(c, o, u[0]); put(c, o + 1, u[1]); put(c, o + 2, u[2]);
       }
@@ -1832,7 +1999,7 @@ struct Phase {
         if (mode == 1) for (int b = 0; b < 3; b++) u[b] = -ldc(G.gl + (size_t)l * 3 + b) - u[b];
         double* o = (mode == 0 ? G.vl : G.dl) + (size_t)l * 3;
         for (int t = 0; t < 3; t++) {
-          double v = Hi[t * 3] * u[0] + Hi[t * 3 + 1] * u[1] + Hi[t * 3 + 2] * u[2];
+          double v = dot3(Hi + t * 3, u);
           put(c, o + t, v);
           nrm += v * v;
         }
@@ -1871,31 +2038,16 @@ struct Phase {
         for (int w = 0; w < kWarps; w++)
           for (int b = 0; b < 3; b++) tot[b] += s[w * 4 + b];
         const int o = threadIdx.x;
-        put(c, &G.vl[(size_t)l * 3 + o], ldc(G.Hinv + (size_t)l * 9 + o * 3) * tot[0] + ldc(G.Hinv + (size_t)l * 9 + o * 3 + 1) * tot[1] +
-                                             ldc(G.Hinv + (size_t)l * 9 + o * 3 + 2) * tot[2]);
+        put(c, &G.vl[(size_t)l * 3 + o], dot3<LdL2>(G.Hinv + (size_t)l * 9 + o * 3, tot));
       }
       __syncthreads();
     }
     for (int h = warp_team(); h < G.n_heavy; h += nwarp_team()) {
       const int l = G.heavy[h];
       if (l < 0) continue;
-      const int t0 = G.upart_ptr[l], n = G.upart_ptr[l + 1] - t0;
-      double uu[3] = {0, 0, 0};
-      for (int tb = t0 + lane; tb < t0 + n; tb += 256) {   // 8 strided partials per lane in flight
-        double pr[8][3];
-#pragma unroll
-        for (int t = 0; t < 8; t++)
-#pragma unroll
-          for (int b = 0; b < 3; b++) pr[t][b] = (tb + 32 * t < t0 + n) ? ldc(G.upart + (size_t)(tb + 32 * t) * 3 + b) : 0.0;
-#pragma unroll
-        for (int t = 0; t < 8; t++)
-#pragma unroll
-          for (int b = 0; b < 3; b++) uu[b] += pr[t][b];
-      }
-      for (int b = 0; b < 3; b++) uu[b] = warp_sum(uu[b]);
-      if (lane < 3)
-        put(c, &G.vl[(size_t)l * 3 + lane], ldc(G.Hinv + (size_t)l * 9 + lane * 3) * uu[0] + ldc(G.Hinv + (size_t)l * 9 + lane * 3 + 1) * uu[1] +
-                                                ldc(G.Hinv + (size_t)l * 9 + lane * 3 + 2) * uu[2]);
+      double uu[3];
+      warp_sum_partials(G.upart, G.upart_ptr[l], G.upart_ptr[l + 1], lane, uu);
+      if (lane < 3) put(c, &G.vl[(size_t)l * 3 + lane], dot3<LdL2>(G.Hinv + (size_t)l * 9 + lane * 3, uu));
     }
   }
 
@@ -1998,22 +2150,8 @@ struct Phase {
           if (rhs) {
             for (int b = 0; b < 3; b++) vv[b] = ldc(G.vl + (size_t)l * 3 + b);
           } else {
-            const int t0 = gi.y, n = gi.z;
-            if (n <= 8) {
-              double pr[8][3], Hi[9];
-#pragma unroll
-              for (int t = 0; t < 8; t++)
-#pragma unroll
-                for (int b = 0; b < 3; b++) pr[t][b] = (t < n) ? ldc(G.upart + (size_t)(t0 + t) * 3 + b) : 0.0;
-#pragma unroll
-              for (int t = 0; t < 9; t++) Hi[t] = ldc(G.Hinv + (size_t)l * 9 + t);
-              double uu[3] = {0, 0, 0};
-#pragma unroll
-              for (int t = 0; t < 8; t++)
-#pragma unroll
-                for (int b = 0; b < 3; b++) uu[b] += pr[t][b];
-#pragma unroll
-              for (int b = 0; b < 3; b++) vv[b] = Hi[b * 3] * uu[0] + Hi[b * 3 + 1] * uu[1] + Hi[b * 3 + 2] * uu[2];
+            if (gi.z <= 8) {
+              plane_vec_small(G.upart, gi.y, gi.z, l, vv);
             } else if (c.use_tma) {   // large graph: solve_heavy() already reduced this plane
               for (int b = 0; b < 3; b++) vv[b] = ldc(G.vl + (size_t)l * 3 + b);
             } else {
@@ -2033,22 +2171,10 @@ struct Phase {
             const int l = G.grp_plane[g0 + g];
             const int t0 = G.upart_ptr[l], n = G.upart_ptr[l + 1] - t0;
             if (n <= 8) continue;
-            double uu[3] = {0, 0, 0};
-            for (int tb = t0 + lane; tb < t0 + n; tb += 256) {   // 8 strided partials per lane in flight
-              double pr[8][3];
-#pragma unroll
-              for (int t = 0; t < 8; t++)
-#pragma unroll
-                for (int b = 0; b < 3; b++) pr[t][b] = (tb + 32 * t < t0 + n) ? ldc(G.upart + (size_t)(tb + 32 * t) * 3 + b) : 0.0;
-#pragma unroll
-              for (int t = 0; t < 8; t++)
-#pragma unroll
-                for (int b = 0; b < 3; b++) uu[b] += pr[t][b];
-            }
-            for (int b = 0; b < 3; b++) uu[b] = warp_sum(uu[b]);
+            double uu[3];
+            warp_sum_partials(G.upart, t0, t0 + n, lane, uu);
             if (lane < 3) {
-              const double v = ldc(G.Hinv + (size_t)l * 9 + lane * 3) * uu[0] + ldc(G.Hinv + (size_t)l * 9 + lane * 3 + 1) * uu[1] +
-                               ldc(G.Hinv + (size_t)l * 9 + lane * 3 + 2) * uu[2];
+              const double v = dot3<LdL2>(G.Hinv + (size_t)l * 9 + lane * 3, uu);
               if (ov < 0) vg[(slot * kMaxGrp + g) * 3 + lane] = v;
               else __stcg(G.ovf + ov + g * 3 + lane, v);
             }
@@ -2083,19 +2209,11 @@ struct Phase {
           if (c.use_tma) {
             mbar_wait(tbar + st, (c.tma_par >> st) & 1u);
             c.tma_par ^= (1u << st);
-            if (key >= 0) {
-              const double* w = tbuf + st * kWStride + lane;
-#pragma unroll
-              for (int a = 0; a < 6; a++) y[a] = w[(a * 3) * 32] * v0 + w[(a * 3 + 1) * 32] * v1 + w[(a * 3 + 2) * 32] * v2;
-            }
+            if (key >= 0) tile_w_v<LdS>(tbuf + st * kWStride + lane, v0, v1, v2, y);
           } else if (key >= 0) {
-            const double* w = G.W + (size_t)(t0 + t) * kWStride + lane;
-#pragma unroll
-            for (int a = 0; a < 6; a++) y[a] = ldc(w + (a * 3) * 32) * v0 + ldc(w + (a * 3 + 1) * 32) * v1 + ldc(w + (a * 3 + 2) * 32) * v2;
+            tile_w_v<LdL2>(G.W + (size_t)(t0 + t) * kWStride + lane, v0, v1, v2, y);
           }
-          seg_suffix_sum<6>(key, y);
-          int pk = __shfl_up_sync(0xffffffffu, key, 1);
-          if (key >= 0 && (lane == 0 || pk != key)) {
+          if (seg_suffix_sum<6>(key, y)) {
             if (ov < 0) {
               double* o = yp + (slot * kMaxPart + (part - part0)) * 6;
               for (int a = 0; a < 6; a++) o[a] = y[a];
@@ -2139,35 +2257,18 @@ struct Phase {
             // record and are loaded together, the rest loop over the incidence list
             const int4 nb = *reinterpret_cast<const int4*>(G.pnbr + (size_t)p * 8);
             const int2 nr = *reinterpret_cast<const int2*>(G.pnbr + (size_t)p * 8 + 4);
-            const int i1 = nr.y;
-            int kk = nr.x;
-            const int nf = (nb.x >= 0) + (nb.z >= 0);
-            const double* Ab[2] = {G.PF + (size_t)(max(nb.x, 0) >> 1) * 120 + 72, G.PF + (size_t)(max(nb.z, 0) >> 1) * 120 + 72};
             const double* xo[2] = {pvec + (size_t)max(nb.y, 0) * 6, pvec + (size_t)max(nb.w, 0) * 6};
-            const int sd[2] = {nb.x & 1, nb.z & 1};
-            double av[2][6], xv[2][6];
+            double av[12], xv[2][6];
+            const int nf = nbr_coeffs(nb, row, av);
 #pragma unroll
             for (int n2 = 0; n2 < 2; n2++)
 #pragma unroll
-              for (int cc = 0; cc < 6; cc++) {
-                av[n2][cc] = (n2 < nf) ? (sd[n2] ? ldc(Ab[n2] + cc * 6 + row) : ldc(Ab[n2] + row * 6 + cc)) : 0.0;
-                xv[n2][cc] = (n2 < nf) ? ldc(xo[n2] + cc) : 0.0;
-              }
+              for (int cc = 0; cc < 6; cc++) xv[n2][cc] = (n2 < nf) ? ldc(xo[n2] + cc) : 0.0;
 #pragma unroll
             for (int n2 = 0; n2 < 2; n2++)
 #pragma unroll
-              for (int cc = 0; cc < 6; cc++) v += av[n2][cc] * xv[n2][cc];
-            for (; kk < i1; kk++) {
-              int inc = G.pinc[kk], f = inc >> 1, side = inc & 1;
-              int j = G.pf_j[f];
-              if (j < 0) continue;
-              int oth = side ? G.pf_i[f] : j;
-              const double* A12 = G.PF + (size_t)f * 120 + 72;
-              for (int cc = 0; cc < 6; cc++) {
-                double a = side ? ldc(A12 + cc * 6 + row) : ldc(A12 + row * 6 + cc);
-                v += a * ldc(pvec + (size_t)oth * 6 + cc);
-              }
-            }
+              for (int cc = 0; cc < 6; cc++) v += av[n2 * 6 + cc] * xv[n2][cc];
+            v = pose_pose_tail(nr.x, nr.y, row, pvec, v);
           }
           v -= ysum;
           qout[o] = v;   // (q is only read back by the owner of the block: not mirrored)
@@ -2334,29 +2435,8 @@ struct Phase {
     } else {
       // full coarse residual rc = sum_k rc_old[k] - alpha * sum_k qcpart[k]  (linear in r)
       __syncthreads();
-      if (bpn == 1) {
-        // one block per coarse interval (graphs up to 5120 poses): block `node` feeds the node through its slot 0,
-        // block `node-1` through slot 1; four outputs per thread so that all 16 loads are in flight together
-        for (int i0 = tid; i0 < ldm; i0 += 4 * kThreads) {
-          double va[4][2], vq[4][2];
-  #pragma unroll
-          for (int m = 0; m < 4; m++) {
-            const int i = i0 + m * kThreads, node = i / 6, row = i - node * 6;
-  #pragma unroll
-            for (int side = 0; side < 2; side++) {
-              const int k = node - side;
-              const bool ok = (i < ldm) && (k >= 0) && (k < G.nblk);
-              va[m][side] = ok ? ldc(rc_old + (size_t)k * 12 + side * 6 + row) : 0.0;
-              vq[m][side] = (ok && !first) ? ldc(G.qcpart + (size_t)k * 12 + side * 6 + row) : 0.0;
-            }
-          }
-  #pragma unroll
-          for (int m = 0; m < 4; m++) {
-            const int i = i0 + m * kThreads;
-            if (i < ldm) src[i] = (0.0 + (va[m][0] - alpha * vq[m][0])) + (va[m][1] - alpha * vq[m][1]);
-          }
-        }
-      } else
+      if (bpn == 1) coarse_residual(rc_old, alpha, first, src);
+      else
       for (int i = tid; i < ldm; i += kThreads) {
         int node = i / 6, row = i % 6;
         // blocks with c0 == node feed `node` through their slot 0, blocks with c0 == node-1 through slot 1;
@@ -2402,35 +2482,7 @@ struct Phase {
         const int lane = tid & 31;
         const int nw = nwarp_team();
         for (int i = warp_team(); i < ldm; i += nw) {
-          const double* arow = Ai + ac_index(G.ldmc, i, 0);
-          double acc = 0;
-          // 128-bit loads, a lane owns column pairs (2 lane + 64 t): a 1 884-wide row is two batches of 16 loads in flight
-          // (pairs never straddle a 128-column tile: tile rows are 16-byte aligned, stride 132)
-          int j = 2 * lane;
-          for (; j + 64 * 15 < ldm; j += 64 * 16) {
-            double2 av[16];
-  #pragma unroll
-            for (int t = 0; t < 16; t++) {
-              const int jj = j + 64 * t;
-              av[t] = __ldcg(reinterpret_cast<const double2*>(arow + (size_t)(jj / kGjChunk) * kGjTile + (jj % kGjChunk)));
-            }
-  #pragma unroll
-            for (int t = 0; t < 16; t++) acc += av[t].x * src[j + 64 * t] + av[t].y * src[j + 64 * t + 1];
-          }
-          {
-            double2 av[16];
-  #pragma unroll
-            for (int t = 0; t < 16; t++) {
-              const int jj = j + 64 * t;
-              av[t] = (jj < ldm) ? __ldcg(reinterpret_cast<const double2*>(arow + (size_t)(jj / kGjChunk) * kGjTile + (jj % kGjChunk))) : make_double2(0.0, 0.0);
-            }
-  #pragma unroll
-            for (int t = 0; t < 16; t++) {
-              const int jj = j + 64 * t;
-              if (jj < ldm) acc += av[t].x * src[jj] + av[t].y * src[jj + 1];   // (ldm = 6 nc is even)
-            }
-          }
-          acc = warp_sum(acc);
+          const double acc = coarse_row_dot(Ai + ac_index(G.ldmc, i, 0), src, ldm, lane);
           if (lane == 0) { put(c, &G.zc[i], acc); dot += src[i] * acc; }
         }
       }
@@ -2497,8 +2549,8 @@ struct Phase {
           const int u = tid >> 2, qq = tid & 3;
           const double* cb = bbuf + stg * kPackedBlock;
           double zl = 0;
-          for (int j = qq; j < u; j += 4) zl += cb[j * kBlockDim - (j * (j - 1)) / 2 + (u - j)] * rv[j];
-          const double* cu = cb + u * kBlockDim - (u * (u - 1)) / 2 - u;
+          for (int j = qq; j < u; j += 4) zl += packed_row(cb, j)[u] * rv[j];
+          const double* cu = packed_row(cb, u);
           for (int j = u + ((qq - u) & 3); j < kBlockDim; j += 4) zl += cu[j] * rv[j];
           zl += __shfl_xor_sync(0xffffffffu, zl, 1);
           zl += __shfl_xor_sync(0xffffffffu, zl, 2);
@@ -2539,22 +2591,11 @@ struct Phase {
       if (live) restrict_block(sA, slot, u, k, np, rc_new);
       if (on) {
         // dense block: z_local = Binv[k] r_block (symmetric: read column u)
-        double zl = 0;
         const int ci = slot + kSlots * rd;
-        if (ci < kCacheBlocks && (c.smem_cache_ok)) {
-          const double* cb = reinterpret_cast<const double*>(g_smem + kSmCache) + (size_t)ci * kPackedBlock;
-          const double* rv = sA + slot * kBlockDim;
-          // rows j < u: element (j,u) ; rows j >= u: element (u,j)
-          for (int j = 0; j < u; j++) zl += cb[j * kBlockDim - (j * (j - 1)) / 2 + (u - j)] * rv[j];
-          const double* cu = cb + u * kBlockDim - (u * (u - 1)) / 2 - u;
-          for (int j = u; j < kBlockDim; j++) zl += cu[j] * rv[j];
-        } else {
-          const double* cb = G.Binv + (size_t)k * kPackedBlock;   // packed upper triangle, straight from L2
-          const double* rv = sA + slot * kBlockDim;
-          for (int j = 0; j < u; j++) zl += ldc(cb + j * kBlockDim - (j * (j - 1)) / 2 + (u - j)) * rv[j];
-          const double* cu = cb + u * kBlockDim - (u * (u - 1)) / 2 - u;
-          for (int j = u; j < kBlockDim; j++) zl += ldc(cu + j) * rv[j];
-        }
+        const double* rv = sA + slot * kBlockDim;
+        const double zl = (ci < kCacheBlocks && c.smem_cache_ok)
+                              ? packed_row_dot<LdS>(reinterpret_cast<const double*>(g_smem + kSmCache) + (size_t)ci * kPackedBlock, u, rv)
+                              : packed_row_dot<LdL2>(G.Binv + (size_t)k * kPackedBlock, u, rv);   // straight from L2
         put(c, &G.z[(size_t)p * 6 + row], zl);
         dot += rn * zl;
       }
@@ -2574,6 +2615,10 @@ struct Phase {
   //   C  coarse residual (linear update) ; A_c^-1 rows -> zc ; x, r updated in registers ; z = Binv r from smem ; r.z -> reduction
   // r, x, z, p, q of a row live in the registers of its thread for the whole solve.  Entry state (from the common prologue):
   // G.r, G.x, G.z (local part), G.zc, rcpart[rcb] ; exit: G.x.  Returns the iteration count.
+  // Both loops call the same helpers for the arithmetic they share: tile_wt_x and seg_suffix_sum
+  // (A, as in sweep_planes), plane_vec_small, warp_sum_partials, mat3_vec / dot3, tile_w_v, nbr_coeffs and pose_pose_tail (B, as in
+  // solve_heavy and pose_phase), coarse_residual and coarse_row_dot (C, as in precondition).  The dense-block apply is its own: it
+  // reads the folded copy below instead of the packed triangle, with two accumulators.
   __device__ int pcg_resident(double lambda, int rcb, const double rz0, double rz, const double tol2, Timer& tmr) {
     const int ldm = 6 * G.nc;
     const int nown_max = (G.nblk + c.tsize - 1) / c.tsize;
@@ -2620,7 +2665,7 @@ struct Phase {
       for (int i = tid; i < kBlockDim * kBlockDim; i += kThreads) {
         const int ra = i / kBlockDim, cb2 = i - ra * kBlockDim;
         if (cb2 < ra) continue;
-        const double v = ldc(Bg + ra * kBlockDim - (ra * (ra - 1)) / 2 + (cb2 - ra));
+        const double v = ldc(packed_row(Bg, ra) + cb2);
         const int fi = kBlockDim - 1 - ra, d = cb2 - ra;
         Bc[ra < kBlockDim / 2 ? ra * 97 + cb2 : fi * 97 + (d < fi ? d : 96)] = v;
       }
@@ -2663,13 +2708,7 @@ struct Phase {
       const double* H = G.Hpp + (size_t)p * 36 + row * 6;
 #pragma unroll
       for (int cc = 0; cc < 6; cc++) trow[cc] = ldc(H + cc) * (cc == row ? (1 + lambda) : 1.0);
-      const double* Ab[2] = {G.PF + (size_t)(max(nb.x, 0) >> 1) * 120 + 72, G.PF + (size_t)(max(nb.z, 0) >> 1) * 120 + 72};
-      const int sd[2] = {nb.x & 1, nb.z & 1};
-#pragma unroll
-      for (int n2 = 0; n2 < 2; n2++)
-#pragma unroll
-        for (int cc = 0; cc < 6; cc++)
-          trow[6 + n2 * 6 + cc] = (n2 < nf) ? (sd[n2] ? ldc(Ab[n2] + cc * 6 + row) : ldc(Ab[n2] + row * 6 + cc)) : 0.0;
+      nbr_coeffs(nb, row, trow + 6);
     }
     __syncthreads();
     // planes seen from more than 8 pose blocks (the ground plane from all): summed once per CTA by all its warps instead of
@@ -2727,16 +2766,8 @@ struct Phase {
             const int info = reinterpret_cast<const int*>(sbs + L.o_ei)[t * 32 + lane];
             const int pe = info & 31;
             double uu[3] = {0, 0, 0};
-            if (pe != 31) {
-              const double* xs = sP + s * kBlockDim + pe * 6;
-              const double* w = reinterpret_cast<const double*>(sbs + L.o_W) + t * kWStride + lane;
-#pragma unroll
-              for (int a = 0; a < 6; a++) {
-                const double xa = xs[a];
-#pragma unroll
-                for (int b = 0; b < 3; b++) uu[b] += w[(a * 3 + b) * 32] * xa;
-              }
-            }
+            if (pe != 31)
+              tile_wt_x<LdS>(reinterpret_cast<const double*>(sbs + L.o_W) + t * kWStride + lane, sP + s * kBlockDim + pe * 6, uu);
             double* se = reinterpret_cast<double*>(sbs) + (size_t)(t * 32 + lane) * 3;
             se[0] = uu[0]; se[1] = uu[1]; se[2] = uu[2];
           }
@@ -2768,44 +2799,15 @@ struct Phase {
       if (live) {
         for (int g = u; g < ng; g += kBlockDim) {
           const int4 gq = gi[g];
-          const int l = gq.x, t0 = gq.y, n = gq.z;
-          if (n >= 0 && n <= 8) {
-            double pr[8][3], Hi[9];
-#pragma unroll
-            for (int t = 0; t < 8; t++)
-#pragma unroll
-              for (int b = 0; b < 3; b++) pr[t][b] = (t < n) ? ldc(G.upartb + (size_t)(t0 + t) * 3 + b) : 0.0;
-#pragma unroll
-            for (int t = 0; t < 9; t++) Hi[t] = ldc(G.Hinv + (size_t)l * 9 + t);
-            double uu[3] = {0, 0, 0};
-#pragma unroll
-            for (int t = 0; t < 8; t++)
-#pragma unroll
-              for (int b = 0; b < 3; b++) uu[b] += pr[t][b];
-#pragma unroll
-            for (int b = 0; b < 3; b++) vg[g * 3 + b] = Hi[b * 3] * uu[0] + Hi[b * 3 + 1] * uu[1] + Hi[b * 3 + 2] * uu[2];
-          }
+          if (gq.z >= 0 && gq.z <= 8) plane_vec_small(G.upartb, gq.y, gq.z, gq.x, vg + g * 3);
         }
         for (int g = wis; g < ng; g += 3) {   // unlisted planes seen from more than 8 pose blocks: a warp of the block sums the partials
           const int4 gq = gi[g];
           const int l = gq.x, t0 = gq.y, n = gq.z;
           if (n <= 8) continue;
-          double uu[3] = {0, 0, 0};
-          for (int tb = t0 + lane; tb < t0 + n; tb += 256) {
-            double pr[8][3];
-#pragma unroll
-            for (int t = 0; t < 8; t++)
-#pragma unroll
-              for (int b = 0; b < 3; b++) pr[t][b] = (tb + 32 * t < t0 + n) ? ldc(G.upartb + (size_t)(tb + 32 * t) * 3 + b) : 0.0;
-#pragma unroll
-            for (int t = 0; t < 8; t++)
-#pragma unroll
-              for (int b = 0; b < 3; b++) uu[b] += pr[t][b];
-          }
-          for (int b = 0; b < 3; b++) uu[b] = warp_sum(uu[b]);
-          if (lane < 3)
-            vg[g * 3 + lane] = ldc(G.Hinv + (size_t)l * 9 + lane * 3) * uu[0] + ldc(G.Hinv + (size_t)l * 9 + lane * 3 + 1) * uu[1] +
-                               ldc(G.Hinv + (size_t)l * 9 + lane * 3 + 2) * uu[2];
+          double uu[3];
+          warp_sum_partials(G.upartb, t0, t0 + n, lane, uu);
+          if (lane < 3) vg[g * 3 + lane] = dot3<LdL2>(G.Hinv + (size_t)l * 9 + lane * 3, uu);
         }
       }
       // listed heavy planes: `wpe` warps each, every warp one contiguous chunk of the plane's per-block partials
@@ -2823,19 +2825,8 @@ struct Phase {
         const int h = warp / wpe, j = warp - h * wpe;
         const int t0 = hvl[h * 4 + 1], n = hvl[h * 4 + 2];
         const int per = (n + wpe - 1) / wpe, a0 = t0 + j * per, a1 = min(t0 + n, a0 + per);
-        double uu[3] = {0, 0, 0};
-        for (int tb = a0 + lane; tb < a1; tb += 256) {
-          double pr[8][3];
-#pragma unroll
-          for (int t = 0; t < 8; t++)
-#pragma unroll
-            for (int b = 0; b < 3; b++) pr[t][b] = (tb + 32 * t < a1) ? ldc(G.upartb + (size_t)(tb + 32 * t) * 3 + b) : 0.0;
-#pragma unroll
-          for (int t = 0; t < 8; t++)
-#pragma unroll
-            for (int b = 0; b < 3; b++) uu[b] += pr[t][b];
-        }
-        for (int b = 0; b < 3; b++) uu[b] = warp_sum(uu[b]);
+        double uu[3];
+        warp_sum_partials(G.upartb, a0, a1, lane, uu);
         if (lane < 3) hvp[(h * kWarps + j) * 3 + lane] = (lane == 0) ? uu[0] : (lane == 1 ? uu[1] : uu[2]);
       }
       if (nh) {
@@ -2844,16 +2835,14 @@ struct Phase {
           double uu[3] = {0, 0, 0};
           for (int j = 0; j < wpe; j++)
             for (int b = 0; b < 3; b++) uu[b] += hvp[(hidx * kWarps + j) * 3 + b];
-          for (int b = 0; b < 3; b++) vg[hg * 3 + b] = hHi[b * 3] * uu[0] + hHi[b * 3 + 1] * uu[1] + hHi[b * 3 + 2] * uu[2];
+          mat3_vec(hHi, uu, vg + hg * 3);
           for (int g = hg + kBlockDim; g < ng; g += kBlockDim)   // (blocks with more than 96 groups: further listed groups of this thread)
             if (gi[g].z < 0) {
               const int hi2 = -gi[g].z - 1, l2 = gi[g].x;
               double u2[3] = {0, 0, 0};
               for (int j = 0; j < wpe; j++)
                 for (int b = 0; b < 3; b++) u2[b] += hvp[(hi2 * kWarps + j) * 3 + b];
-              for (int b = 0; b < 3; b++)
-                vg[g * 3 + b] = ldc(G.Hinv + (size_t)l2 * 9 + b * 3) * u2[0] + ldc(G.Hinv + (size_t)l2 * 9 + b * 3 + 1) * u2[1] +
-                                ldc(G.Hinv + (size_t)l2 * 9 + b * 3 + 2) * u2[2];
+              for (int b = 0; b < 3; b++) vg[g * 3 + b] = dot3<LdL2>(G.Hinv + (size_t)l2 * 9 + b * 3, u2);
             }
         }
       }
@@ -2871,14 +2860,9 @@ struct Phase {
             double y[6] = {0, 0, 0, 0, 0, 0};
             if (key >= 0) {
               const double* vv = reinterpret_cast<const double*>(sbs) + ((info >> 5) & 511) * 3;
-              const double v0 = vv[0], v1 = vv[1], v2 = vv[2];
-              const double* w = reinterpret_cast<const double*>(sbs + L.o_W) + t * kWStride + lane;
-#pragma unroll
-              for (int a = 0; a < 6; a++) y[a] = w[(a * 3) * 32] * v0 + w[(a * 3 + 1) * 32] * v1 + w[(a * 3 + 2) * 32] * v2;
+              tile_w_v<LdS>(reinterpret_cast<const double*>(sbs + L.o_W) + t * kWStride + lane, vv[0], vv[1], vv[2], y);
             }
-            seg_suffix_sum<6>(key, y);
-            const int pk = __shfl_up_sync(0xffffffffu, key, 1);
-            if (key >= 0 && (lane == 0 || pk != key)) {
+            if (seg_suffix_sum<6>(key, y)) {
               double* yo = reinterpret_cast<double*>(sbs + r16(G.res_ng * 24)) + (size_t)(info >> 14) * 6;
 #pragma unroll
               for (int a = 0; a < 6; a++) yo[a] = y[a];
@@ -2911,17 +2895,7 @@ struct Phase {
               vb += trow[12 + cc] * (here ? sP[slot * kBlockDim + (oth1 - k * kBlockPoses) * 6 + cc] : ldc(pvec + (size_t)oth1 * 6 + cc));
           }
           vv += va + vb;
-          for (int kk = nr.x; kk < nr.y; kk++) {   // further pose-pose factors of this pose (loop closures): generic list
-            const int inc = G.pinc[kk], f = inc >> 1, side = inc & 1;
-            const int j = G.pf_j[f];
-            if (j < 0) continue;
-            const int ot = side ? G.pf_i[f] : j;
-            const double* A12 = G.PF + (size_t)f * 120 + 72;
-            for (int cc = 0; cc < 6; cc++) {
-              const double a = side ? ldc(A12 + cc * 6 + row) : ldc(A12 + row * 6 + cc);
-              vv += a * ldc(pvec + (size_t)ot * 6 + cc);
-            }
-          }
+          vv = pose_pose_tail(nr.x, nr.y, row, pvec, vv);   // further pose-pose factors of this pose (loop closures)
         }
         q_u = vv - ysum;
         dot = p_u * q_u;
@@ -2937,25 +2911,7 @@ struct Phase {
       // ================= C =================
       const double* rc_old = G.rcpart[rcb];
       double* rc_new = G.rcpart[rcb ^ 1];
-      for (int i0 = tid; i0 < ldm; i0 += 4 * kThreads) {
-        double va[4][2], vq[4][2];
-#pragma unroll
-        for (int m = 0; m < 4; m++) {
-          const int i = i0 + m * kThreads, node = i / 6, rr = i - node * 6;
-#pragma unroll
-          for (int side = 0; side < 2; side++) {
-            const int kb = node - side;
-            const bool ok = (i < ldm) && (kb >= 0) && (kb < G.nblk);
-            va[m][side] = ok ? ldc(rc_old + (size_t)kb * 12 + side * 6 + rr) : 0.0;
-            vq[m][side] = ok ? ldc(G.qcpart + (size_t)kb * 12 + side * 6 + rr) : 0.0;
-          }
-        }
-#pragma unroll
-        for (int m = 0; m < 4; m++) {
-          const int i = i0 + m * kThreads;
-          if (i < ldm) src[i] = (0.0 + (va[m][0] - alpha * vq[m][0])) + (va[m][1] - alpha * vq[m][1]);
-        }
-      }
+      coarse_residual(rc_old, alpha, false, src);
       if (on) { x_u += alpha * p_u; r_u -= alpha * q_u; }
       if (live) sR[slot * kBlockDim + u] = on ? r_u : 0.0;
       __syncthreads();
@@ -2970,33 +2926,7 @@ struct Phase {
         const int nw = bal ? ne * kWarps : nwarp_team();
         const int w0 = bal ? (c.rank >= n3 ? warp * ne + (c.rank - n3) : ldm) : warp_team();
         for (int i = w0; i < ldm; i += nw) {
-          const double* arow = Ai + ac_index(G.ldmc, i, 0);
-          double acc = 0;
-          int j = 2 * lane;
-          for (; j + 64 * 15 < ldm; j += 64 * 16) {
-            double2 av[16];
-#pragma unroll
-            for (int t = 0; t < 16; t++) {
-              const int jj = j + 64 * t;
-              av[t] = __ldcg(reinterpret_cast<const double2*>(arow + (size_t)(jj / kGjChunk) * kGjTile + (jj % kGjChunk)));
-            }
-#pragma unroll
-            for (int t = 0; t < 16; t++) acc += av[t].x * src[j + 64 * t] + av[t].y * src[j + 64 * t + 1];
-          }
-          {
-            double2 av[16];
-#pragma unroll
-            for (int t = 0; t < 16; t++) {
-              const int jj = j + 64 * t;
-              av[t] = (jj < ldm) ? __ldcg(reinterpret_cast<const double2*>(arow + (size_t)(jj / kGjChunk) * kGjTile + (jj % kGjChunk))) : make_double2(0.0, 0.0);
-            }
-#pragma unroll
-            for (int t = 0; t < 16; t++) {
-              const int jj = j + 64 * t;
-              if (jj < ldm) acc += av[t].x * src[jj] + av[t].y * src[jj + 1];
-            }
-          }
-          acc = warp_sum(acc);
+          const double acc = coarse_row_dot(Ai + ac_index(G.ldmc, i, 0), src, ldm, lane);
           if (lane == 0) { G.zc[i] = acc; dot += src[i] * acc; }
         }
       }
@@ -3006,7 +2936,7 @@ struct Phase {
         // a warp is on one side of the fold), a lane per row, two accumulators; consecutive lanes read consecutive or
         // odd-strided words in every segment of the row.
         double* sZ = sE;   // [96] per slot (scratch, free in phase C)
-        for (int task = warp; task < 4 * nown && G.prm.fine_timers != 3; task += kWarps) {   // (fine_timers == 3: timing experiment without the mat-vec)
+        for (int task = warp; task < 4 * nown; task += kWarps) {
           const int s = task >> 2, part = task & 3;
           const int uu = (part == 0 ? 0 : part == 1 ? 32 : part == 2 ? 48 : 80) + lane;
           const bool act = (part & 1) ? lane < 16 : true;
