@@ -362,6 +362,14 @@ class GpuGraphAPI(GraphAPI):
         forms (the default of the CUDA library)."""
         self._chk(self.lib.pus_set_jacobian_mode(self.h, 1 if int(mode) == 0 else 0))
 
+    def set_linear_solver(self, direct):
+        """direct=True: solve the reduced pose system exactly (dense Cholesky on the device, graphs of at most 640 poses);
+        direct=False: block-preconditioned CG (the default)."""
+        self._chk(self.lib.pus_set_linear_solver(self.h, 1 if direct else 0))
+
+    def linear_solver_is_direct(self):
+        return self._chk(self.lib.pus_get_linear_solver(self.h)) == 1
+
     def get_solver_options(self):
         o = SolverOptions()
         self._chk(self.lib.pus_get_solver_options(self.h, C.byref(o)))

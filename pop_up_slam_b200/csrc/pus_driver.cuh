@@ -127,6 +127,61 @@ __device__ double schur_solve(Phase& ph, Ctx& c, double lambda, int* its, Timer&
   return sqrt(v[0]);
 }
 
+#ifdef PUS_DIRECT
+// Exact direct solve (pus::kdirect): replaces schur_setup / schur_solve.  Sub-timers: 8 plane inverses, 10 per-incidence
+// W / Y blocks, 11 assembly of S, 12 factorization, 13 right-hand side, 14 triangular solves.
+__device__ void direct_setup(Phase& ph, Ctx& c, double lambda, Timer& ft) {
+  ft.sync();
+  if (c.rank == 0 && threadIdx.x == 0) *G.dflag = 0u;
+  ph.plane_inverse(lambda);
+  team_barrier(c);
+  ft.lap(8);
+  ph.direct_wy();
+  team_barrier(c);
+  ft.lap(10);
+  ph.direct_assemble(lambda);
+  team_barrier(c);
+  ft.lap(11);
+  if (G.prm.mode == MODE_DEBUG && G.prm.debug_stage == 4) return;   // stop after the assembly ("Sdir")
+  ph.direct_factor();
+  ft.lap(12);
+}
+
+// x = S^-1 b, then the planes as schur_solve does.  *its = 0, or -1 after a non-positive pivot: then delta = 0.
+__device__ double direct_solve(Phase& ph, Ctx& c, double lambda, int* its, Timer& ft) {
+  if (G.prm.mode == MODE_DEBUG && G.prm.debug_stage == 4) { *its = 0; return 0.0; }
+  ft.sync();
+  const bool failed = __ldcg(G.dflag) != 0u;
+  double v[1];
+  if (failed) {
+    for (int i = ph.tid_team(); i < G.N * 6; i += ph.nthr_team()) G.x[i] = 0.0;
+    for (int i = ph.tid_team(); i < G.M * 3; i += ph.nthr_team()) G.dl[i] = 0.0;
+    team_barrier(c);
+    *its = -1;
+    return 0.0;
+  }
+  ph.pose_phase(true, nullptr, lambda, nullptr, nullptr);   // b = -gp + W Hll_d^-1 gl
+  team_barrier(c);
+  ft.lap(13);
+  ph.direct_trsv();
+  for (int i = ph.tid_team(); i < G.N * 6; i += ph.nthr_team()) G.x[i] = ldc(G.dvec + i);
+  team_barrier(c);
+  ft.lap(14);
+  ph.sweep_planes(G.x, nullptr, 0.0);
+  team_barrier(c);
+  v[0] = ph.solve_planes(1) + ph.norm_x();
+  team_reduce<1>(c, G.red, v);
+  *its = 0;
+  return sqrt(v[0]);
+}
+#define schur_setup(ph, c, lambda, ft, rebuild) direct_setup(ph, c, lambda, ft)
+#define schur_solve(ph, c, lambda, its, ft, warm) ((void)(warm), direct_solve(ph, c, lambda, its, ft))
+// a failed factorization (|delta| = 0) is a rejected LM step, not convergence
+#define PUS_SOLVE_FAILED(its) || ((its) < 0 && iter < kTraceCap)
+#else
+#define PUS_SOLVE_FAILED(its)
+#endif
+
 __device__ void run_graph_impl(Ctx& c) {
   Phase ph(c);
   const LmParams& P = G.prm;
@@ -215,7 +270,7 @@ __device__ void run_graph_impl(Ctx& c) {
     tm.lap(3);
   } else if (P.method == 1) {
     int last_pcg = its;
-    while ((P.max_iter <= 0 || iter < P.max_iter) && dnorm > P.eps2 && err > P.eps_abs) {
+    while ((P.max_iter <= 0 || iter < P.max_iter) && (dnorm > P.eps2 PUS_SOLVE_FAILED(its)) && err > P.eps_abs) {
       iter++;
       ph.apply_delta();
       team_barrier(c);
@@ -371,5 +426,9 @@ __global__ void __launch_bounds__(kThreads, 1) lm_kernel(const DevGraph* graphs,
   if (c.cluster) cluster_sync_all();   // no CTA exits while a peer may still address its shared memory
 }
 
-
+#undef PUS_SOLVE_FAILED
+#ifdef PUS_DIRECT
+#undef schur_setup
+#undef schur_solve
+#endif
 #undef G

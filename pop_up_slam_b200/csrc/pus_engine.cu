@@ -27,6 +27,10 @@ using namespace kplain;
 void* span_kernel_ptr();
 size_t span_devgraph_bytes();
 cudaError_t span_kernel_prepare();
+// the third (pus::kdirect, pus_direct.cu): the kernel of handles in direct linear-solver mode
+void* direct_kernel_ptr();
+size_t direct_devgraph_bytes();
+cudaError_t direct_kernel_prepare();
 
 // ---------------------------------------------------------------------------------------------
 // host engine
@@ -49,8 +53,10 @@ struct Solver {
   int robust_kind = 0;
   double robust_b = 1.0;
   int jac_numeric = 0;
+  int linear_solver = 0;       // 0: PCG, 1: exact dense Cholesky of the reduced pose system (pus_set_linear_solver)
   pus_solver_options opt;
   Compiled c;
+  DirectTables dt;             // (direct mode only)
   uint64_t compiled_topo = 0;
   bool meas_dirty = true;
   int span_w = 1, span_r = 0;  // one graph spanning ranks: world / rank and the peers' arenas (CUDA IPC mappings)
@@ -178,7 +184,11 @@ static int ensure_device(Solver* s) {
     s->num_sms = p.multiProcessorCount;
     CUDA_OK(cudaFuncSetAttribute(kplain::lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     CUDA_OK(span_kernel_prepare());
-    if (span_devgraph_bytes() != sizeof(DevGraph)) { g_err = "device-code instantiations disagree on the DevGraph layout"; return -1; }
+    CUDA_OK(direct_kernel_prepare());
+    if (span_devgraph_bytes() != sizeof(DevGraph) || direct_devgraph_bytes() != sizeof(DevGraph)) {
+      g_err = "device-code instantiations disagree on the DevGraph layout";
+      return -1;
+    }
   }
   return 0;
 }
@@ -215,6 +225,7 @@ static int upload(Solver* s) {
     s->recycle_device();
     std::string err;
     if (!compile_graph(s->g, s->c, err)) { g_err = err; return -1; }
+    if (s->linear_solver == 1 && !build_direct(s->c, s->dt, err)) { g_err = err; return -1; }
     const Compiled& c = s->c;
     if (kSmRc + 6 * c.nc * 8 > kSmemBytes) { g_err = "graph too large for the coarse-space shared-memory buffer"; return -1; }
     DevGraph& d = s->hd;
@@ -252,7 +263,6 @@ static int upload(Solver* s) {
     AL(Binv, (size_t)c.nblk * kPackedBlock, "Binv"); AL(Wc, (size_t)c.nce * 18, "Wc"); AL(Yc, (size_t)c.nce * 18, "Yc");
     AL(Ac, ac_doubles(6 * c.nc_pad), "Ac"); AL(Atri, ac_tri_doubles(6 * c.nc_pad), "Atri"); AL(Apan, ac_panel_doubles(6 * c.nc_pad), "Apan");
     AL(Wc2, (size_t)c.nce2 * 18, "Wc2"); AL(Yc2, (size_t)c.nce2 * 18, "Yc2"); AL(D2inv, (size_t)c.ng2 * kBlockDim * kBlockDim, "D2inv");
-#undef AL
     {
       // The vectors the PCG phases exchange live in ONE allocation (the "mirror arena"): when one graph spans several
       // ranks every rank lays it out identically, so a peer's copy of any element is at a fixed byte offset.
@@ -279,6 +289,20 @@ static int upload(Solver* s) {
       }
       d.span_w = 1; d.span_r = 0;
     }
+    if (s->linear_solver == 1) {   // the dense solve's tables and its tile store (about 65 MB at the 640-pose cap)
+      const DirectTables& dt = s->dt;
+      const size_t nb = dt.nb, ninc = dt.inc_pose.size();
+      d.dnb = dt.nb; d.dninc = (int)ninc;
+#define UPD(field, vec) if (s->dupload(&d.field, vec, &bytes) < 0) return -1
+      UPD(dinc_plane, dt.inc_plane); UPD(dinc_lo, dt.inc_lo); UPD(dinc_hi, dt.inc_hi);
+      UPD(dlp_ptr, dt.lp_ptr); UPD(dlp_a, dt.lp_a); UPD(dlp_b, dt.lp_b); UPD(dfp_ptr, dt.fp_ptr); UPD(dfp_f, dt.fp_f);
+#undef UPD
+      AL(Wd, ninc * 18, "Wd"); AL(Yd, ninc * 18, "Yd");
+      AL(Sd, nb * (nb + 1) / 2 * kAcTile, nullptr); AL(Dsnap, (2 * nb + 2) * kAcTile, nullptr); AL(Dinv, nb * kAcTile, nullptr);
+      AL(dvec, 2 * 48 * nb, nullptr);
+      if (s->dalloc(&d.dflag, 1) < 0) return -1;
+    }
+#undef AL
     CUDA_OK(cudaMemsetAsync(d.W, 0, T * kWStride * sizeof(double), s->stream));
     CUDA_OK(cudaMemsetAsync(d.Wt, 0, TL * kWStride * sizeof(double), s->stream));
     if (s->dalloc(&s->d_graph, 1) < 0 || s->dalloc(&s->d_res, 1) < 0 || s->dalloc(&s->d_trace, 1) < 0 ||
@@ -372,8 +396,12 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
     if (!ss[i]->uploaded) { g_err = "graph not uploaded"; return -1; }
     if (ss[i]->device != s0->device) { g_err = "all graphs of a batch must live on one device"; return -1; }
   }
+  const int direct = s0->linear_solver;
+  for (int i = 0; i < n; i++)
+    if (ss[i]->linear_solver != direct) { g_err = "one launch cannot mix direct and PCG handles"; return -1; }
+  void* const kern = direct ? direct_kernel_ptr() : (void*)kplain::lm_kernel;
   int per_sm = 0;
-  CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kplain::lm_kernel, kThreads, kSmemBytes));
+  CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, kSmemBytes));
   if (per_sm < 1) { g_err = "lm_kernel does not fit on an SM"; return -1; }
   const int max_ctas = s0->num_sms * 1;
   int team = 1, grid = 1;
@@ -433,7 +461,7 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
       if (cl == team) t = cl;
       else if (n == 1 && s0->opt.team_ctas <= 0 && s0->c.levels == 2 && s0->c.nblk <= 2 * cl) t = cl;
       if (t > 1) {
-        if (t > 8) cudaFuncSetAttribute(kplain::lm_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+        if (t > 8) cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
         const int teams = (n == 1) ? 1 : std::min(n, max_ctas / t);
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(teams * t); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = kSmemBytes; cfg.stream = s0->stream;
@@ -441,12 +469,14 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
         at[0].id = cudaLaunchAttributeClusterDimension;
         at[0].val.clusterDim.x = t; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
-        static int active_cache[17] = {-1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1};   // per cluster size (one device type per process)
-        int active = active_cache[t];
+        // per kernel and cluster size (one device type per process)
+        static int active_cache[2][17] = {{-1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+                                          {-1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1}};
+        int active = active_cache[direct][t];
         if (active < 0) {
           active = 0;
-          if (cudaOccupancyMaxActiveClusters(&active, (void*)kplain::lm_kernel, &cfg) != cudaSuccess) { active = 0; cudaGetLastError(); }
-          active_cache[t] = active;
+          if (cudaOccupancyMaxActiveClusters(&active, kern, &cfg) != cudaSuccess) { active = 0; cudaGetLastError(); }
+          active_cache[direct][t] = active;
         }
         if (active >= teams) {
           team = t; grid = teams * t; use_cluster = 1;
@@ -489,7 +519,7 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
   unsigned* a3 = s0->d_bar;
   int a4 = use_cluster;
   void* args[] = {(void*)&a0, (void*)&a1, (void*)&a2, (void*)&a3, (void*)&a4};
-  void* kfn = spanning ? span_kernel_ptr() : (void*)kplain::lm_kernel;
+  void* kfn = spanning ? span_kernel_ptr() : kern;
   cudaError_t le;
   if (use_cluster) {
     // a team only synchronises inside its cluster, whose CTAs the hardware co-schedules: no cooperative launch needed
@@ -530,7 +560,7 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
     }
     pus_stats& st = s->stats;
     st.lm_iterations = s->res.iterations; st.accepted = s->res.accepted; st.relinearizations = s->res.relin;
-    st.chi2_evals = s->res.chi2_evals; st.pcg_iterations = s->res.pcg_iters; st.chi2_initial = s->res.chi2_initial;
+    st.chi2_evals = s->res.chi2_evals; st.pcg_iterations = direct ? 0 : s->res.pcg_iters; st.chi2_initial = s->res.chi2_initial;
     st.chi2_final = s->res.chi2_final; st.kernel_ms = ms; st.n_poses = s->c.N; st.n_planes = s->c.M; st.n_pose_plane = s->c.Epl;
     int npr = 0;
     for (int f = 0; f < s->c.Epf; f++) npr += s->c.pf_j[f] < 0;
@@ -810,6 +840,19 @@ int pus_set_robust(pus_handle h, int kind, double b) {
   SV(h)->robust_kind = kind; SV(h)->robust_b = b; return 0;
 }
 int pus_set_jacobian_mode(pus_handle h, int numeric) { NEED(h); SV(h)->jac_numeric = numeric ? 1 : 0; return 0; }
+int pus_set_linear_solver(pus_handle h, int kind) {
+  NEED(h);
+  Solver* s = SV(h);
+  if (kind != 0 && kind != 1) { g_err = "bad linear solver kind (0 = PCG, 1 = direct)"; return -1; }
+  if (kind != s->linear_solver) { s->linear_solver = kind; s->g.topo_version++; }   // the next upload lays the graph out again
+  return 0;
+}
+int pus_get_linear_solver(pus_handle h) { NEED(h); return SV(h)->linear_solver; }
+static int refuse_direct_span(Solver* s, const char* fn) {
+  if (s->linear_solver != 1) return 0;
+  g_err = std::string(fn) + ": the direct linear solver does not span ranks (set the PCG solver, kind 0)";
+  return -1;
+}
 int pus_get_solver_options(pus_handle h, pus_solver_options* out) { NEED(h); *out = SV(h)->opt; return 0; }
 int pus_set_solver_options(pus_handle h, const pus_solver_options* in) { NEED(h); SV(h)->opt = *in; return 0; }
 
@@ -827,7 +870,11 @@ static int solve_many(pus_handle* hs, int n, int* iters, int mode, int restore) 
   for (int i = 0; i < n; i++) ss[i] = SV(hs[i]);
   if (ensure_device(ss[0]) < 0) return -1;
   BatchStreams bs(hs, n, ss[0]->stream);
-  if (launch(ss.data(), n, mode, restore, 0, 0.0) < 0) return -1;
+  // direct-mode and PCG handles run in their own kernels: a mixed batch is two launches, one per kind
+  std::vector<Solver*> part[2];
+  for (int i = 0; i < n; i++) part[ss[i]->linear_solver == 1].push_back(ss[i]);
+  for (int k = 0; k < 2; k++)
+    if (!part[k].empty() && launch(part[k].data(), (int)part[k].size(), mode, restore, 0, 0.0) < 0) return -1;
   if (iters) for (int i = 0; i < n; i++) iters[i] = ss[i]->res.iterations;
   return 0;
 }
@@ -869,6 +916,7 @@ int pus_batch_optimize_many(pus_handle* hs, int n, int* iters) {
 int pus_span_export(pus_handle h, void* out64) {
   NEED(h);
   Solver* s = SV(h);
+  if (refuse_direct_span(s, "pus_span_export") < 0) return -1;
   if (upload(s) < 0) return -1;
   cudaIpcMemHandle_t mh;
   CUDA_OK(cudaIpcGetMemHandle(&mh, s->arena));
@@ -888,6 +936,7 @@ int pus_span_connect(pus_handle h, int rank, int world, const void* handles) {
   NEED(h);
   Solver* s = SV(h);
   if (world < 1 || world > 8 || rank < 0 || rank >= world) { g_err = "pus_span_connect: world must be 1..8"; return -1; }
+  if (refuse_direct_span(s, "pus_span_connect") < 0) return -1;
   if (!s->uploaded || !s->arena) { g_err = "pus_span_connect: call pus_span_export first"; return -1; }
   pus_span_disconnect(h);
   CUDA_OK(cudaSetDevice(s->device));
@@ -912,6 +961,7 @@ static void span_fill(Solver* s, int rank, int world, const std::vector<char*>& 
 int pus_span_optimize(pus_handle h, int* iters) {
   NEED(h);
   Solver* s = SV(h);
+  if (refuse_direct_span(s, "pus_span_optimize") < 0) return -1;
   if (s->span_w <= 1) { g_err = "pus_span_optimize: not connected"; return -1; }
   if (upload(s) < 0) return -1;   // values only: a rebuild would move the arena the peers have mapped
   if (s->span_topo != s->compiled_topo) { g_err = "pus_span_optimize: the graph changed since pus_span_connect; export / connect again"; return -1; }
@@ -925,6 +975,7 @@ int pus_span_optimize(pus_handle h, int* iters) {
 }
 int pus_span_emulate_optimize(pus_handle* hs, int world, int* iters) {
   if (world < 1 || world > 8) { g_err = "pus_span_emulate_optimize: world must be 1..8"; return -1; }
+  for (int i = 0; i < world; i++) if (refuse_direct_span(SV(hs[i]), "pus_span_emulate_optimize") < 0) return -1;
   Solver* s0 = SV(hs[0]);
   if (ensure_device(s0) < 0) return -1;
   BatchStreams bs(hs, world, s0->stream);
@@ -1369,6 +1420,20 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
   if (nm == "blk_grp_ptr") return ints(c.blk_grp_ptr);
   if (nm == "blk_part_ptr") return ints(c.blk_part_ptr);
   if (nm == "blk_ovf") return ints(c.blk_ovf);   // (empty: no pose block over the pose phase's shared-memory limits)
+  // direct mode: the host tables of the assembly of S
+  if (nm == "dinc_pose") return ints(s->dt.inc_pose);
+  if (nm == "dinc_plane") return ints(s->dt.inc_plane);
+  if (nm == "dinc_lo") return ints(s->dt.inc_lo);
+  if (nm == "dinc_hi") return ints(s->dt.inc_hi);
+  if (nm == "dlp_ptr") return ints(s->dt.lp_ptr);
+  if (nm == "dlp_a") return ints(s->dt.lp_a);
+  if (nm == "dlp_b") return ints(s->dt.lp_b);
+  if (nm == "dfp_ptr") return ints(s->dt.fp_ptr);
+  if (nm == "dfp_f") return ints(s->dt.fp_f);
+  if (nm == "pf_i") return ints(c.pf_i);
+  if (nm == "pf_j") return ints(c.pf_j);
+  if (nm == "pl_pose") return ints(c.pl_pose);
+  if (nm == "pl_ptr") return ints(c.pl_ptr);
   if (nm == "dims") {
     double d[12] = {(double)c.N, (double)c.M, (double)c.Epl, (double)c.Epf, (double)c.Elp, (double)c.ntile, (double)c.nblk, (double)c.nc, (double)c.nce, (double)c.ngrp, (double)c.nslot, (double)c.ntile_pl};
     if (cap >= 12) std::memcpy(out, d, sizeof(d));
@@ -1386,6 +1451,27 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
     if (cnt <= cap)
       for (size_t e = 0; e < nt * 32; e++)
         for (int k = 0; k < 18; k++) out[e * 18 + k] = tmp[(e >> 5) * kWStride + k * 32 + (e & 31)];
+    return cnt;
+  }
+  if (nm == "Sdir" || nm == "Ldir") {   // direct mode: S after the assembly (debug stage 4) or L after the factorization, n x n
+    if (s->linear_solver != 1) { g_err = "not in direct linear-solver mode"; return -1; }
+    const int nb = s->hd.dnb, n = 6 * c.N;
+    const size_t total = (size_t)nb * (nb + 1) / 2 * kAcTile;
+    std::vector<double> tmp(total);
+    if (cudaMemcpy(tmp.data(), s->hd.Sd, total * 8, cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
+    const long long cnt = (long long)n * n;
+    if (cnt <= cap)
+      for (int r = 0; r < n; r++)
+        for (int q = 0; q < n; q++)
+          out[(size_t)r * n + q] = q > r ? 0.0 : tmp[(size_t)((r / 48) * (r / 48 + 1) / 2 + q / 48) * kAcTile + (r % 48) * kAcLd + q % 48];
+    return cnt;
+  }
+  if (nm == "delta") {   // [x (6 N) | dl (3 M)] of the last linear solve
+    const long long cnt = 6ll * c.N + 3ll * c.M;
+    if (cnt <= cap) {
+      if (c.N && cudaMemcpy(out, s->hd.x, (size_t)c.N * 48, cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
+      if (c.M && cudaMemcpy(out + 6 * c.N, s->hd.dl, (size_t)c.M * 24, cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
+    }
     return cnt;
   }
   if (nm == "Acinv") {  // de-tiled: row-major ldm x ldm
@@ -1429,6 +1515,7 @@ int pus_debug_compile(pus_handle h) {
   Solver* s = SV(h);
   std::string err;
   if (!compile_graph(s->g, s->c, err)) { g_err = err; return -1; }
+  if (s->linear_solver == 1 && !build_direct(s->c, s->dt, err)) { g_err = err; return -1; }
   return 0;
 }
 

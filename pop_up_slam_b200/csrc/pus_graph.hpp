@@ -641,4 +641,81 @@ inline bool compile_graph(const Graph& g, Compiled& c, std::string& err) {
   return true;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Tables of the exact direct solve (pus_set_linear_solver(h, 1)), built only for handles in that mode.  The reduced pose
+// system S is assembled entry by entry; for every pose pair a >= b (index a (a + 1) / 2 + b) the host lists what couples
+// the two poses, in a fixed order:
+//   dfp: pose-pose factors, f * 2 + side (side 1: the factor's second pose is a, its block enters transposed), factor order;
+//   dlp: planes seen from both poses, as a pair of (pose, plane) incidences (the coarse assembly's lp lists with P = I),
+//        plane-ascending.  An incidence covers every edge between its pose and plane (a pose that observes a plane twice
+//        has one incidence with two edges), as a range of plane-major slots.
+// ------------------------------------------------------------------------------------------------
+constexpr int kDirectMaxPoses = 640;   // order 3 840: 80 tile columns of 48
+
+struct DirectTables {
+  int nb = 0;   // tile rows of the padded order 48 nb >= 6 N
+  std::vector<int> inc_pose, inc_plane, inc_lo, inc_hi;
+  std::vector<int> lp_ptr, lp_a, lp_b, fp_ptr, fp_f;
+};
+
+inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err) {
+  d = DirectTables();
+  const int N = c.N, M = c.M;
+  if (N > kDirectMaxPoses) {
+    err = "direct linear solver: the graph has " + std::to_string(N) + " live poses; the dense solve handles at most " +
+          std::to_string(kDirectMaxPoses) + " (use the PCG solver, kind 0)";
+    return false;
+  }
+  d.nb = std::max(1, (6 * N + 47) / 48);
+  std::vector<int> inc_ptr(M + 1, 0);
+  for (int l = 0; l < M; l++) {
+    for (int s = c.pl_ptr[l]; s < c.pl_ptr[l + 1];) {
+      int e = s + 1;
+      while (e < c.pl_ptr[l + 1] && c.pl_pose[e] == c.pl_pose[s]) e++;
+      d.inc_pose.push_back(c.pl_pose[s]); d.inc_plane.push_back(l); d.inc_lo.push_back(s); d.inc_hi.push_back(e);
+      s = e;
+    }
+    inc_ptr[l + 1] = (int)d.inc_pose.size();
+  }
+  const size_t np = (size_t)N * (N + 1) / 2;
+  auto pair = [](int a, int b) { return (size_t)a * (a + 1) / 2 + b; };
+  d.lp_ptr.assign(np + 1, 0);
+  for (int pass = 0; pass < 2; pass++) {
+    std::vector<int> fill;
+    if (pass == 1) {
+      for (size_t q = 0; q < np; q++) d.lp_ptr[q + 1] += d.lp_ptr[q];
+      d.lp_a.assign(std::max(1, d.lp_ptr[np]), 0);
+      d.lp_b.assign(std::max(1, d.lp_ptr[np]), 0);
+      fill.assign(d.lp_ptr.begin(), d.lp_ptr.end() - 1);
+    }
+    for (int l = 0; l < M; l++)   // incidences are pose-ascending inside a plane: i >= j gives a >= b
+      for (int i = inc_ptr[l]; i < inc_ptr[l + 1]; i++)
+        for (int j = inc_ptr[l]; j <= i; j++) {
+          const size_t q = pair(d.inc_pose[i], d.inc_pose[j]);
+          if (pass == 0) d.lp_ptr[q + 1]++;
+          else { const int at = fill[q]++; d.lp_a[at] = i; d.lp_b[at] = j; }
+        }
+  }
+  d.fp_ptr.assign(np + 1, 0);
+  for (int pass = 0; pass < 2; pass++) {
+    std::vector<int> fill;
+    if (pass == 1) {
+      for (size_t q = 0; q < np; q++) d.fp_ptr[q + 1] += d.fp_ptr[q];
+      d.fp_f.assign(std::max(1, d.fp_ptr[np]), 0);
+      fill.assign(d.fp_ptr.begin(), d.fp_ptr.end() - 1);
+    }
+    for (int f = 0; f < c.Epf; f++) {
+      if (c.pf_j[f] < 0) continue;
+      for (int side = 0; side < 2; side++) {
+        const int a = side ? c.pf_j[f] : c.pf_i[f], b = side ? c.pf_i[f] : c.pf_j[f];
+        if (a < b) continue;
+        const size_t q = pair(a, b);
+        if (pass == 0) d.fp_ptr[q + 1]++;
+        else d.fp_f[fill[q]++] = f * 2 + side;
+      }
+    }
+  }
+  return true;
+}
+
 }  // namespace pus

@@ -120,6 +120,17 @@ struct DevGraph {
   LmParams prm;
   LmResult* res;
   LmTrace* trace;
+  // exact direct solve (pus::kdirect only; zero / null for PCG handles): the reduced system of order 48 dnb as the lower
+  // triangle of 48x48 tiles, tile (I, J) at dtile(I, J) = I (I + 1) / 2 + J
+  int dnb, dninc;
+  const int *dinc_plane, *dinc_lo, *dinc_hi;              // (pose, plane) incidences, plane-major: plane-major slot range
+  const int *dlp_ptr, *dlp_a, *dlp_b, *dfp_ptr, *dfp_f;  // per pose pair a >= b: incidence pairs (plane-ascending), factor sides
+  double *Wd, *Yd;       // [dninc][18]: W_al (summed over the pair's edges) and W_al Hll_d^-1
+  double *Sd;            // S, factored in place into L
+  double *Dsnap;         // [2 step parities][dnb] pivot-column snapshots, then [2] P_K = A_KK^-1
+  double *Dinv;          // [dnb] L_KK^-1
+  double *dvec;          // [2][48 dnb] triangular-solve vectors
+  unsigned* dflag;       // set when a pivot is not positive
 };
 
 // The graph descriptor of the solve in progress and the dynamic shared memory, named at namespace scope so that every
@@ -3029,4 +3040,313 @@ struct Phase {
     for (int i = tid_team(); i < G.N * 7; i += nthr_team()) G.pose_lin[i] = ldc(G.pose_trial + i);
     for (int i = tid_team(); i < G.M * 4; i += nthr_team()) G.plane_lin[i] = ldc(G.plane_trial + i);
   }
+
+#ifdef PUS_DIRECT
+  // ================= exact direct solve (DESIGN.md section 5): dense Cholesky of the reduced pose system =================
+  // Every sum below has one order that does not depend on the team: each output entry is written by one thread, and the
+  // tile products of the factorization read the same operands whichever CTA computes them.  No atomics.
+  __device__ __forceinline__ static int dtile(int i, int j) { return i * (i + 1) / 2 + j; }
+  template <typename T>
+  __device__ __forceinline__ static T* tile_at(T* base, int t) { return base + (size_t)t * kAcTile; }
+
+  // W_al = sum of the (pose a, plane l) edges' W blocks in slot order, Y_al = W_al Hll_d^-1
+  __device__ void direct_wy() {
+    for (int q = tid_team(); q < G.dninc; q += nthr_team()) {
+      const int l = G.dinc_plane[q];
+      double w[18];
+      for (int k = 0; k < 18; k++) w[k] = 0.0;
+      for (int s = G.dinc_lo[q]; s < G.dinc_hi[q]; s++)
+        for (int k = 0; k < 18; k++) w[k] += ldc(G.Wt + (size_t)(s >> 5) * kWStride + k * 32 + (s & 31));
+      double Hi[9];
+      for (int t = 0; t < 9; t++) Hi[t] = ldc(G.Hinv + (size_t)l * 9 + t);
+      for (int r = 0; r < 6; r++)
+        for (int m = 0; m < 3; m++) {
+          G.Wd[(size_t)q * 18 + r * 3 + m] = w[r * 3 + m];
+          G.Yd[(size_t)q * 18 + r * 3 + m] = w[r * 3] * Hi[m] + w[r * 3 + 1] * Hi[3 + m] + w[r * 3 + 2] * Hi[6 + m];
+        }
+    }
+  }
+
+  // S = Hpp_d + (pose-pose blocks) - sum_l Y_al W_bl^T, entry by entry (output-stationary): the diagonal block, then the
+  // pose-pose factor blocks in factor order, then the plane products in plane order.  Upper halves of diagonal tiles are 0,
+  // the padding is identity.  Tile column 0 also goes to the step-0 pivot-column snapshot.
+  __device__ void direct_assemble(double lambda) {
+    const int nb = G.dnb, n6 = 6 * G.N;
+    const long long total = (long long)nb * (nb + 1) / 2 * 2304;
+    int tprev = -1, ti = 0, tj = 0;
+    for (long long idx = tid_team(); idx < total; idx += nthr_team()) {
+      const int t = (int)(idx / 2304), e = (int)(idx - (long long)t * 2304), er = e / 48, ec = e - er * 48;
+      if (t != tprev) {
+        ti = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+        while (ti * (ti + 1) / 2 > t) ti--;
+        while ((ti + 1) * (ti + 2) / 2 <= t) ti++;
+        tj = t - ti * (ti + 1) / 2;
+        tprev = t;
+      }
+      const int i = 48 * ti + er, j = 48 * tj + ec;
+      double v = 0.0;
+      if (j > i) {
+        v = 0.0;
+      } else if (i >= n6) {
+        v = (i == j) ? 1.0 : 0.0;
+      } else {
+        const int a = i / 6, r = i - a * 6, b = j / 6, cc = j - b * 6;
+        if (a == b) {
+          v = ldc(G.Hpp + (size_t)a * 36 + r * 6 + cc);
+          if (r == cc) v *= (1 + lambda);   // Cholesky.cpp:91-97
+        }
+        const size_t q = (size_t)a * (a + 1) / 2 + b;
+        for (int k = G.dfp_ptr[q]; k < G.dfp_ptr[q + 1]; k++) {
+          const int fs = G.dfp_f[k], f = fs >> 1;
+          v += (fs & 1) ? ldc(G.PF + (size_t)f * 120 + 72 + cc * 6 + r) : ldc(G.PF + (size_t)f * 120 + 72 + r * 6 + cc);
+        }
+        for (int k = G.dlp_ptr[q]; k < G.dlp_ptr[q + 1]; k++) {
+          const double* y = G.Yd + (size_t)G.dlp_a[k] * 18 + r * 3;
+          const double* w = G.Wd + (size_t)G.dlp_b[k] * 18 + cc * 3;
+          v -= ldc(y) * ldc(w) + ldc(y + 1) * ldc(w + 1) + ldc(y + 2) * ldc(w + 2);
+        }
+      }
+      tile_at(G.Sd, t)[er * kAcLd + ec] = v;
+      if (tj == 0) tile_at(G.Dsnap, ti)[er * kAcLd + ec] = v;
+    }
+  }
+
+  // one CTA: A (48x48, lower half read) <- L = chol(A) with a zero upper half, Li <- L^-1, P <- Li^T Li = A^-1.
+  // Returns false when a pivot is not positive (the outputs are then meaningless).
+  __device__ bool chol48(double* A, double* Li, double* P) {
+    const int tid = threadIdx.x;
+    bool ok = true;
+    for (int k = 0; k < 48; k++) {
+      __syncthreads();
+      const double d = A[k * kAcLd + k];
+      ok = ok && (d > 0.0);
+      const double s = (d > 0.0) ? sqrt(d) : 1.0;
+      __syncthreads();
+      if (tid >= k && tid < 48) A[tid * kAcLd + k] = (tid == k) ? s : A[tid * kAcLd + k] / s;
+      __syncthreads();
+      for (int e = tid; e < 48 * 48; e += kThreads) {
+        const int i = e / 48, j = e - i * 48;
+        if (j > k && i >= j) A[i * kAcLd + j] -= A[i * kAcLd + k] * A[j * kAcLd + k];
+      }
+    }
+    __syncthreads();
+    for (int e = tid; e < 48 * 48; e += kThreads) {
+      const int i = e / 48, j = e - i * 48;
+      if (j > i) A[i * kAcLd + j] = 0.0;
+    }
+    if (tid < 48) {   // column tid of L^-1 by forward substitution
+      const int cl = tid;
+      for (int i = 0; i < 48; i++) {
+        double v = 0.0;
+        if (i >= cl) {
+          v = (i == cl) ? 1.0 : 0.0;
+          for (int m = cl; m < i; m++) v -= A[i * kAcLd + m] * Li[m * kAcLd + cl];
+          v /= A[i * kAcLd + i];
+        }
+        Li[i * kAcLd + cl] = v;
+      }
+    }
+    __syncthreads();
+    for (int e = tid; e < 48 * 48; e += kThreads) {
+      const int r = e / 48, cl = e - r * 48;
+      double v = 0.0;
+      for (int m = max(r, cl); m < 48; m++) v += Li[m * kAcLd + r] * Li[m * kAcLd + cl];
+      P[r * kAcLd + cl] = v;
+    }
+    __syncthreads();
+    return ok;
+  }
+
+  __device__ void load_tile(double* dst, const double* src) {
+    for (int e = threadIdx.x; e < 48 * 48; e += kThreads) dst[(e / 48) * kAcLd + e % 48] = ldc(src + (e / 48) * kAcLd + e % 48);
+  }
+  __device__ void store_tile(double* dst, const double* src) {
+    for (int e = threadIdx.x; e < 48 * 48; e += kThreads) dst[(e / 48) * kAcLd + e % 48] = src[(e / 48) * kAcLd + e % 48];
+  }
+
+  // S = L L^T in place, right-looking by tile columns, one team barrier per step.  Tile t belongs to CTA t % tsize.  Step K
+  // reads pivot column K only from its snapshot (published by the owners of those tiles at the end of step K-1, double-
+  // buffered by step parity), so the owners may overwrite it with L in the same step:
+  //   panel     L_iK = C_i L_KK^-T
+  //   trailing  A_ij <- A_ij + T_i C_j^T,  T_i = -C_i P_K  (P_K = A_KK^-1 = L_KK^-T L_KK^-1),  K < j <= i
+  // on the FP64 tensor cores.  Look-ahead: the owner of tile (K+1, K+1) updates it first, factors it and publishes L_{K+1}^-1
+  // and P_{K+1}; step 0's pivot is factored by every CTA from the snapshot.
+  __device__ void direct_factor() {
+    const int nb = G.dnb, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3;
+    double* Ps = reinterpret_cast<double*>(g_smem + kSmWork);
+    double* Li = Ps + kAcTile;
+    double* Ci = Li + kAcTile;
+    double* Ti = Ci + kAcTile;
+    double* Cj = Ti + kAcTile;
+    double* Md = Cj + kAcTile;
+    double* Pn = Md + kAcTile;
+    double* piv = G.Dsnap + (size_t)2 * nb * kAcTile;
+    const int T = c.tsize;
+    auto frag = [&](int s, int& r, int& cc) {
+      const int q = warp + 16 * s;
+      r = 8 * (q / 6) + fr;
+      cc = 8 * (q % 6) + 2 * fc;
+      return q < 36;
+    };
+    auto form_T = [&]() {   // Ti = -Ci Ps
+      double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+      mma48<false>(acc, Ci, Ps);
+      int r, cc;
+#pragma unroll
+      for (int s = 0; s < 3; s++)
+        if (frag(s, r, cc)) *reinterpret_cast<double2*>(Ti + r * kAcLd + cc) = make_double2(-acc[s][0], -acc[s][1]);
+    };
+    auto update = [&](int i, int j, double (&acc)[3][2]) {   // acc = A_ij + Ti C_j^T (Cj loaded)
+      const double* tile = tile_at(G.Sd, dtile(i, j));
+      int r, cc;
+#pragma unroll
+      for (int s = 0; s < 3; s++)
+        if (frag(s, r, cc)) {
+          const double2 v = __ldcg(reinterpret_cast<const double2*>(tile + r * kAcLd + cc));
+          acc[s][0] = v.x; acc[s][1] = v.y;
+        }
+      mma48<true>(acc, Ti, Cj);
+    };
+    auto factor_pivot = [&](int d, bool publish) {   // Md holds A_dd: L_dd into the store, L_dd^-1 and P_d out
+      const bool ok = chol48(Md, Li, Pn);
+      if (!ok && tid == 0) *G.dflag = 1u;
+      if (publish) {
+        store_tile(tile_at(G.Sd, dtile(d, d)), Md);
+        store_tile(tile_at(G.Dinv, d), Li);
+        store_tile(tile_at(piv, d & 1), Pn);
+      }
+    };
+
+    for (int K = 0; K < nb; K++) {
+      const double* snap = G.Dsnap + (size_t)(K & 1) * nb * kAcTile;
+      double* snapn = G.Dsnap + (size_t)((K + 1) & 1) * nb * kAcTile;
+      if (K == 0) {
+        load_tile(Md, snap);
+        factor_pivot(0, c.rank == 0);
+        store_tile(Ps, Pn);
+      } else {
+        load_tile(Ps, tile_at(piv, K & 1));
+        load_tile(Li, tile_at(G.Dinv, K));
+      }
+      __syncthreads();
+      const int d = K + 1;
+      int trow = -1, trowT = -1;   // tile rows whose C_i / T_i are in shared memory (T_i only once an owned trailing tile needs it)
+      if (d < nb && dtile(d, d) % T == c.rank) {   // look-ahead
+        load_tile(Ci, tile_at(snap, d));
+        __syncthreads();
+        form_T();
+        store_tile(Cj, Ci);
+        __syncthreads();
+        double acc[3][2];
+        update(d, d, acc);
+        int r, cc;
+#pragma unroll
+        for (int s = 0; s < 3; s++)
+          if (frag(s, r, cc)) *reinterpret_cast<double2*>(Md + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+        // (Li of step K is needed below for the panel: factor into Pn / a copy of Li, then restore)
+        __syncthreads();
+        double* Lsave = Cj;
+        store_tile(Lsave, Li);
+        __syncthreads();
+        factor_pivot(d, true);
+        __syncthreads();
+        store_tile(Li, Lsave);
+        __syncthreads();
+        trow = trowT = d;
+      }
+      for (int i = K; i < nb; i++) {
+        const int t0 = dtile(i, K);
+        int j = K + ((c.rank - t0 % T) % T + T) % T;
+        for (; j <= i; j += T) {
+          if (j == K && i == K) continue;                // the pivot: factored already
+          if (i == d && j == d) continue;                // done by the look-ahead
+          if (trow != i) {
+            __syncthreads();
+            load_tile(Ci, tile_at(snap, i));
+            __syncthreads();
+            trow = i;
+          }
+          if (j != K && trowT != i) {   // (read after the barrier that precedes the C_j load below)
+            form_T();
+            trowT = i;
+          }
+          double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+          int r, cc;
+          if (j == K) {   // panel: L_iK = C_i L_KK^-T
+            mma48<true>(acc, Ci, Li);
+#pragma unroll
+            for (int s = 0; s < 3; s++)
+              if (frag(s, r, cc))
+                *reinterpret_cast<double2*>(tile_at(G.Sd, t0) + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+            continue;
+          }
+          __syncthreads();
+          load_tile(Cj, tile_at(snap, j));
+          __syncthreads();
+          update(i, j, acc);
+#pragma unroll
+          for (int s = 0; s < 3; s++) {
+            if (!frag(s, r, cc)) continue;
+            *reinterpret_cast<double2*>(tile_at(G.Sd, dtile(i, j)) + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+            if (j == d) *reinterpret_cast<double2*>(tile_at(snapn, i) + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+          }
+        }
+      }
+      __syncthreads();
+      team_barrier(c);
+    }
+  }
+
+  // L y = b, then L^T x = y, blocked by tile row with the stored L_KK^-1; one team barrier per tile row.  Every CTA forms
+  // y_K (x_K) itself from the finished part of the vector, then the team subtracts its contribution from the rows still open
+  // (each entry by one thread, in step order).  dvec[0] = the running right-hand side / x, dvec[1] = y.
+  __device__ void direct_trsv() {
+    const int nb = G.dnb, n = 48 * nb, n6 = 6 * G.N, tid = threadIdx.x;
+    double* rv = G.dvec;
+    double* yv = G.dvec + n;
+    double* sv = reinterpret_cast<double*>(g_smem + kSmWork);   // [48] the vector piece of this step, [48] its product
+    for (int i = tid_team(); i < n; i += nthr_team()) rv[i] = (i < n6) ? ldc(G.b + i) : 0.0;
+    team_barrier(c);
+    for (int K = 0; K < nb; K++) {   // forward: y_K = L_KK^-1 r_K;  r_J -= L_JK y_K  (J > K)
+      const double* Li = tile_at(G.Dinv, K);
+      if (tid < 48) sv[tid] = ldc(rv + 48 * K + tid);
+      __syncthreads();
+      if (tid < 48) {
+        double v = 0.0;
+        for (int m = 0; m <= tid; m++) v += ldc(Li + tid * kAcLd + m) * sv[m];
+        sv[48 + tid] = v;
+        if (c.rank == 0) yv[48 * K + tid] = v;
+      }
+      __syncthreads();
+      for (int row = 48 * (K + 1) + tid_team(); row < n; row += nthr_team()) {
+        const double* Lr = tile_at(G.Sd, dtile(row / 48, K)) + (row % 48) * kAcLd;
+        double v = ldc(rv + row);
+        for (int m = 0; m < 48; m++) v -= ldc(Lr + m) * sv[48 + m];
+        rv[row] = v;
+      }
+      __syncthreads();
+      team_barrier(c);
+    }
+    for (int K = nb - 1; K >= 0; K--) {   // backward: x_K = L_KK^-T y_K;  y_J -= L_KJ^T x_K  (J < K)
+      const double* Li = tile_at(G.Dinv, K);
+      if (tid < 48) sv[tid] = ldc(yv + 48 * K + tid);
+      __syncthreads();
+      if (tid < 48) {
+        double v = 0.0;
+        for (int m = tid; m < 48; m++) v += ldc(Li + m * kAcLd + tid) * sv[m];
+        sv[48 + tid] = v;
+        if (c.rank == 0) rv[48 * K + tid] = v;
+      }
+      __syncthreads();
+      for (int row = tid_team(); row < 48 * K; row += nthr_team()) {
+        const double* Lc = tile_at(G.Sd, dtile(K, row / 48)) + (row % 48);
+        double v = ldc(yv + row);
+        for (int m = 0; m < 48; m++) v -= ldc(Lc + m * kAcLd) * sv[48 + m];
+        yv[row] = v;
+      }
+      __syncthreads();
+      team_barrier(c);
+    }
+  }
+#endif
 };
