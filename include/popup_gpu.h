@@ -312,8 +312,15 @@ int pus_load_isam_dataset(pus_handle h, const char* path, int* n_poses, int* n_f
 long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long capacity);
 /* run single stages on the uploaded graph: 0 linearise at the current linpoint (fills Hpp..W),
  * 1 build Schur preconditioner for `lambda`, 2 one solve for `lambda` (fills "delta"),
- * 3 y = S*x for the vector previously stored with pus_debug_store("x") */
+ * 3 y = S*x for the vector previously stored with pus_debug_store("x").
+ * Direct linear-solver mode only: 4 stop after the assembly of S ("Sdir"), 1 also factors it ("Ldir");
+ * 5 factors the S stored with pus_debug_store("Sdir") (no linearisation, `lambda` unused) and, unless a pivot is not
+ * positive, solves S x = b for the vector stored with pus_debug_store("b"), leaving x in "x".  pus_debug_fetch("dflag")
+ * returns one value: 1 when the last factorization met a non-positive pivot, else 0.  Stage 5 is refused for a PCG handle. */
 int pus_debug_run_stage(pus_handle h, int stage, double lambda);
+/* copy host doubles into a named device buffer; "Sdir" (direct mode, after pus_upload) takes a dense row-major (6 N)^2
+ * matrix, of which the lower triangle is laid out as the assembly lays out S (padding rows are identity); it refuses
+ * any other element count */
 long long pus_debug_store(pus_handle h, const char* name, const double* in, long long count);
 
 #ifdef __cplusplus

@@ -229,6 +229,19 @@ __device__ void run_graph_impl(Ctx& c) {
       team_barrier(c);
       return;
     }
+#ifdef PUS_DIRECT
+    if (P.debug_stage == 5) {  // factor the S stored with pus_debug_store("Sdir"), then x = S^-1 b for the stored b
+      if (lead) *G.dflag = 0u;
+      team_barrier(c);
+      ph.direct_factor();
+      if (__ldcg(G.dflag) == 0u) {
+        ph.direct_trsv();
+        for (int i = ph.tid_team(); i < G.N * 6; i += ph.nthr_team()) G.x[i] = ldc(G.dvec + i);
+        team_barrier(c);
+      }
+      return;
+    }
+#endif
     linearize(ph, c);
     if (lead) res->relin = 1;
     if (P.debug_stage >= 1) {

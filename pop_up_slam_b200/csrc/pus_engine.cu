@@ -298,7 +298,7 @@ static int upload(Solver* s) {
       UPD(dlp_ptr, dt.lp_ptr); UPD(dlp_a, dt.lp_a); UPD(dlp_b, dt.lp_b); UPD(dfp_ptr, dt.fp_ptr); UPD(dfp_f, dt.fp_f);
 #undef UPD
       AL(Wd, ninc * 18, "Wd"); AL(Yd, ninc * 18, "Yd");
-      AL(Sd, nb * (nb + 1) / 2 * kAcTile, nullptr); AL(Dsnap, (2 * nb + 2) * kAcTile, nullptr); AL(Dinv, nb * kAcTile, nullptr);
+      AL(Sd, nb * (nb + 1) / 2 * kAcTile, nullptr); AL(Dsnap, 2 * nb * kAcTile, nullptr); AL(Dinv, nb * kAcTile, nullptr);
       AL(dvec, 2 * 48 * nb, nullptr);
       if (s->dalloc(&d.dflag, 1) < 0) return -1;
     }
@@ -1466,6 +1466,13 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
           out[(size_t)r * n + q] = q > r ? 0.0 : tmp[(size_t)((r / 48) * (r / 48 + 1) / 2 + q / 48) * kAcTile + (r % 48) * kAcLd + q % 48];
     return cnt;
   }
+  if (nm == "dflag") {   // direct mode: 1 when the last factorization met a non-positive pivot, else 0
+    if (s->linear_solver != 1) { g_err = "not in direct linear-solver mode"; return -1; }
+    unsigned f = 0;
+    if (cudaMemcpy(&f, s->hd.dflag, sizeof(f), cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
+    if (cap >= 1) out[0] = f ? 1.0 : 0.0;
+    return 1;
+  }
   if (nm == "delta") {   // [x (6 N) | dl (3 M)] of the last linear solve
     const long long cnt = 6ll * c.N + 3ll * c.M;
     if (cnt <= cap) {
@@ -1496,6 +1503,27 @@ long long pus_debug_store(pus_handle h, const char* name, const double* in, long
   NEED(h);
   Solver* s = SV(h);
   cudaSetDevice(s->device);
+  if (std::string(name) == "Sdir") {   // direct mode: a dense row-major S (n x n) for debug stage 5, laid out as direct_assemble does
+    if (s->linear_solver != 1) { g_err = "Sdir: not in direct linear-solver mode"; return -1; }
+    if (!s->uploaded) { g_err = "Sdir: call pus_upload first"; return -1; }
+    const int nb = s->hd.dnb, n = 6 * s->c.N;
+    if (count != (long long)n * n) { g_err = "Sdir: expected (6 N)^2 = " + std::to_string((long long)n * n) + " elements"; return -1; }
+    std::vector<double> tiles((size_t)nb * (nb + 1) / 2 * kAcTile, 0.0);
+    for (int ti = 0; ti < nb; ti++)
+      for (int tj = 0; tj <= ti; tj++) {
+        double* t = tiles.data() + (size_t)(ti * (ti + 1) / 2 + tj) * kAcTile;
+        for (int er = 0; er < 48; er++)
+          for (int ec = 0; ec < 48; ec++) {
+            const int i = 48 * ti + er, j = 48 * tj + ec;
+            t[er * kAcLd + ec] = j > i ? 0.0 : (i >= n ? (i == j ? 1.0 : 0.0) : in[(size_t)i * n + j]);   // lower half, identity padding
+          }
+      }
+    if (cudaMemcpy(s->hd.Sd, tiles.data(), tiles.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) { g_err = "memcpy"; return -1; }
+    for (int ti = 0; ti < nb; ti++)   // tile column 0 is also the step-0 pivot-column snapshot (parity 0)
+      if (cudaMemcpy(s->hd.Dsnap + (size_t)ti * kAcTile, tiles.data() + (size_t)(ti * (ti + 1) / 2) * kAcTile, kAcTile * 8,
+                     cudaMemcpyHostToDevice) != cudaSuccess) { g_err = "memcpy"; return -1; }
+    return count;
+  }
   auto it = s->named.find(name);
   if (it == s->named.end()) { g_err = std::string("unknown buffer ") + name; return -1; }
   if (count > (long long)it->second.second) { g_err = "too many elements"; return -1; }
@@ -1506,6 +1534,7 @@ int pus_debug_run_stage(pus_handle h, int stage, double lambda) {
   NEED(h);
   Solver* s = SV(h);
   if (!s->uploaded) { g_err = "call pus_upload first"; return -1; }
+  if (stage == 5 && s->linear_solver != 1) { g_err = "debug stage 5 factors a stored Sdir: direct linear-solver mode only"; return -1; }
   return launch(&s, 1, MODE_DEBUG, 0, stage, lambda);
 }
 

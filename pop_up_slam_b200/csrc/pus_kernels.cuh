@@ -127,7 +127,7 @@ struct DevGraph {
   const int *dlp_ptr, *dlp_a, *dlp_b, *dfp_ptr, *dfp_f;  // per pose pair a >= b: incidence pairs (plane-ascending), factor sides
   double *Wd, *Yd;       // [dninc][18]: W_al (summed over the pair's edges) and W_al Hll_d^-1
   double *Sd;            // S, factored in place into L
-  double *Dsnap;         // [2 step parities][dnb] pivot-column snapshots, then [2] P_K = A_KK^-1
+  double *Dsnap;         // [2 step parities][dnb] pivot-column snapshots
   double *Dinv;          // [dnb] L_KK^-1
   double *dvec;          // [2][48 dnb] triangular-solve vectors
   unsigned* dflag;       // set when a pivot is not positive
@@ -3111,9 +3111,9 @@ struct Phase {
     }
   }
 
-  // one CTA: A (48x48, lower half read) <- L = chol(A) with a zero upper half, Li <- L^-1, P <- Li^T Li = A^-1.
+  // one CTA: A (48x48, lower half read) <- L = chol(A) with a zero upper half, Li <- L^-1.
   // Returns false when a pivot is not positive (the outputs are then meaningless).
-  __device__ bool chol48(double* A, double* Li, double* P) {
+  __device__ bool chol48(double* A, double* Li) {
     const int tid = threadIdx.x;
     bool ok = true;
     for (int k = 0; k < 48; k++) {
@@ -3147,13 +3147,6 @@ struct Phase {
       }
     }
     __syncthreads();
-    for (int e = tid; e < 48 * 48; e += kThreads) {
-      const int r = e / 48, cl = e - r * 48;
-      double v = 0.0;
-      for (int m = max(r, cl); m < 48; m++) v += Li[m * kAcLd + r] * Li[m * kAcLd + cl];
-      P[r * kAcLd + cl] = v;
-    }
-    __syncthreads();
     return ok;
   }
 
@@ -3168,19 +3161,19 @@ struct Phase {
   // reads pivot column K only from its snapshot (published by the owners of those tiles at the end of step K-1, double-
   // buffered by step parity), so the owners may overwrite it with L in the same step:
   //   panel     L_iK = C_i L_KK^-T
-  //   trailing  A_ij <- A_ij + T_i C_j^T,  T_i = -C_i P_K  (P_K = A_KK^-1 = L_KK^-T L_KK^-1),  K < j <= i
-  // on the FP64 tensor cores.  Look-ahead: the owner of tile (K+1, K+1) updates it first, factors it and publishes L_{K+1}^-1
-  // and P_{K+1}; step 0's pivot is factored by every CTA from the snapshot.
+  //   trailing  A_ij <- A_ij - L_iK L_jK^T,  K < j <= i
+  // on the FP64 tensor cores.  A CTA forms -L_iK once per tile row in which it owns a trailing tile and L_jK for every such
+  // tile; each product reads only L_KK^-1 and snapshot tiles, so every CTA that forms it gets the same bits.  (A trailing
+  // update through A_KK^-1 or L_KK^-1 alone, with one product per tile, loses backward stability when A_KK is ill-conditioned:
+  // DESIGN.md section 5.1.)  Look-ahead: the owner of tile (K+1, K+1) updates it first, factors it and publishes L_{K+1}^-1;
+  // step 0's pivot is factored by every CTA from the snapshot.
   __device__ void direct_factor() {
     const int nb = G.dnb, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3;
-    double* Ps = reinterpret_cast<double*>(g_smem + kSmWork);
-    double* Li = Ps + kAcTile;
+    double* Li = reinterpret_cast<double*>(g_smem + kSmWork);
     double* Ci = Li + kAcTile;
     double* Ti = Ci + kAcTile;
     double* Cj = Ti + kAcTile;
     double* Md = Cj + kAcTile;
-    double* Pn = Md + kAcTile;
-    double* piv = G.Dsnap + (size_t)2 * nb * kAcTile;
     const int T = c.tsize;
     auto frag = [&](int s, int& r, int& cc) {
       const int q = warp + 16 * s;
@@ -3188,17 +3181,26 @@ struct Phase {
       cc = 8 * (q % 6) + 2 * fc;
       return q < 36;
     };
-    auto form_T = [&]() {   // Ti = -Ci Ps
+    auto form_T = [&]() {   // Ti = -L_iK = -(Ci Li^T)
       double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
-      mma48<false>(acc, Ci, Ps);
+      mma48<true>(acc, Ci, Li);
       int r, cc;
 #pragma unroll
       for (int s = 0; s < 3; s++)
         if (frag(s, r, cc)) *reinterpret_cast<double2*>(Ti + r * kAcLd + cc) = make_double2(-acc[s][0], -acc[s][1]);
     };
-    auto update = [&](int i, int j, double (&acc)[3][2]) {   // acc = A_ij + Ti C_j^T (Cj loaded)
-      const double* tile = tile_at(G.Sd, dtile(i, j));
+    auto update = [&](int i, int j, double (&acc)[3][2]) {   // Cj (loaded) <- L_jK = Cj Li^T, then acc = A_ij + Ti L_jK^T
       int r, cc;
+      {
+        double l[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+        mma48<true>(l, Cj, Li);
+        __syncthreads();
+#pragma unroll
+        for (int s = 0; s < 3; s++)
+          if (frag(s, r, cc)) *reinterpret_cast<double2*>(Cj + r * kAcLd + cc) = make_double2(l[s][0], l[s][1]);
+        __syncthreads();
+      }
+      const double* tile = tile_at(G.Sd, dtile(i, j));
 #pragma unroll
       for (int s = 0; s < 3; s++)
         if (frag(s, r, cc)) {
@@ -3207,13 +3209,12 @@ struct Phase {
         }
       mma48<true>(acc, Ti, Cj);
     };
-    auto factor_pivot = [&](int d, bool publish) {   // Md holds A_dd: L_dd into the store, L_dd^-1 and P_d out
-      const bool ok = chol48(Md, Li, Pn);
+    auto factor_pivot = [&](int d, bool publish) {   // Md holds A_dd: L_dd into the store, L_dd^-1 out
+      const bool ok = chol48(Md, Li);
       if (!ok && tid == 0) *G.dflag = 1u;
       if (publish) {
         store_tile(tile_at(G.Sd, dtile(d, d)), Md);
         store_tile(tile_at(G.Dinv, d), Li);
-        store_tile(tile_at(piv, d & 1), Pn);
       }
     };
 
@@ -3223,9 +3224,7 @@ struct Phase {
       if (K == 0) {
         load_tile(Md, snap);
         factor_pivot(0, c.rank == 0);
-        store_tile(Ps, Pn);
       } else {
-        load_tile(Ps, tile_at(piv, K & 1));
         load_tile(Li, tile_at(G.Dinv, K));
       }
       __syncthreads();
@@ -3243,7 +3242,7 @@ struct Phase {
 #pragma unroll
         for (int s = 0; s < 3; s++)
           if (frag(s, r, cc)) *reinterpret_cast<double2*>(Md + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
-        // (Li of step K is needed below for the panel: factor into Pn / a copy of Li, then restore)
+        // (Li of step K is needed below for the panel and T_i: keep a copy of it, then restore)
         __syncthreads();
         double* Lsave = Cj;
         store_tile(Lsave, Li);
