@@ -45,9 +45,13 @@ typedef Eigen::Matrix4d Matrix4d;
 typedef Eigen::Vector3d Vector3d;
 typedef Eigen::Vector4d Vector4d;
 typedef Eigen::Matrix<double, 6, 1> Vector6d;
+typedef Eigen::VectorXd VectorXd;
+inline VectorXd to_vectorxd(const std::vector<double>& v) { VectorXd x((int)v.size()); for (size_t i = 0; i < v.size(); i++) x((int)i) = v[i]; return x; }
 inline double mget(const MatrixXd& m, int r, int c) { return m(r, c); }
 inline int mrows(const MatrixXd& m) { return (int)m.rows(); }
 #else
+typedef std::vector<double> VectorXd;   // Slam::weighted_errors / Factor::error in the Eigen-free flavour
+inline VectorXd to_vectorxd(const std::vector<double>& v) { return v; }
 struct MatrixXd {
   int r = 0, c = 0;
   std::vector<double> a;
@@ -334,6 +338,13 @@ class Factor {
   std::vector<Node*>& nodes() { return _nodes; }          // Factor.h:79
   const Noise& noise() const { return _noise; }           // Factor.h:204
   virtual int _attach(pus_handle h) = 0;                  // issues the pus_add_* call
+  VectorXd error() const {                                // Factor.h:67-77 at the estimate, evaluated on the device
+    std::vector<double> e(6);
+    const int n = pus_factor_errors(_h, 1, &_id, e.data());
+    if (n < 0) throw std::runtime_error(std::string("Factor::error: ") + pus_last_error());
+    e.resize(n);
+    return to_vectorxd(e);
+  }
 };
 
 template <class T> class FactorT : public Factor {
@@ -422,6 +433,15 @@ class Pose3d_Plane3d_Factor2 : public Pose3d_Plane3d_Factor {
   }
 };
 
+// Slam::jacobian() of the façade: iSAM returns a SparseSystem (ISAM/include/isam/SparseSystem.h), which the façade does not
+// provide; this struct carries the same matrix as CSR (rows in factor order, columns in node order, ascending columns within
+// a row, zeros stored) and rhs = Jacobian::rhs() = minus the residual rows.
+struct SparseJacobian {
+  long long rows = 0, cols = 0;
+  std::vector<int> row_ptr, col_idx;   // [rows + 1], [nnz]
+  std::vector<double> values, rhs;     // [nnz], [rows]
+};
+
 // robust costs (ISAM/include/isam/robust.h:101-118); Slam::set_cost_function takes these tags
 struct cost_func_t { int kind; double b; };
 inline cost_func_t cost_huber_tag(double b) { return cost_func_t{1, b}; }
@@ -489,6 +509,23 @@ class Slam {
     s.step = ++_step; return s;
   }
   double chi2() { double c = 0; detail::check(pus_chi2(_h, &c)); return c; }       // Slam.cpp:266-268
+  // the error / Jacobian export at the current estimate (evaluated on the device; see pus_weighted_errors .. pus_local_chi2)
+  VectorXd weighted_errors() {                                                      // Slam.cpp:254-264
+    const long long rows = pus_weighted_errors(_h, nullptr, 0); detail::check((int)(rows < 0 ? -1 : 0));
+    std::vector<double> e((size_t)rows);
+    detail::check((int)(pus_weighted_errors(_h, e.data(), rows) < 0 ? -1 : 0));
+    return to_vectorxd(e);
+  }
+  double normalized_chi2() { double c = 0; detail::check(pus_normalized_chi2(_h, &c)); return c; }                 // Slam.cpp:287-289
+  double local_chi2(int last_n) { double c = 0; detail::check(pus_local_chi2(_h, last_n, &c)); return c; }       // Slam.cpp:270-285
+  SparseJacobian jacobian() {                                                       // Slam.cpp:379-432
+    SparseJacobian J;
+    detail::check(pus_jacobian_dims(_h, &J.rows, &J.cols));
+    const long long nnz = pus_jacobian(_h, nullptr, nullptr, nullptr, nullptr, 0); detail::check((int)(nnz < 0 ? -1 : 0));
+    J.row_ptr.resize((size_t)J.rows + 1); J.col_idx.resize((size_t)nnz); J.values.resize((size_t)nnz); J.rhs.resize((size_t)J.rows);
+    detail::check((int)(pus_jacobian(_h, J.row_ptr.data(), J.col_idx.data(), J.values.data(), J.rhs.data(), nnz) < 0 ? -1 : 0));
+    return J;
+  }
   void save(const std::string& fname) const { detail::check(pus_save_graph(_h, fname.c_str(), 0)); }   // Slam.cpp:84-89
 
   // ---- not in iSAM: the two per-solve loops of Mapper_mono that otherwise round-trip through the host ----

@@ -32,6 +32,9 @@
  *   - the direct linear solver (pus_set_linear_solver(h, 1)) handles at most 640 live poses (a dense reduced system of
  *     order 3 840, about 65 MB of device memory); a larger graph fails at upload with a message and launches nothing.
  *     It does not span ranks: the pus_span_* entry points refuse a direct-mode handle.
+ *   - the error / Jacobian export (pus_weighted_errors .. pus_local_chi2) evaluates at the estimate only (iSAM's default
+ *     Selector ESTIMATE; LINPOINT is not provided) and writes caller-owned host arrays only.  Its indices are int32: a
+ *     graph whose Jacobian has more than 2^31 - 1 nonzeros is refused with a message.
  */
 #ifndef POPUP_GPU_H
 #define POPUP_GPU_H
@@ -271,6 +274,43 @@ int pus_refresh_run(pus_handle h, double* new_meas);
  * applies it to every stored polygon vertex (Mapping.cpp:609-632): pts_out[i] = float(project(double(pts_in[i])))
  * onto the current device-resident estimate of plane node plane_of_point[i]. */
 int pus_project_to_planes(pus_handle h, int n_points, const int* plane_of_point, const float* pts_in, float* pts_out);
+
+/* ---- weighted errors and the stacked Jacobian at the current estimate ---------------------------- */
+/* Evaluated on the device, one thread per live factor, with the residual and Jacobian code the solver linearises with.
+ * Rows follow the factor order and columns the node order of pus_factor_row / pus_node_start (Slam::update_starts
+ * Slam.cpp:59-67, jacobian_partial :395-432).  Each call first re-uploads the graph if its topology, host values or
+ * measurements changed since the last upload, as pus_project_to_planes does; otherwise it reads the device-resident
+ * estimate of the last solve.  The outputs do not depend on the linear solver (PCG and direct handles agree bit for bit)
+ * and repeated calls are bit-identical (no floating-point atomics; the sums below reduce in a fixed order).
+ * A graph without live factors, a bad factor id or too small a capacity fails with a message. */
+/* VectorXd Slam::weighted_errors(ESTIMATE)  Slam.cpp:254-264: Factor::error of every live factor, stacked.  Returns the
+ * number of rows (the sum of the live factors' dims); out = NULL is a size query. */
+long long pus_weighted_errors(pus_handle h, double* out, long long capacity);
+/* VectorXd Factor::error(ESTIMATE)  Factor.h:67-77 of n factors: their rows packed in the order of fids.  Returns the
+ * total number of rows. */
+int pus_factor_errors(pus_handle h, int n, const int* fids, double* out);
+/* SparseSystem::num_rows() / num_cols() of Slam::jacobian(): the sum of the live factors' dims and of the live nodes' dims
+ * (host only). */
+int pus_jacobian_dims(pus_handle h, long long* rows, long long* cols);
+/* SparseSystem Slam::jacobian()  Slam.cpp:379-432 at the current estimate, as CSR: row_ptr [rows + 1], col_idx / values
+ * [nnz], rhs [rows] = Jacobian::rhs() = minus the residual rows (Jacobian.h:97-98).  Within a row the columns ascend and
+ * zeros stay stored ("0-entries not omitted", Slam.cpp:425).  Any output may be NULL; cap_nnz = 0 is a size query.
+ * Returns nnz.  The blocks follow pus_set_jacobian_mode, as the solve does:
+ *   mode 0 (default)  closed forms; they agree with the reference's central differences to its O(eps^2) truncation error
+ *                     (about 1e-8 relative);
+ *   mode 1            the reference's central differences (numericalDiff, eps = 1e-4) through the Euler round trip of the
+ *                     linearisation point, as Factor::jacobian forms them.  rhs is then the residual at the round-tripped
+ *                     point, as upstream (it differs from -pus_weighted_errors in the last bits).
+ *                     This is Slam::jacobian()'s default branch, jacobian_partial.  With force_numerical_jacobian the
+ *                     reference runs jacobian_numerical_columnwise instead, which has the same values but omits exact zeros
+ *                     and returns +residual as its rhs (Slam.cpp:365, 375); the export does not follow that branch.
+ * row_ptr / col_idx depend only on the graph's structure and are built once per layout, on the device. */
+long long pus_jacobian(pus_handle h, int* row_ptr, int* col_idx, double* values, double* rhs, long long cap_nnz);
+/* double Slam::normalized_chi2()  Slam.cpp:287-289: chi2 / (rows - columns) */
+int pus_normalized_chi2(pus_handle h, double* out);
+/* double Slam::local_chi2(int last_n)  Slam.cpp:270-285: the sum of squares of the weighted errors of the last_n most recent
+ * live factors (all of them when last_n exceeds their number; 0 when last_n <= 0) */
+int pus_local_chi2(pus_handle h, int last_n, double* out);
 
 /* ---- one graph spanning several ranks (SURVEY.md 8e, second bullet) --------------------------- */
 /* Every rank holds the whole graph (build it identically on each) and runs its own persistent kernel; the PCG

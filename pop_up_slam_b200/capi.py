@@ -425,6 +425,58 @@ class GpuGraphAPI(GraphAPI):
         fn.argtypes = [C.c_void_p]
         self._chk(fn(self.h))
 
+    # -- weighted errors / stacked Jacobian at the current estimate (evaluated on the device) --
+    def jacobian_dims(self):
+        """(rows, columns) of the stacked system: the live factors' dims and the live nodes' dims."""
+        r, c = C.c_longlong(0), C.c_longlong(0)
+        self._chk(self.lib.pus_jacobian_dims(self.h, C.byref(r), C.byref(c)))
+        return r.value, c.value
+
+    def weighted_errors(self):
+        """Slam::weighted_errors(): Factor::error of every live factor, stacked in factor order (numpy, float64)."""
+        fn = self.lib.pus_weighted_errors
+        fn.restype = C.c_longlong
+        fn.argtypes = [C.c_void_p, c_double_p, C.c_longlong]
+        rows = self._chk(fn(self.h, None, 0))
+        out = np.zeros(rows)
+        self._chk(fn(self.h, _dp(out), rows))
+        return out
+
+    def factor_errors(self, fids):
+        """Factor::error of the given factors, their rows concatenated in the order of fids."""
+        fids = _i32(np.atleast_1d(fids))
+        out = np.zeros(6 * len(fids))
+        fn = self.lib.pus_factor_errors
+        fn.argtypes = [C.c_void_p, C.c_int, c_int_p, c_double_p]
+        n = self._chk(fn(self.h, len(fids), _ip(fids), _dp(out)))
+        return out[:n].copy()
+
+    def jacobian(self):
+        """Slam::jacobian() at the current estimate, in the handle's Jacobian mode: (scipy.sparse.csr_matrix, rhs), with
+        rhs = Jacobian::rhs() = minus the residual rows."""
+        import scipy.sparse as sp
+        fn = self.lib.pus_jacobian
+        fn.restype = C.c_longlong
+        fn.argtypes = [C.c_void_p, c_int_p, c_int_p, c_double_p, c_double_p, C.c_longlong]
+        rows, cols = self.jacobian_dims()
+        nnz = self._chk(fn(self.h, None, None, None, None, 0))
+        row_ptr = np.zeros(rows + 1, dtype=np.int32)
+        col_idx = np.zeros(max(nnz, 1), dtype=np.int32)
+        vals = np.zeros(max(nnz, 1))
+        rhs = np.zeros(rows)
+        self._chk(fn(self.h, _ip(row_ptr), _ip(col_idx), _dp(vals), _dp(rhs), nnz))
+        return sp.csr_matrix((vals[:nnz], col_idx[:nnz], row_ptr), shape=(rows, cols)), rhs
+
+    def normalized_chi2(self):
+        out = C.c_double(0)
+        self._chk(self.lib.pus_normalized_chi2(self.h, C.byref(out)))
+        return out.value
+
+    def local_chi2(self, last_n):
+        out = C.c_double(0)
+        self._chk(self.lib.pus_local_chi2(self.h, int(last_n), C.byref(out)))
+        return out.value
+
     def debug_fetch(self, name, cap):
         out = np.zeros(int(cap))
         n = self.lib.pus_debug_fetch(self.h, name.encode(), _dp(out), C.c_longlong(int(cap)))

@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "../../include/popup_gpu.h"
+#include "pus_export.cuh"
 #include "pus_graph.hpp"
 
 namespace pus {
@@ -91,6 +92,19 @@ struct Solver {
     double* d_out = nullptr;
   } rt;
   bool meas_device_newer = false;        // pus_refresh_run(h, NULL) left newer pose-plane measurements on the device than in the host mirrors
+  // per-layout tables of the error / Jacobian export (pus_export.cuh), built by the first export after a layout rebuild
+  struct ExportTables {
+    uint64_t topo = 0;                    // compiled_topo they were built for (0: none)
+    long long rows = 0, cols = 0, nnz = 0;
+    std::vector<ExportRec> rec;           // per record of the layout
+    std::vector<int> fid2rec;             // factor id -> record, -1 dead
+    std::vector<int> live_row;            // first row of the k-th live factor (factor order), then the total row count
+    void* mem = nullptr; size_t bytes = 0;   // device: rec, row_ptr [rows + 1], col_idx [nnz]
+    ExportRec* d_rec = nullptr;
+    int *d_row_ptr = nullptr, *d_col_idx = nullptr;
+    bool structure = false;               // d_row_ptr / d_col_idx filled for this layout
+    cudaEvent_t ev_copy = nullptr;        // recorded after an export's device-to-host copies
+  } xt;
   std::map<std::string, std::pair<double*, size_t>> named;  // debug access to double buffers
   DevGraph hd;
   DevGraph* d_graph = nullptr;
@@ -685,6 +699,8 @@ int pus_destroy(pus_handle h) {
   if (s->d_batch) cudaFree(s->d_batch);
   if (s->d_batch_res) cudaFree(s->d_batch_res);
   if (s->rt.mem) cudaFree(s->rt.mem);
+  if (s->xt.mem) cudaFree(s->xt.mem);
+  if (s->xt.ev_copy) cudaEventDestroy(s->xt.ev_copy);
   if (s->scratch) cudaFree(s->scratch);
   if (s->ev0) cudaEventDestroy(s->ev0);
   if (s->ev1) cudaEventDestroy(s->ev1);
@@ -1251,6 +1267,249 @@ int pus_project_to_planes(pus_handle h, int n_points, const int* plane_of_point,
   CUDA_OK(cudaMemcpyAsync(pts_out, d_out, (size_t)n_points * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
   return 0;
+}
+
+// ---- weighted errors / stacked Jacobian at the current estimate (pus_export.cu) ----
+// Every export starts as pus_project_to_planes does: re-upload when the topology, the host values or the measurements changed,
+// otherwise only bind the device (the estimate on the device is then the one a resident solve left there).  The per-record
+// table is rebuilt after a layout rebuild: one pass over the nodes (column of every live node) and one over the factors (first
+// row and first value of every live factor), not Graph::node_start / factor_row per factor.
+static int export_prepare(Solver* s, const char* fn) {
+  if (s->g.num_factors() == 0) { g_err = std::string(fn) + ": the graph has no live factors"; return -1; }
+  if (!s->uploaded || s->compiled_topo != s->g.topo_version || s->values_dirty || s->meas_dirty) {
+    if (upload(s) < 0) return -1;
+  } else if (ensure_device(s) < 0) {
+    return -1;
+  }
+  Solver::ExportTables& x = s->xt;
+  if (!x.ev_copy) CUDA_OK(cudaEventCreate(&x.ev_copy));
+  if (x.topo == s->compiled_topo) return 0;
+  const Graph& g = s->g;
+  const Compiled& c = s->c;
+  std::vector<int> col(g.nodes.size(), -1);
+  long long cols = 0, rows = 0, nnz = 0;
+  for (size_t i = 0; i < g.nodes.size(); i++)
+    if (g.nodes[i].alive) { col[i] = (int)cols; cols += g.nodes[i].kind == NODE_POSE ? 6 : 3; }
+  std::vector<int> frow(g.factors.size(), -1), fval(g.factors.size(), -1);
+  x.live_row.clear();
+  for (size_t f = 0; f < g.factors.size(); f++) {
+    const HFactor& F = g.factors[f];
+    if (!F.alive) continue;
+    int ncols = 0;
+    for (int k = 0; k < F.n_nodes; k++) ncols += g.nodes[F.nodes[k]].kind == NODE_POSE ? 6 : 3;
+    frow[f] = (int)rows; fval[f] = (int)nnz;
+    x.live_row.push_back((int)rows);
+    rows += F.dim;
+    nnz += (long long)F.dim * ncols;
+    if (nnz > 0x7fffffffll || cols > 0x7fffffffll) {
+      g_err = std::string(fn) + ": the Jacobian has more than 2^31 - 1 nonzeros or columns; its int32 indices cannot address it";
+      x.topo = 0;
+      return -1;
+    }
+  }
+  x.live_row.push_back((int)rows);
+  x.rows = rows; x.cols = cols; x.nnz = nnz;
+  const int nrec = c.nslot + c.Epf + c.Elp;
+  x.rec.assign(nrec, ExportRec{-1, -1, -1, -1});
+  x.fid2rec.assign(g.factors.size(), -1);
+  auto fill = [&](int q, int fid) {
+    if (fid < 0) return;
+    const HFactor& F = g.factors[fid];
+    x.rec[q] = ExportRec{frow[fid], fval[fid], col[F.nodes[0]], F.n_nodes == 2 ? col[F.nodes[1]] : -1};
+    x.fid2rec[fid] = q;
+  };
+  for (int e = 0; e < c.nslot; e++) fill(e, c.pp_fid[e]);
+  for (int f = 0; f < c.Epf; f++) fill(c.nslot + f, c.pf_fid[f]);
+  for (int f = 0; f < c.Elp; f++) fill(c.nslot + c.Epf + f, c.lp_fid[f]);
+  auto al = [](size_t b) { return (b + 255) / 256 * 256; };
+  const size_t need = al(sizeof(ExportRec) * (size_t)std::max(nrec, 1)) + al(4 * (size_t)(rows + 1)) + al(4 * (size_t)std::max(nnz, 1ll));
+  CUDA_OK(cudaSetDevice(s->device));
+  if (need > x.bytes) {
+    if (x.mem) { cudaStreamSynchronize(s->stream); cudaFree(x.mem); x.mem = nullptr; x.bytes = 0; }
+    CUDA_OK(cudaMalloc(&x.mem, need));
+    x.bytes = need;
+  }
+  char* base = static_cast<char*>(x.mem);
+  x.d_rec = reinterpret_cast<ExportRec*>(base);
+  x.d_row_ptr = reinterpret_cast<int*>(base + al(sizeof(ExportRec) * (size_t)std::max(nrec, 1)));
+  x.d_col_idx = reinterpret_cast<int*>(reinterpret_cast<char*>(x.d_row_ptr) + al(4 * (size_t)(rows + 1)));
+  if (nrec) CUDA_OK(cudaMemcpyAsync(x.d_rec, x.rec.data(), sizeof(ExportRec) * nrec, cudaMemcpyHostToDevice, s->stream));
+  CUDA_OK(cudaStreamSynchronize(s->stream));   // (x.rec may be rebuilt before a later copy would have run)
+  x.structure = false;
+  x.topo = s->compiled_topo;
+  return 0;
+}
+
+// evaluate records recs[0..n) (nullptr: every record) into d_err (and the Jacobian values / rhs when d_vals != nullptr);
+// the kernel time goes to stats.kernel_ms
+static int export_run(Solver* s, const int* d_recs, const int* d_orow, int n, double* d_err, double* d_vals, double* d_rhs) {
+  const Compiled& c = s->c;
+  const DevGraph& d = s->hd;
+  ExportArgs a;
+  a.pose_lin = d.pose_lin; a.plane_lin = d.plane_lin;
+  a.pp_pose = d.pp_pose; a.pp_plane = d.pp_plane; a.pp_meas = d.pp_meas; a.pp_sinf = d.pp_sinf; a.pp_rays = d.pp_rays;
+  a.pp_kind = d.pp_kind; a.n_f2 = c.n_f2;
+  a.pf_i = d.pf_i; a.pf_j = d.pf_j; a.pf_meas = d.pf_meas; a.pf_sinf = d.pf_sinf;
+  a.lp_plane = d.lp_plane; a.lp_meas = d.lp_meas; a.lp_sinf = d.lp_sinf;
+  a.nslot = c.nslot; a.Epf = c.Epf; a.Elp = c.Elp;
+  a.robust_kind = s->robust_kind; a.robust_b = s->robust_b; a.numeric = s->jac_numeric;
+  a.rec = s->xt.d_rec; a.recs = d_recs; a.orow = d_orow; a.n = n;
+  a.err = d_err; a.vals = d_vals; a.rhs = d_rhs;
+  CUDA_OK(cudaEventRecord(s->ev0, s->stream));
+  CUDA_OK(launch_export(s->stream, a));
+  CUDA_OK(cudaEventRecord(s->ev1, s->stream));
+  return 0;
+}
+// wait for the export; kernel time = ev0 -> ev1 around the evaluation, copy time = ev1 -> ev_copy (recorded here, after the
+// device-to-host copies the caller enqueued)
+static int export_finish(Solver* s, int launches, long long d2h_bytes) {
+  CUDA_OK(cudaEventRecord(s->xt.ev_copy, s->stream));
+  CUDA_OK(cudaEventSynchronize(s->xt.ev_copy));
+  float ms = 0, ms2 = 0;
+  CUDA_OK(cudaEventElapsedTime(&ms, s->ev0, s->ev1));
+  CUDA_OK(cudaEventElapsedTime(&ms2, s->ev1, s->xt.ev_copy));
+  s->stats.kernel_ms = ms; s->stats.d2h_ms = ms2; s->stats.d2h_bytes = d2h_bytes; s->stats.gpu_launches = launches;
+  return 0;
+}
+
+// the errors of every live factor into device scratch; returns the scratch pointer (nullptr on failure)
+static double* export_all_errors(Solver* s, Scratch& sc, size_t extra) {
+  const Solver::ExportTables& x = s->xt;
+  if (!sc.reserve(Scratch::al(8 * (size_t)x.rows) + extra)) { g_err = "scratch allocation failed"; return nullptr; }
+  double* d_err = sc.put<double>(nullptr, (size_t)x.rows);
+  if (!d_err) { g_err = "scratch allocation failed"; return nullptr; }
+  if (export_run(s, nullptr, nullptr, (int)x.rec.size(), d_err, nullptr, nullptr) < 0) return nullptr;
+  return d_err;
+}
+
+// sum of squares of rows [lo, rows) of the weighted errors (fixed order); chi2 of the whole graph for lo = 0
+static int export_sumsq(Solver* s, long long lo, double* out) {
+  Scratch sc{s, s->stream};
+  const size_t extra = Scratch::al(8 * kExportRedBlocks) + Scratch::al(8);
+  double* d_err = export_all_errors(s, sc, extra);
+  if (!d_err) return -1;
+  double* part = sc.put<double>(nullptr, kExportRedBlocks);
+  double* d_out = sc.put<double>(nullptr, 1);
+  if (!part || !d_out) { g_err = "scratch allocation failed"; return -1; }
+  CUDA_OK(launch_sumsq(s->stream, d_err, lo, s->xt.rows, part, d_out));
+  CUDA_OK(cudaMemcpyAsync(out, d_out, 8, cudaMemcpyDeviceToHost, s->stream));
+  return export_finish(s, 3, 8);
+}
+
+long long pus_weighted_errors(pus_handle h, double* out, long long capacity) {
+  NEED(h);
+  Solver* s = SV(h);
+  if (export_prepare(s, "pus_weighted_errors") < 0) return -1;
+  const long long rows = s->xt.rows;
+  if (!out) return rows;   // size query
+  if (capacity < rows) { g_err = "pus_weighted_errors: capacity " + std::to_string(capacity) + " < " + std::to_string(rows) + " rows"; return -1; }
+  Scratch sc{s, s->stream};
+  double* d_err = export_all_errors(s, sc, 0);
+  if (!d_err) return -1;
+  CUDA_OK(cudaMemcpyAsync(out, d_err, 8 * (size_t)rows, cudaMemcpyDeviceToHost, s->stream));
+  if (export_finish(s, 1, 8 * rows) < 0) return -1;
+  return rows;
+}
+
+int pus_factor_errors(pus_handle h, int n, const int* fids, double* out) {
+  NEED(h);
+  Solver* s = SV(h);
+  if (n < 0 || (n > 0 && (!fids || !out))) { g_err = "pus_factor_errors: bad arguments"; return -1; }
+  for (int i = 0; i < n; i++)
+    if (!s->g.ok_factor(fids[i])) { g_err = "pus_factor_errors: bad factor id " + std::to_string(fids[i]); return -1; }
+  if (export_prepare(s, "pus_factor_errors") < 0) return -1;
+  if (n == 0) return 0;
+  std::vector<int> recs(n), orow(n);
+  int total = 0;
+  for (int i = 0; i < n; i++) {
+    recs[i] = s->xt.fid2rec[fids[i]];
+    orow[i] = total;
+    total += s->g.factors[fids[i]].dim;
+  }
+  Scratch sc{s, s->stream};
+  if (!sc.reserve(2 * Scratch::al(4 * (size_t)n) + Scratch::al(8 * (size_t)total))) { g_err = "scratch allocation failed"; return -1; }
+  int* d_recs = sc.put(recs.data(), n);
+  int* d_orow = sc.put(orow.data(), n);
+  double* d_err = sc.put<double>(nullptr, total);
+  if (!d_recs || !d_orow || !d_err) { g_err = "scratch allocation failed"; return -1; }
+  if (export_run(s, d_recs, d_orow, n, d_err, nullptr, nullptr) < 0) return -1;
+  CUDA_OK(cudaMemcpyAsync(out, d_err, 8 * (size_t)total, cudaMemcpyDeviceToHost, s->stream));
+  if (export_finish(s, 1, 8ll * total) < 0) return -1;   // (also keeps recs / orow alive until their copies ran)
+  return total;
+}
+
+int pus_jacobian_dims(pus_handle h, long long* rows, long long* cols) {
+  NEED(h);
+  const Solver* s = SV(h);
+  if (s->xt.topo != 0 && s->xt.topo == s->compiled_topo && s->compiled_topo == s->g.topo_version) {   // the export's tables are current
+    if (rows) *rows = s->xt.rows;
+    if (cols) *cols = s->xt.cols;
+    return 0;
+  }
+  const Graph& g = s->g;   // (no export since the last structural edit: one pass over the host graph)
+  long long r = 0, c = 0;
+  for (const HFactor& f : g.factors) if (f.alive) r += f.dim;
+  for (const HNode& n : g.nodes) if (n.alive) c += n.kind == NODE_POSE ? 6 : 3;
+  if (rows) *rows = r;
+  if (cols) *cols = c;
+  return 0;
+}
+
+long long pus_jacobian(pus_handle h, int* row_ptr, int* col_idx, double* values, double* rhs, long long cap_nnz) {
+  NEED(h);
+  Solver* s = SV(h);
+  if (export_prepare(s, "pus_jacobian") < 0) return -1;
+  Solver::ExportTables& x = s->xt;
+  if (cap_nnz == 0) return x.nnz;   // size query
+  if (cap_nnz < x.nnz) { g_err = "pus_jacobian: cap_nnz " + std::to_string(cap_nnz) + " < " + std::to_string(x.nnz) + " nonzeros"; return -1; }
+  cudaStream_t st = s->stream;
+  const int nrec = (int)x.rec.size();
+  if ((row_ptr || col_idx) && !x.structure) {   // once per layout
+    CUDA_OK(launch_export_structure(st, x.d_rec, nrec, s->c.nslot, s->c.Epf, s->hd.pf_j, (int)x.rows, (int)x.nnz, x.d_row_ptr, x.d_col_idx));
+    x.structure = true;
+  }
+  Scratch sc{s, st};
+  double* d_vals = nullptr;
+  double* d_rhs = nullptr;
+  CUDA_OK(cudaEventRecord(s->ev0, st));
+  CUDA_OK(cudaEventRecord(s->ev1, st));
+  if (values || rhs) {
+    if (!sc.reserve(2 * Scratch::al(8 * (size_t)x.rows) + Scratch::al(8 * (size_t)x.nnz))) { g_err = "scratch allocation failed"; return -1; }
+    double* d_err = sc.put<double>(nullptr, (size_t)x.rows);
+    d_rhs = sc.put<double>(nullptr, (size_t)x.rows);
+    d_vals = sc.put<double>(nullptr, (size_t)x.nnz);
+    if (!d_err || !d_rhs || !d_vals) { g_err = "scratch allocation failed"; return -1; }
+    if (export_run(s, nullptr, nullptr, nrec, d_err, d_vals, d_rhs) < 0) return -1;
+  }
+  long long bytes = 0;
+  if (row_ptr) { CUDA_OK(cudaMemcpyAsync(row_ptr, x.d_row_ptr, 4 * (size_t)(x.rows + 1), cudaMemcpyDeviceToHost, st)); bytes += 4 * (x.rows + 1); }
+  if (col_idx) { CUDA_OK(cudaMemcpyAsync(col_idx, x.d_col_idx, 4 * (size_t)x.nnz, cudaMemcpyDeviceToHost, st)); bytes += 4 * x.nnz; }
+  if (values) { CUDA_OK(cudaMemcpyAsync(values, d_vals, 8 * (size_t)x.nnz, cudaMemcpyDeviceToHost, st)); bytes += 8 * x.nnz; }
+  if (rhs) { CUDA_OK(cudaMemcpyAsync(rhs, d_rhs, 8 * (size_t)x.rows, cudaMemcpyDeviceToHost, st)); bytes += 8 * x.rows; }
+  if (export_finish(s, (values || rhs) ? 1 : 0, bytes) < 0) return -1;
+  return x.nnz;
+}
+
+int pus_normalized_chi2(pus_handle h, double* out) {
+  NEED(h);
+  Solver* s = SV(h);
+  if (!out) { g_err = "pus_normalized_chi2: null output"; return -1; }
+  if (export_prepare(s, "pus_normalized_chi2") < 0) return -1;
+  double chi2 = 0;
+  if (export_sumsq(s, 0, &chi2) < 0) return -1;
+  *out = chi2 / (double)(s->xt.rows - s->xt.cols);   // as Slam.cpp:287-289 (no guard for rows <= columns there either)
+  return 0;
+}
+
+int pus_local_chi2(pus_handle h, int last_n, double* out) {
+  NEED(h);
+  Solver* s = SV(h);
+  if (!out) { g_err = "pus_local_chi2: null output"; return -1; }
+  if (export_prepare(s, "pus_local_chi2") < 0) return -1;
+  const std::vector<int>& lr = s->xt.live_row;   // nlive + 1 entries
+  const int nlive = (int)lr.size() - 1;
+  const long long lo = last_n <= 0 ? lr[nlive] : lr[std::max(0, nlive - last_n)];
+  return export_sumsq(s, lo, out);
 }
 
 // ---- graph text I/O (host only) ----
