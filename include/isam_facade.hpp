@@ -476,8 +476,9 @@ class Slam {
   void set_cost_function(cost_func_t f) { detail::check(pus_set_robust(_h, f.kind, f.b)); }   // Slam.cpp:212-214
   // Extension, no iSAM counterpart (kept out of Properties, which mirrors iSAM's struct): solve the reduced pose system
   // exactly by a dense Cholesky on the device instead of PCG -- with force_numerical_jacobian, a solve that does what the
-  // reference does step for step.  Graphs of at most 640 poses; see pus_set_linear_solver.
-  enum LinearSolver { LINEAR_SOLVER_PCG = 0, LINEAR_SOLVER_DIRECT = 1 };
+  // reference does step for step.  DIRECT: dense, graphs of at most 640 poses; BAND: the same exact solve on the envelope
+  // of a bordered system, graphs of any size within its device-memory budget; see pus_set_linear_solver.
+  enum LinearSolver { LINEAR_SOLVER_PCG = 0, LINEAR_SOLVER_DIRECT = 1, LINEAR_SOLVER_BAND = 2 };
   void set_linear_solver(LinearSolver kind) { detail::check(pus_set_linear_solver(_h, (int)kind)); }
   void add_node(Pose3d_Node* n) { n->_attach(_h); _nodes.push_back(n); }            // Slam.cpp:91-94
   void add_node(Plane3d_Node* n) { n->_attach(_h); _nodes.push_back(n); }

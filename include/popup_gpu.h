@@ -29,9 +29,11 @@
  * Limits (a solve fails with a message instead of producing a wrong answer):
  *   - Slam::update() only with mod_batch = 1 (what PPS sets); relative-parameterised plane factors, anchor nodes,
  *     dog-leg and covariance recovery are not provided.
- *   - the direct linear solver (pus_set_linear_solver(h, 1)) handles at most 640 live poses (a dense reduced system of
- *     order 3 840, about 65 MB of device memory); a larger graph fails at upload with a message and launches nothing.
- *     It does not span ranks: the pus_span_* entry points refuse a direct-mode handle.
+ *   - the dense direct linear solver (pus_set_linear_solver(h, 1)) handles at most 640 live poses (a dense reduced system
+ *     of order 3 840, about 65 MB of device memory); a larger graph fails at upload with a message and launches nothing.
+ *     The band direct solver (kind 2) takes any graph whose envelope fits 8 GiB of device memory (tiles, snapshots, pivot
+ *     inverses, vectors and tables; there is no fill-reducing reordering); a larger one fails at upload with a message
+ *     stating the need and launches nothing.  Neither spans ranks: the pus_span_* entry points refuse a direct-mode handle.
  *   - the error / Jacobian export (pus_weighted_errors .. pus_local_chi2) evaluates at the estimate only (iSAM's default
  *     Selector ESTIMATE; LINPOINT is not provided) and writes caller-owned host arrays only.  Its indices are int32: a
  *     graph whose Jacobian has more than 2^31 - 1 nonzeros is refused with a message.
@@ -185,17 +187,22 @@ int pus_set_jacobian_mode(pus_handle h, int numeric);
 /* Linear solver of the reduced pose system S dp = b (DESIGN.md section 5); a handle setting, no iSAM counterpart.
  * kind 0 (default): block-preconditioned CG to pcg_rel_tol.  kind 1: exact -- S assembled densely on the device, factored
  * S = L L^T (48x48 tiles, FP64 tensor cores) and solved by two blocked triangular solves, as the reference's direct
- * Cholesky (ISAM/isamlib/Cholesky.cpp:68-147) solves the same damped system.  Every linear solve is bit-identical across
+ * Cholesky (ISAM/isamlib/Cholesky.cpp:68-147) solves the same damped system.  kind 2: exact as kind 1, on the envelope of
+ * a bordered system -- the poses in insertion order, then the few planes seen from most of the trajectory (chosen by
+ * observer span, at most 64) kept as unknowns instead of being eliminated; the tiles outside the envelope are never stored,
+ * factored or read (DESIGN.md section 5.2).  Every linear solve is bit-identical across
  * team sizes, barrier kinds and batch positions; the chi2 and |delta| of the trace come from the team reduction, whose order
  * follows the team size, so whole runs agree bit for bit as long as no accept / reject decision is a tie in the last bits.  It applies to pus_batch_optimize (LM and GN), pus_update, pus_solve_resident
- * and the _many forms; a batch may mix both kinds (each kind runs as a launch of its own).  In direct mode
+ * and the _many forms; a batch may mix all kinds (PCG and direct handles run as launches of their own).  In direct mode
  * pus_get_trace's pcg entry is 0 for a step whose factorization succeeded and -1 for one that met a non-positive pivot
  * (the step is then delta = 0: LM evaluates it as a trial step, rejects it and raises lambda; GN stops; pus_update applies
  * the zero step, leaving the estimate where it was), pus_stats.pcg_iterations is 0, phase_ms[1] is
  * assembly + factorization and phase_ms[2] the triangular solves + plane back-substitution, and the set-up sub-slots are
  * 8 plane inverses, 10 (pose, plane) blocks W and W Hll^-1, 11 assembly of S, 12 factorization, 13 right-hand side,
  * 14 triangular solves.  Limits: see the header's Limits block.  Changing the kind lays the graph out again at the next
- * upload. */
+ * upload.  The debug hooks of direct mode ("Sdir", "Ldir", stages 4 and 5) use the bordered order in kind 2: 6 N pose rows,
+ * then 3 per bordered plane; a stored "Sdir" must lie inside the envelope, and stage 5 writes the bordered planes' part of
+ * the solution to their dl. */
 int pus_set_linear_solver(pus_handle h, int kind);
 int pus_get_linear_solver(pus_handle h);   /* the kind, or < 0 on error */
 int pus_get_solver_options(pus_handle h, pus_solver_options* out);

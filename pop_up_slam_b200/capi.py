@@ -363,12 +363,23 @@ class GpuGraphAPI(GraphAPI):
         self._chk(self.lib.pus_set_jacobian_mode(self.h, 1 if int(mode) == 0 else 0))
 
     def set_linear_solver(self, direct):
-        """direct=True: solve the reduced pose system exactly (dense Cholesky on the device, graphs of at most 640 poses);
-        direct=False: block-preconditioned CG (the default)."""
-        self._chk(self.lib.pus_set_linear_solver(self.h, 1 if direct else 0))
+        """direct=True or 1: solve the reduced pose system exactly (dense Cholesky on the device, graphs of at most 640 poses);
+        2: exactly, by a band Cholesky of the bordered system (any graph within its device-memory budget);
+        direct=False or 0: block-preconditioned CG (the default)."""
+        if isinstance(direct, bool):
+            kind = 1 if direct else 0
+        elif isinstance(direct, (int, np.integer)) and int(direct) in (0, 1, 2):
+            kind = int(direct)
+        else:
+            raise ValueError(f"linear solver: expected True / False or a kind 0, 1 or 2, got {direct!r}")
+        self._chk(self.lib.pus_set_linear_solver(self.h, kind))
+
+    def linear_solver_kind(self):
+        """0 = PCG, 1 = dense direct, 2 = band direct."""
+        return self._chk(self.lib.pus_get_linear_solver(self.h))
 
     def linear_solver_is_direct(self):
-        return self._chk(self.lib.pus_get_linear_solver(self.h)) == 1
+        return self.linear_solver_kind() == 1
 
     def get_solver_options(self):
         o = SolverOptions()

@@ -147,7 +147,7 @@ __device__ void direct_setup(Phase& ph, Ctx& c, double lambda, Timer& ft) {
   ft.lap(12);
 }
 
-// x = S^-1 b, then the planes as schur_solve does.  *its = 0, or -1 after a non-positive pivot: then delta = 0.
+// x = S^-1 b, then the planes as schur_solve does (the bordered planes too: the same delta in exact arithmetic).  *its = 0, or -1 after a non-positive pivot: then delta = 0.
 __device__ double direct_solve(Phase& ph, Ctx& c, double lambda, int* its, Timer& ft) {
   if (G.prm.mode == MODE_DEBUG && G.prm.debug_stage == 4) { *its = 0; return 0.0; }
   ft.sync();
@@ -160,7 +160,8 @@ __device__ double direct_solve(Phase& ph, Ctx& c, double lambda, int* its, Timer
     *its = -1;
     return 0.0;
   }
-  ph.pose_phase(true, nullptr, lambda, nullptr, nullptr);   // b = -gp + W Hll_d^-1 gl
+  if (G.dnbord) ph.direct_rhs();                                // band layout with bordered planes
+  else ph.pose_phase(true, nullptr, lambda, nullptr, nullptr);   // b = -gp + W Hll_d^-1 gl
   team_barrier(c);
   ft.lap(13);
   ph.direct_trsv();
@@ -237,6 +238,8 @@ __device__ void run_graph_impl(Ctx& c) {
       if (__ldcg(G.dflag) == 0u) {
         ph.direct_trsv();
         for (int i = ph.tid_team(); i < G.N * 6; i += ph.nthr_team()) G.x[i] = ldc(G.dvec + i);
+        for (int k = ph.tid_team(); k < 3 * G.dnbord; k += ph.nthr_team())   // a bordered plane's part of x goes to its dl
+          G.dl[(size_t)ldc(G.dbord + k / 3) * 3 + k % 3] = ldc(G.dvec + 48 * G.dnbp + k);
         team_barrier(c);
       }
       return;

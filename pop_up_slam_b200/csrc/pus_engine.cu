@@ -54,7 +54,7 @@ struct Solver {
   int robust_kind = 0;
   double robust_b = 1.0;
   int jac_numeric = 0;
-  int linear_solver = 0;       // 0: PCG, 1: exact dense Cholesky of the reduced pose system (pus_set_linear_solver)
+  int linear_solver = 0;       // 0: PCG, 1: exact dense Cholesky of the reduced pose system, 2: exact band Cholesky (pus_set_linear_solver)
   pus_solver_options opt;
   Compiled c;
   DirectTables dt;             // (direct mode only)
@@ -239,7 +239,7 @@ static int upload(Solver* s) {
     s->recycle_device();
     std::string err;
     if (!compile_graph(s->g, s->c, err)) { g_err = err; return -1; }
-    if (s->linear_solver == 1 && !build_direct(s->c, s->dt, err)) { g_err = err; return -1; }
+    if (s->linear_solver != 0 && !build_direct(s->c, s->dt, err, s->linear_solver)) { g_err = err; return -1; }
     const Compiled& c = s->c;
     if (kSmRc + 6 * c.nc * 8 > kSmemBytes) { g_err = "graph too large for the coarse-space shared-memory buffer"; return -1; }
     DevGraph& d = s->hd;
@@ -283,7 +283,8 @@ static int upload(Solver* s) {
       struct Item { double** p; size_t n; const char* name; };
       const Item items[] = {
           {&d.vl, M * 3, "vl"}, {&d.dl, M * 3, "dl"}, {&d.upart, (size_t)c.n_upart * 3, "upart"},
-          {&d.x, N * 6, "x"}, {&d.r, N * 6, "r"}, {&d.z, N * 6, "z"}, {&d.q, N * 6, "q"}, {&d.b, N * 6, "b"},
+          {&d.x, N * 6, "x"}, {&d.r, N * 6, "r"}, {&d.z, N * 6, "z"}, {&d.q, N * 6, "q"},
+          {&d.b, N * 6 + (s->linear_solver == 2 ? 3 * s->dt.border.size() : 0), "b"},   // (band solve: then 3 per bordered plane)
           {&d.pv[0], N * 6, "pv0"}, {&d.pv[1], N * 6, "pv1"}, {&d.xprev, N * 6, "xprev"}, {&d.zc, (size_t)6 * c.nc, "zc"},
           {&d.zc2, (size_t)6 * c.nc2, "zc2"}, {&d.rc3, (size_t)6 * c.nc, "rc3"},
           {&d.rcpart[0], (size_t)c.nblk * 12, "rcpart0"}, {&d.rcpart[1], (size_t)c.nblk * 12, "rcpart1"},
@@ -303,16 +304,19 @@ static int upload(Solver* s) {
       }
       d.span_w = 1; d.span_r = 0;
     }
-    if (s->linear_solver == 1) {   // the dense solve's tables and its tile store (about 65 MB at the 640-pose cap)
+    if (s->linear_solver != 0) {   // the direct solve's tables and its tile store (dense: about 65 MB at the 640-pose cap)
+      static_assert(kDirectTileBytes == kAcTile * 8, "band byte count: tile size");
       const DirectTables& dt = s->dt;
       const size_t nb = dt.nb, ninc = dt.inc_pose.size();
-      d.dnb = dt.nb; d.dninc = (int)ninc;
+      d.dnb = dt.nb; d.dninc = (int)ninc; d.dnbp = dt.nbp; d.dnbord = (int)dt.border.size();
 #define UPD(field, vec) if (s->dupload(&d.field, vec, &bytes) < 0) return -1
       UPD(dinc_plane, dt.inc_plane); UPD(dinc_lo, dt.inc_lo); UPD(dinc_hi, dt.inc_hi);
       UPD(dlp_ptr, dt.lp_ptr); UPD(dlp_a, dt.lp_a); UPD(dlp_b, dt.lp_b); UPD(dfp_ptr, dt.fp_ptr); UPD(dfp_f, dt.fp_f);
+      UPD(dfirst, dt.first); UPD(dtoff, dt.toff); UPD(dpoff, dt.poff); UPD(dcol_ptr, dt.col_ptr); UPD(dcol_row, dt.col_row);
+      UPD(dbord, dt.border); UPD(dbinc, dt.binc);
 #undef UPD
       AL(Wd, ninc * 18, "Wd"); AL(Yd, ninc * 18, "Yd");
-      AL(Sd, nb * (nb + 1) / 2 * kAcTile, nullptr); AL(Dsnap, 2 * nb * kAcTile, nullptr); AL(Dinv, nb * kAcTile, nullptr);
+      AL(Sd, (size_t)dt.toff[nb] * kAcTile, nullptr); AL(Dsnap, 2 * nb * kAcTile, nullptr); AL(Dinv, nb * kAcTile, nullptr);
       AL(dvec, 2 * 48 * nb, nullptr);
       if (s->dalloc(&d.dflag, 1) < 0) return -1;
     }
@@ -410,9 +414,9 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
     if (!ss[i]->uploaded) { g_err = "graph not uploaded"; return -1; }
     if (ss[i]->device != s0->device) { g_err = "all graphs of a batch must live on one device"; return -1; }
   }
-  const int direct = s0->linear_solver;
+  const bool direct = s0->linear_solver != 0;   // dense and band handles share the direct solve's kernel
   for (int i = 0; i < n; i++)
-    if (ss[i]->linear_solver != direct) { g_err = "one launch cannot mix direct and PCG handles"; return -1; }
+    if ((ss[i]->linear_solver != 0) != direct) { g_err = "one launch cannot mix direct and PCG handles"; return -1; }
   void* const kern = direct ? direct_kernel_ptr() : (void*)kplain::lm_kernel;
   int per_sm = 0;
   CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, kSmemBytes));
@@ -859,14 +863,14 @@ int pus_set_jacobian_mode(pus_handle h, int numeric) { NEED(h); SV(h)->jac_numer
 int pus_set_linear_solver(pus_handle h, int kind) {
   NEED(h);
   Solver* s = SV(h);
-  if (kind != 0 && kind != 1) { g_err = "bad linear solver kind (0 = PCG, 1 = direct)"; return -1; }
+  if (kind < 0 || kind > 2) { g_err = "bad linear solver kind (0 = PCG, 1 = dense direct, 2 = band direct)"; return -1; }
   if (kind != s->linear_solver) { s->linear_solver = kind; s->g.topo_version++; }   // the next upload lays the graph out again
   return 0;
 }
 int pus_get_linear_solver(pus_handle h) { NEED(h); return SV(h)->linear_solver; }
 static int refuse_direct_span(Solver* s, const char* fn) {
-  if (s->linear_solver != 1) return 0;
-  g_err = std::string(fn) + ": the direct linear solver does not span ranks (set the PCG solver, kind 0)";
+  if (s->linear_solver == 0) return 0;
+  g_err = std::string(fn) + ": the direct linear solvers do not span ranks (set the PCG solver, kind 0)";
   return -1;
 }
 int pus_get_solver_options(pus_handle h, pus_solver_options* out) { NEED(h); *out = SV(h)->opt; return 0; }
@@ -886,9 +890,9 @@ static int solve_many(pus_handle* hs, int n, int* iters, int mode, int restore) 
   for (int i = 0; i < n; i++) ss[i] = SV(hs[i]);
   if (ensure_device(ss[0]) < 0) return -1;
   BatchStreams bs(hs, n, ss[0]->stream);
-  // direct-mode and PCG handles run in their own kernels: a mixed batch is two launches, one per kind
+  // direct-mode (dense and band) and PCG handles run in their own kernels: a mixed batch is two launches, one per kernel
   std::vector<Solver*> part[2];
-  for (int i = 0; i < n; i++) part[ss[i]->linear_solver == 1].push_back(ss[i]);
+  for (int i = 0; i < n; i++) part[ss[i]->linear_solver != 0].push_back(ss[i]);
   for (int k = 0; k < 2; k++)
     if (!part[k].empty() && launch(part[k].data(), (int)part[k].size(), mode, restore, 0, 0.0) < 0) return -1;
   if (iters) for (int i = 0; i < n; i++) iters[i] = ss[i]->res.iterations;
@@ -1648,6 +1652,10 @@ int pus_load_isam_dataset(pus_handle h, const char* path, int* n_poses, int* n_f
   return rc;
 }
 
+// order of the direct solve's system without padding (6 N, then 3 per bordered plane), and row r's row in the padded layout
+static int direct_order(const Solver* s) { return 6 * s->c.N + 3 * (int)s->dt.border.size(); }
+static int direct_row(const Solver* s, int r) { return r < 6 * s->c.N ? r : 48 * s->dt.nbp + r - 6 * s->c.N; }
+
 long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long cap) {
   NEED(h);
   Solver* s = SV(h);
@@ -1689,6 +1697,10 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
   if (nm == "dlp_b") return ints(s->dt.lp_b);
   if (nm == "dfp_ptr") return ints(s->dt.fp_ptr);
   if (nm == "dfp_f") return ints(s->dt.fp_f);
+  // band mode: the bordered planes, the first tile column of every tile row, and the device bytes of the solve
+  if (nm == "bborder") return ints(s->dt.border);
+  if (nm == "bfirst") return ints(s->dt.first);
+  if (nm == "bbytes") { if (cap >= 1) out[0] = (double)s->dt.bytes; return 1; }
   if (nm == "pf_i") return ints(c.pf_i);
   if (nm == "pf_j") return ints(c.pf_j);
   if (nm == "pl_pose") return ints(c.pl_pose);
@@ -1713,20 +1725,24 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
     return cnt;
   }
   if (nm == "Sdir" || nm == "Ldir") {   // direct mode: S after the assembly (debug stage 4) or L after the factorization, n x n
-    if (s->linear_solver != 1) { g_err = "not in direct linear-solver mode"; return -1; }
-    const int nb = s->hd.dnb, n = 6 * c.N;
-    const size_t total = (size_t)nb * (nb + 1) / 2 * kAcTile;
+    if (s->linear_solver == 0) { g_err = "not in direct linear-solver mode"; return -1; }
+    const DirectTables& dt = s->dt;
+    const int n = direct_order(s);   // (band: 6 N pose rows, then 3 per bordered plane, padding stripped)
+    const size_t total = (size_t)dt.toff[dt.nb] * kAcTile;
     std::vector<double> tmp(total);
     if (cudaMemcpy(tmp.data(), s->hd.Sd, total * 8, cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
     const long long cnt = (long long)n * n;
     if (cnt <= cap)
       for (int r = 0; r < n; r++)
-        for (int q = 0; q < n; q++)
-          out[(size_t)r * n + q] = q > r ? 0.0 : tmp[(size_t)((r / 48) * (r / 48 + 1) / 2 + q / 48) * kAcTile + (r % 48) * kAcLd + q % 48];
+        for (int q = 0; q < n; q++) {
+          const int pr = direct_row(s, r), pq = direct_row(s, q), ti = pr / 48, tj = pq / 48;
+          out[(size_t)r * n + q] = (q > r || tj < dt.first[ti]) ? 0.0
+                                   : tmp[(size_t)(dt.toff[ti] + tj - dt.first[ti]) * kAcTile + (pr % 48) * kAcLd + pq % 48];
+        }
     return cnt;
   }
   if (nm == "dflag") {   // direct mode: 1 when the last factorization met a non-positive pivot, else 0
-    if (s->linear_solver != 1) { g_err = "not in direct linear-solver mode"; return -1; }
+    if (s->linear_solver == 0) { g_err = "not in direct linear-solver mode"; return -1; }
     unsigned f = 0;
     if (cudaMemcpy(&f, s->hd.dflag, sizeof(f), cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
     if (cap >= 1) out[0] = f ? 1.0 : 0.0;
@@ -1763,24 +1779,39 @@ long long pus_debug_store(pus_handle h, const char* name, const double* in, long
   Solver* s = SV(h);
   cudaSetDevice(s->device);
   if (std::string(name) == "Sdir") {   // direct mode: a dense row-major S (n x n) for debug stage 5, laid out as direct_assemble does
-    if (s->linear_solver != 1) { g_err = "Sdir: not in direct linear-solver mode"; return -1; }
+    if (s->linear_solver == 0) { g_err = "Sdir: not in direct linear-solver mode"; return -1; }
     if (!s->uploaded) { g_err = "Sdir: call pus_upload first"; return -1; }
-    const int nb = s->hd.dnb, n = 6 * s->c.N;
-    if (count != (long long)n * n) { g_err = "Sdir: expected (6 N)^2 = " + std::to_string((long long)n * n) + " elements"; return -1; }
-    std::vector<double> tiles((size_t)nb * (nb + 1) / 2 * kAcTile, 0.0);
+    const DirectTables& dt = s->dt;
+    const int nb = dt.nb, n = direct_order(s);
+    if (count != (long long)n * n) {
+      g_err = s->linear_solver == 1 ? "Sdir: expected (6 N)^2 = " + std::to_string((long long)n * n) + " elements"
+                                    : "Sdir: expected (6 N + 3 B)^2 = " + std::to_string((long long)n * n) + " elements";
+      return -1;
+    }
+    std::vector<int> orig(48 * nb, -1);   // padded row -> row of the stored matrix (-1: padding)
+    for (int r = 0; r < n; r++) orig[direct_row(s, r)] = r;
+    for (int r = 0; r < n; r++)
+      for (int q = 0; q < r; q++)
+        if (in[(size_t)r * n + q] != 0.0 && direct_row(s, q) / 48 < dt.first[direct_row(s, r) / 48]) {
+          g_err = "Sdir: entry (" + std::to_string(r) + ", " + std::to_string(q) + ") lies outside the band layout's envelope";
+          return -1;
+        }
+    std::vector<double> tiles((size_t)dt.toff[nb] * kAcTile, 0.0);
     for (int ti = 0; ti < nb; ti++)
-      for (int tj = 0; tj <= ti; tj++) {
-        double* t = tiles.data() + (size_t)(ti * (ti + 1) / 2 + tj) * kAcTile;
+      for (int tj = dt.first[ti]; tj <= ti; tj++) {
+        double* t = tiles.data() + (size_t)(dt.toff[ti] + tj - dt.first[ti]) * kAcTile;
         for (int er = 0; er < 48; er++)
           for (int ec = 0; ec < 48; ec++) {
-            const int i = 48 * ti + er, j = 48 * tj + ec;
-            t[er * kAcLd + ec] = j > i ? 0.0 : (i >= n ? (i == j ? 1.0 : 0.0) : in[(size_t)i * n + j]);   // lower half, identity padding
+            const int i = 48 * ti + er, j = 48 * tj + ec, oi = orig[i], oj = orig[j];
+            t[er * kAcLd + ec] = j > i ? 0.0 : ((oi < 0 || oj < 0) ? (i == j ? 1.0 : 0.0) : in[(size_t)oi * n + oj]);   // lower half, identity padding
           }
       }
     if (cudaMemcpy(s->hd.Sd, tiles.data(), tiles.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) { g_err = "memcpy"; return -1; }
-    for (int ti = 0; ti < nb; ti++)   // tile column 0 is also the step-0 pivot-column snapshot (parity 0)
-      if (cudaMemcpy(s->hd.Dsnap + (size_t)ti * kAcTile, tiles.data() + (size_t)(ti * (ti + 1) / 2) * kAcTile, kAcTile * 8,
+    for (int ti = 0; ti < nb; ti++) {   // a row's first tile is also the pivot-column snapshot of the step that first reads it
+      const int f = dt.first[ti];
+      if (cudaMemcpy(s->hd.Dsnap + ((size_t)(f & 1) * nb + ti) * kAcTile, tiles.data() + (size_t)dt.toff[ti] * kAcTile, kAcTile * 8,
                      cudaMemcpyHostToDevice) != cudaSuccess) { g_err = "memcpy"; return -1; }
+    }
     return count;
   }
   auto it = s->named.find(name);
@@ -1793,7 +1824,7 @@ int pus_debug_run_stage(pus_handle h, int stage, double lambda) {
   NEED(h);
   Solver* s = SV(h);
   if (!s->uploaded) { g_err = "call pus_upload first"; return -1; }
-  if (stage == 5 && s->linear_solver != 1) { g_err = "debug stage 5 factors a stored Sdir: direct linear-solver mode only"; return -1; }
+  if (stage == 5 && s->linear_solver == 0) { g_err = "debug stage 5 factors a stored Sdir: direct linear-solver mode only"; return -1; }
   return launch(&s, 1, MODE_DEBUG, 0, stage, lambda);
 }
 
@@ -1803,7 +1834,7 @@ int pus_debug_compile(pus_handle h) {
   Solver* s = SV(h);
   std::string err;
   if (!compile_graph(s->g, s->c, err)) { g_err = err; return -1; }
-  if (s->linear_solver == 1 && !build_direct(s->c, s->dt, err)) { g_err = err; return -1; }
+  if (s->linear_solver != 0 && !build_direct(s->c, s->dt, err, s->linear_solver)) { g_err = err; return -1; }
   return 0;
 }
 

@@ -642,31 +642,84 @@ inline bool compile_graph(const Graph& g, Compiled& c, std::string& err) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Tables of the exact direct solve (pus_set_linear_solver(h, 1)), built only for handles in that mode.  The reduced pose
-// system S is assembled entry by entry; for every pose pair a >= b (index a (a + 1) / 2 + b) the host lists what couples
-// the two poses, in a fixed order:
+// Tables of the exact direct solves (pus_set_linear_solver(h, 1) dense, (h, 2) band), built only for handles in those modes.
+// The reduced system is assembled entry by entry; for every pose pair a >= b inside the envelope (index pair_index(a, b))
+// the host lists what couples the two poses, in a fixed order:
 //   dfp: pose-pose factors, f * 2 + side (side 1: the factor's second pose is a, its block enters transposed), factor order;
-//   dlp: planes seen from both poses, as a pair of (pose, plane) incidences (the coarse assembly's lp lists with P = I),
-//        plane-ascending.  An incidence covers every edge between its pose and plane (a pose that observes a plane twice
-//        has one incidence with two edges), as a range of plane-major slots.
+//   dlp: eliminated planes seen from both poses, as a pair of (pose, plane) incidences (the coarse assembly's lp lists with
+//        P = I), plane-ascending.  An incidence covers every edge between its pose and plane (a pose that observes a plane
+//        twice has one incidence with two edges), as a range of plane-major slots.
+// Band layout (kind 2): the poses in insertion order, padded to a whole tile with identity, then 3 rows per bordered plane
+// (plane-ascending), padded likewise.  A bordered plane stays an unknown of the reduced system instead of being eliminated:
+// eliminating a plane couples every pair of its observers, so the few planes seen from most of the trajectory (the ground
+// plane, a plane merged by a loop closure) would make the whole system dense.  Tile row i holds tiles first[i] .. i only
+// (first[i]: the smallest tile column any of its rows couples to); a Cholesky factor has no fill outside that envelope.
+// The dense solve (kind 1) is the same layout with no bordered plane and first = 0.
 // ------------------------------------------------------------------------------------------------
-constexpr int kDirectMaxPoses = 640;   // order 3 840: 80 tile columns of 48
+constexpr int kDirectMaxPoses = 640;          // order 3 840: 80 tile columns of 48
+constexpr int kBandMaxBorder = 64;            // most bordered planes the band layout tries
+constexpr long long kBandBudgetBytes = 8ll << 30;   // device memory a band solve may take (8 GiB)
+constexpr long long kDirectTileBytes = 48ll * 52 * 8;   // one 48 x 48 tile at leading dimension 52 (kAcTile doubles)
 
 struct DirectTables {
-  int nb = 0;   // tile rows of the padded order 48 nb >= 6 N
+  int nb = 0;    // tile rows of the padded order 48 nb
+  int nbp = 0;   // tile rows of the poses (>= 6 N / 48); the bordered planes' rows start at tile row nbp
   std::vector<int> inc_pose, inc_plane, inc_lo, inc_hi;
   std::vector<int> lp_ptr, lp_a, lp_b, fp_ptr, fp_f;
+  std::vector<int> first, toff, poff;   // per tile row: first tile column, tile offset (+ total); per pose: first pair index
+  std::vector<int> col_ptr, col_row;    // per tile column K: the tile rows i > K with first[i] <= K, ascending
+  std::vector<int> border, binc;        // bordered planes (ascending); [lo, hi) of each one's incidences
+  long long bytes = 0;                  // device memory of the solve's tiles, vectors and tables
 };
 
-inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err) {
+// first[] of a layout that borders the planes with bslot >= 0 (nbord of them), and the device bytes it takes
+inline long long band_envelope(const Compiled& c, const std::vector<int>& inc_ptr, const std::vector<int>& inc_pose,
+                               const std::vector<int>& bslot, int nbord, std::vector<int>& first, int& nbp, int& nb) {
+  const int N = c.N, M = c.M;
+  nbp = std::max(1, (6 * N + 47) / 48);
+  nb = nbp + (3 * nbord + 47) / 48;
+  std::vector<int> mp(N);   // smallest pose each pose couples to
+  for (int a = 0; a < N; a++) mp[a] = a;
+  for (int f = 0; f < c.Epf; f++) {
+    if (c.pf_j[f] < 0) continue;
+    const int hi = std::max(c.pf_i[f], c.pf_j[f]), lo = std::min(c.pf_i[f], c.pf_j[f]);
+    mp[hi] = std::min(mp[hi], lo);
+  }
+  first.assign(nb, 0);
+  for (int i = 0; i < nb; i++) first[i] = i;
+  long long lp = 0;
+  for (int l = 0; l < M; l++) {
+    const int n = inc_ptr[l + 1] - inc_ptr[l];
+    if (n == 0) continue;
+    const int pmin = inc_pose[inc_ptr[l]];   // incidences are pose-ascending inside a plane
+    if (bslot[l] >= 0) {
+      const int t = nbp + 3 * bslot[l] / 48;
+      first[t] = std::min(first[t], pmin / 8);
+    } else {
+      lp += (long long)n * (n + 1) / 2;
+      for (int i = inc_ptr[l]; i < inc_ptr[l + 1]; i++) mp[inc_pose[i]] = std::min(mp[inc_pose[i]], pmin);
+    }
+  }
+  for (int a = 0; a < N; a++) first[a / 8] = std::min(first[a / 8], mp[a] / 8);   // 8 poses of 6 rows per tile
+  long long tiles = 0, npair = 0, fp = 0;
+  for (int i = 0; i < nb; i++) tiles += i - first[i] + 1;
+  for (int a = 0; a < N; a++) npair += a - 8 * first[a / 8] + 1;
+  for (int f = 0; f < c.Epf; f++) fp += c.pf_j[f] >= 0;
+  const long long ninc = (long long)inc_pose.size();
+  const long long ints = 2 * (npair + 1) + 2 * lp + fp + 3 * ninc + nb + (nb + 1) + N + (nb + 1) + (tiles - nb) + 3 * nbord;
+  return (tiles + 3ll * nb) * kDirectTileBytes   // tiles, two pivot-column snapshots, pivot inverses
+         + 8 * (2ll * 48 * nb + 36 * ninc + 3ll * nbord) + 4 * ints;   // solve vectors, W / Y per incidence, border rhs, tables
+}
+
+// kind 1: dense (at most kDirectMaxPoses poses); kind 2: band, within kBandBudgetBytes
+inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err, int kind = 1) {
   d = DirectTables();
   const int N = c.N, M = c.M;
-  if (N > kDirectMaxPoses) {
+  if (kind == 1 && N > kDirectMaxPoses) {
     err = "direct linear solver: the graph has " + std::to_string(N) + " live poses; the dense solve handles at most " +
           std::to_string(kDirectMaxPoses) + " (use the PCG solver, kind 0)";
     return false;
   }
-  d.nb = std::max(1, (6 * N + 47) / 48);
   std::vector<int> inc_ptr(M + 1, 0);
   for (int l = 0; l < M; l++) {
     for (int s = c.pl_ptr[l]; s < c.pl_ptr[l + 1];) {
@@ -677,8 +730,61 @@ inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err) {
     }
     inc_ptr[l + 1] = (int)d.inc_pose.size();
   }
-  const size_t np = (size_t)N * (N + 1) / 2;
-  auto pair = [](int a, int b) { return (size_t)a * (a + 1) / 2 + b; };
+  std::vector<int> bslot(M, -1);
+  if (kind == 1) {
+    d.nbp = d.nb = std::max(1, (6 * N + 47) / 48);
+    d.first.assign(d.nb, 0);
+  } else {
+    // border the k planes of widest observer span (pose order; ties: lower index), k = 0 .. min(M, 64), whichever k takes
+    // the fewest device bytes (ties: the smaller k)
+    std::vector<int> span(M, 0), order(M);
+    for (int l = 0; l < M; l++) {
+      if (inc_ptr[l + 1] > inc_ptr[l]) span[l] = d.inc_pose[inc_ptr[l + 1] - 1] - d.inc_pose[inc_ptr[l]];
+      order[l] = l;
+    }
+    std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return span[x] > span[y]; });
+    long long best = -1;
+    int best_k = 0;
+    std::vector<int> fk, bs(M, -1);
+    for (int k = 0; k <= std::min(M, kBandMaxBorder); k++) {
+      std::fill(bs.begin(), bs.end(), -1);
+      std::vector<int> chosen(order.begin(), order.begin() + k);
+      std::sort(chosen.begin(), chosen.end());
+      for (int q = 0; q < k; q++) bs[chosen[q]] = q;
+      int nbp = 0, nb = 0;
+      const long long bytes = band_envelope(c, inc_ptr, d.inc_pose, bs, k, fk, nbp, nb);
+      if (best < 0 || bytes < best) { best = bytes; best_k = k; }
+    }
+    d.border.assign(order.begin(), order.begin() + best_k);
+    std::sort(d.border.begin(), d.border.end());
+    for (int q = 0; q < best_k; q++) bslot[d.border[q]] = q;
+    d.bytes = band_envelope(c, inc_ptr, d.inc_pose, bslot, best_k, d.first, d.nbp, d.nb);
+    if (d.bytes > kBandBudgetBytes) {
+      err = "band linear solver: the graph needs " + std::to_string(d.bytes) + " bytes of device memory (" +
+            std::to_string(N) + " poses, " + std::to_string(best_k) + " bordered planes); the budget is " +
+            std::to_string(kBandBudgetBytes) + " bytes (use the PCG solver, kind 0)";
+      d = DirectTables();
+      return false;
+    }
+    for (int q = 0; q < best_k; q++) { d.binc.push_back(inc_ptr[d.border[q]]); d.binc.push_back(inc_ptr[d.border[q] + 1]); }
+  }
+  const int nb = d.nb;
+  d.toff.assign(nb + 1, 0);
+  for (int i = 0; i < nb; i++) d.toff[i + 1] = d.toff[i] + i - d.first[i] + 1;
+  d.col_ptr.assign(nb + 1, 0);
+  for (int i = 0; i < nb; i++)
+    for (int K = d.first[i]; K < i; K++) d.col_ptr[K + 1]++;
+  for (int K = 0; K < nb; K++) d.col_ptr[K + 1] += d.col_ptr[K];
+  d.col_row.assign(std::max(1, d.col_ptr[nb]), 0);
+  {
+    std::vector<int> fill(d.col_ptr.begin(), d.col_ptr.end() - 1);
+    for (int i = 0; i < nb; i++)
+      for (int K = d.first[i]; K < i; K++) d.col_row[fill[K]++] = i;
+  }
+  d.poff.assign(N + 1, 0);
+  for (int a = 0; a < N; a++) d.poff[a + 1] = d.poff[a] + a - 8 * d.first[a / 8] + 1;
+  const size_t np = (size_t)d.poff[N];
+  auto pair = [&](int a, int b) { return (size_t)d.poff[a] + b - 8 * d.first[a / 8]; };
   d.lp_ptr.assign(np + 1, 0);
   for (int pass = 0; pass < 2; pass++) {
     std::vector<int> fill;
@@ -688,13 +794,15 @@ inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err) {
       d.lp_b.assign(std::max(1, d.lp_ptr[np]), 0);
       fill.assign(d.lp_ptr.begin(), d.lp_ptr.end() - 1);
     }
-    for (int l = 0; l < M; l++)   // incidences are pose-ascending inside a plane: i >= j gives a >= b
+    for (int l = 0; l < M; l++) {   // incidences are pose-ascending inside a plane: i >= j gives a >= b
+      if (bslot[l] >= 0) continue;
       for (int i = inc_ptr[l]; i < inc_ptr[l + 1]; i++)
         for (int j = inc_ptr[l]; j <= i; j++) {
           const size_t q = pair(d.inc_pose[i], d.inc_pose[j]);
           if (pass == 0) d.lp_ptr[q + 1]++;
           else { const int at = fill[q]++; d.lp_a[at] = i; d.lp_b[at] = j; }
         }
+    }
   }
   d.fp_ptr.assign(np + 1, 0);
   for (int pass = 0; pass < 2; pass++) {

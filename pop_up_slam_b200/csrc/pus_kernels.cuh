@@ -120,11 +120,15 @@ struct DevGraph {
   LmParams prm;
   LmResult* res;
   LmTrace* trace;
-  // exact direct solve (pus::kdirect only; zero / null for PCG handles): the reduced system of order 48 dnb as the lower
-  // triangle of 48x48 tiles, tile (I, J) at dtile(I, J) = I (I + 1) / 2 + J
-  int dnb, dninc;
+  // exact direct solves (pus::kdirect only; zero / null for PCG handles): the reduced system of order 48 dnb as the envelope
+  // of its lower triangle in 48x48 tiles (pus_graph.hpp, DirectTables), tile (I, J) at dtile(I, J) = dtoff[I] + J - dfirst[I];
+  // the dense solve has dfirst = 0, no bordered plane and dnbp = dnb
+  int dnb, dninc, dnbp, dnbord;                           // tile rows; incidences; pose tile rows; bordered planes
   const int *dinc_plane, *dinc_lo, *dinc_hi;              // (pose, plane) incidences, plane-major: plane-major slot range
-  const int *dlp_ptr, *dlp_a, *dlp_b, *dfp_ptr, *dfp_f;  // per pose pair a >= b: incidence pairs (plane-ascending), factor sides
+  const int *dlp_ptr, *dlp_a, *dlp_b, *dfp_ptr, *dfp_f;  // per envelope pose pair a >= b: incidence pairs (plane-ascending), factor sides
+  const int *dfirst, *dtoff, *dpoff;                     // per tile row: first tile column, tile offset; per pose: first pair index
+  const int *dcol_ptr, *dcol_row;                        // per tile column K: the tile rows i > K of the envelope in it
+  const int *dbord, *dbinc;                              // bordered planes (ascending); [lo, hi) of each one's incidences
   double *Wd, *Yd;       // [dninc][18]: W_al (summed over the pair's edges) and W_al Hll_d^-1
   double *Sd;            // S, factored in place into L
   double *Dsnap;         // [2 step parities][dnb] pivot-column snapshots
@@ -3045,7 +3049,8 @@ struct Phase {
   // ================= exact direct solve (DESIGN.md section 5): dense Cholesky of the reduced pose system =================
   // Every sum below has one order that does not depend on the team: each output entry is written by one thread, and the
   // tile products of the factorization read the same operands whichever CTA computes them.  No atomics.
-  __device__ __forceinline__ static int dtile(int i, int j) { return i * (i + 1) / 2 + j; }
+  __device__ __forceinline__ static int dtile(int i, int j) { return ldc(G.dtoff + i) + j - ldc(G.dfirst + i); }
+  __device__ __forceinline__ static int dpair(int a, int b) { return ldc(G.dpoff + a) + b - 8 * ldc(G.dfirst + a / 8); }
   template <typename T>
   __device__ __forceinline__ static T* tile_at(T* base, int t) { return base + (size_t)t * kAcTile; }
 
@@ -3067,26 +3072,51 @@ struct Phase {
     }
   }
 
-  // S = Hpp_d + (pose-pose blocks) - sum_l Y_al W_bl^T, entry by entry (output-stationary): the diagonal block, then the
-  // pose-pose factor blocks in factor order, then the plane products in plane order.  Upper halves of diagonal tiles are 0,
-  // the padding is identity.  Tile column 0 also goes to the step-0 pivot-column snapshot.
+  // S = Hpp_d + (pose-pose blocks) - sum_l Y_al W_bl^T over the eliminated planes, entry by entry (output-stationary): the
+  // diagonal block, then the pose-pose factor blocks in factor order, then the plane products in plane order.  Band layout:
+  // a bordered plane's rows hold W_al^T against its observers and its damped Hll block on the diagonal (0 against the other
+  // bordered planes).  Upper halves of diagonal tiles are 0, the padding is identity.  The first tile of each row also goes
+  // to the pivot-column snapshot of the step that first reads it (step first[i], parity first[i] & 1).
   __device__ void direct_assemble(double lambda) {
-    const int nb = G.dnb, n6 = 6 * G.N;
-    const long long total = (long long)nb * (nb + 1) / 2 * 2304;
-    int tprev = -1, ti = 0, tj = 0;
+    const int nb = G.dnb, n6 = 6 * G.N, np6 = 48 * G.dnbp;
+    const long long total = (long long)ldc(G.dtoff + nb) * 2304;
+    int tprev = -1, ti = 0, tj = 0, f0 = 0;
     for (long long idx = tid_team(); idx < total; idx += nthr_team()) {
       const int t = (int)(idx / 2304), e = (int)(idx - (long long)t * 2304), er = e / 48, ec = e - er * 48;
-      if (t != tprev) {
-        ti = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-        while (ti * (ti + 1) / 2 > t) ti--;
-        while ((ti + 1) * (ti + 2) / 2 <= t) ti++;
-        tj = t - ti * (ti + 1) / 2;
+      if (t != tprev) {   // tile row: the last one whose offset is <= t
+        int lo = 0, hi = nb - 1;
+        while (lo < hi) {
+          const int mid = (lo + hi + 1) >> 1;
+          if (ldc(G.dtoff + mid) <= t) lo = mid; else hi = mid - 1;
+        }
+        ti = lo;
+        f0 = ldc(G.dfirst + ti);
+        tj = f0 + t - ldc(G.dtoff + ti);
         tprev = t;
       }
       const int i = 48 * ti + er, j = 48 * tj + ec;
       double v = 0.0;
       if (j > i) {
         v = 0.0;
+      } else if (i >= np6) {   // a bordered plane's row
+        const int k = i - np6, kb = k / 3, m = k - kb * 3;
+        if (k >= 3 * G.dnbord) {
+          v = (i == j) ? 1.0 : 0.0;
+        } else if (j >= np6) {
+          if ((j - np6) / 3 == kb) {
+            const int cc = j - np6 - kb * 3;
+            v = ldc(G.Hll + (size_t)ldc(G.dbord + kb) * 9 + m * 3 + cc);
+            if (m == cc) v *= (1 + lambda);   // Cholesky.cpp:91-97
+          }
+        } else if (j < n6) {   // W_al of the incidence (pose b, plane): incidences are pose-ascending inside a plane
+          const int b = j / 6, r = j - b * 6;
+          int lo = ldc(G.dbinc + 2 * kb), hi = ldc(G.dbinc + 2 * kb + 1);
+          while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (ldc(G.pl_pose + ldc(G.dinc_lo + mid)) < b) lo = mid + 1; else hi = mid;
+          }
+          if (lo < ldc(G.dbinc + 2 * kb + 1) && ldc(G.pl_pose + ldc(G.dinc_lo + lo)) == b) v = ldc(G.Wd + (size_t)lo * 18 + r * 3 + m);
+        }
       } else if (i >= n6) {
         v = (i == j) ? 1.0 : 0.0;
       } else {
@@ -3095,7 +3125,7 @@ struct Phase {
           v = ldc(G.Hpp + (size_t)a * 36 + r * 6 + cc);
           if (r == cc) v *= (1 + lambda);   // Cholesky.cpp:91-97
         }
-        const size_t q = (size_t)a * (a + 1) / 2 + b;
+        const size_t q = dpair(a, b);
         for (int k = G.dfp_ptr[q]; k < G.dfp_ptr[q + 1]; k++) {
           const int fs = G.dfp_f[k], f = fs >> 1;
           v += (fs & 1) ? ldc(G.PF + (size_t)f * 120 + 72 + cc * 6 + r) : ldc(G.PF + (size_t)f * 120 + 72 + r * 6 + cc);
@@ -3107,8 +3137,27 @@ struct Phase {
         }
       }
       tile_at(G.Sd, t)[er * kAcLd + ec] = v;
-      if (tj == 0) tile_at(G.Dsnap, ti)[er * kAcLd + ec] = v;
+      if (tj == f0) tile_at(G.Dsnap + (size_t)(tj & 1) * nb * kAcTile, ti)[er * kAcLd + ec] = v;
     }
+  }
+
+  // band layout: b = [-gp + sum over the eliminated planes of Y_al g_l ; -g_l of the bordered planes].  The list of the pair
+  // (a, a) holds exactly one record (q, q) per eliminated incidence q of pose a, plane-ascending.  (The dense solve forms b in
+  // pose_phase, with every plane eliminated.)
+  __device__ void direct_rhs() {
+    const int n6 = 6 * G.N;
+    for (int i = tid_team(); i < n6; i += nthr_team()) {
+      const int a = i / 6, r = i - a * 6, q = dpair(a, a);
+      double v = -ldc(G.gp + i);
+      for (int k = G.dlp_ptr[q]; k < G.dlp_ptr[q + 1]; k++) {
+        const int inc = G.dlp_a[k];
+        const double* y = G.Yd + (size_t)inc * 18 + r * 3;
+        const double* g = G.gl + (size_t)G.dinc_plane[inc] * 3;
+        v += ldc(y) * ldc(g) + ldc(y + 1) * ldc(g + 1) + ldc(y + 2) * ldc(g + 2);
+      }
+      G.b[i] = v;
+    }
+    for (int k = tid_team(); k < 3 * G.dnbord; k += nthr_team()) G.b[n6 + k] = -ldc(G.gl + (size_t)ldc(G.dbord + k / 3) * 3 + k % 3);
   }
 
   // one CTA: A (48x48, lower half read) <- L = chol(A) with a zero upper half, Li <- L^-1.
@@ -3158,15 +3207,17 @@ struct Phase {
   }
 
   // S = L L^T in place, right-looking by tile columns, one team barrier per step.  Tile t belongs to CTA t % tsize.  Step K
-  // reads pivot column K only from its snapshot (published by the owners of those tiles at the end of step K-1, double-
-  // buffered by step parity), so the owners may overwrite it with L in the same step:
+  // visits the envelope only: the tile rows i with first[i] <= K and the trailing tiles (i, j) with first[j] <= K as well
+  // (L_jK = 0 otherwise).  It reads pivot column K only from its snapshot (published by the owners of those tiles at the end
+  // of step K-1, or by the assembly for the rows that start at column K; double-buffered by step parity), so the owners may
+  // overwrite it with L in the same step:
   //   panel     L_iK = C_i L_KK^-T
   //   trailing  A_ij <- A_ij - L_iK L_jK^T,  K < j <= i
   // on the FP64 tensor cores.  A CTA forms -L_iK once per tile row in which it owns a trailing tile and L_jK for every such
   // tile; each product reads only L_KK^-1 and snapshot tiles, so every CTA that forms it gets the same bits.  (A trailing
   // update through A_KK^-1 or L_KK^-1 alone, with one product per tile, loses backward stability when A_KK is ill-conditioned:
-  // DESIGN.md section 5.1.)  Look-ahead: the owner of tile (K+1, K+1) updates it first, factors it and publishes L_{K+1}^-1;
-  // step 0's pivot is factored by every CTA from the snapshot.
+  // DESIGN.md section 5.1.)  Look-ahead: the owner of tile (K+1, K+1) updates it first (unless row K+1 starts at column
+  // K+1), factors it and publishes L_{K+1}^-1; step 0's pivot is factored by every CTA from the snapshot.
   __device__ void direct_factor() {
     const int nb = G.dnb, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3;
     double* Li = reinterpret_cast<double*>(g_smem + kSmWork);
@@ -3231,17 +3282,22 @@ struct Phase {
       const int d = K + 1;
       int trow = -1, trowT = -1;   // tile rows whose C_i / T_i are in shared memory (T_i only once an owned trailing tile needs it)
       if (d < nb && dtile(d, d) % T == c.rank) {   // look-ahead
-        load_tile(Ci, tile_at(snap, d));
-        __syncthreads();
-        form_T();
-        store_tile(Cj, Ci);
-        __syncthreads();
-        double acc[3][2];
-        update(d, d, acc);
-        int r, cc;
+        const bool coupled = ldc(G.dfirst + d) <= K;
+        if (coupled) {
+          load_tile(Ci, tile_at(snap, d));
+          __syncthreads();
+          form_T();
+          store_tile(Cj, Ci);
+          __syncthreads();
+          double acc[3][2];
+          update(d, d, acc);
+          int r, cc;
 #pragma unroll
-        for (int s = 0; s < 3; s++)
-          if (frag(s, r, cc)) *reinterpret_cast<double2*>(Md + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+          for (int s = 0; s < 3; s++)
+            if (frag(s, r, cc)) *reinterpret_cast<double2*>(Md + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+        } else {   // row d starts at column d: its pivot is the assembled tile
+          load_tile(Md, tile_at(G.Sd, dtile(d, d)));
+        }
         // (Li of step K is needed below for the panel and T_i: keep a copy of it, then restore)
         __syncthreads();
         double* Lsave = Cj;
@@ -3251,14 +3307,18 @@ struct Phase {
         __syncthreads();
         store_tile(Li, Lsave);
         __syncthreads();
-        trow = trowT = d;
+        if (coupled) trow = trowT = d;
       }
-      for (int i = K; i < nb; i++) {
+      for (int p = ldc(G.dcol_ptr + K); p < ldc(G.dcol_ptr + K + 1); p++) {   // the rows i > K of column K
+        const int i = ldc(G.dcol_row + p);
         const int t0 = dtile(i, K);
         int j = K + ((c.rank - t0 % T) % T + T) % T;
         for (; j <= i; j += T) {
-          if (j == K && i == K) continue;                // the pivot: factored already
           if (i == d && j == d) continue;                // done by the look-ahead
+          if (j > K && ldc(G.dfirst + j) > K) {           // L_jK = 0: no update; step K+1 still reads the tile's snapshot
+            if (j == d) load_tile(tile_at(snapn, i), tile_at(G.Sd, dtile(i, d)));
+            continue;
+          }
           if (trow != i) {
             __syncthreads();
             load_tile(Ci, tile_at(snap, i));
@@ -3298,13 +3358,16 @@ struct Phase {
 
   // L y = b, then L^T x = y, blocked by tile row with the stored L_KK^-1; one team barrier per tile row.  Every CTA forms
   // y_K (x_K) itself from the finished part of the vector, then the team subtracts its contribution from the rows still open
-  // (each entry by one thread, in step order).  dvec[0] = the running right-hand side / x, dvec[1] = y.
+  // (each entry by one thread, in step order), within the envelope: forward, the rows of tile column K; backward, the tile
+  // columns first[K] .. K-1 of row K.  dvec[0] = the running right-hand side / x, dvec[1] = y.  b holds 6 N pose entries,
+  // then 3 per bordered plane.
   __device__ void direct_trsv() {
-    const int nb = G.dnb, n = 48 * nb, n6 = 6 * G.N, tid = threadIdx.x;
+    const int nb = G.dnb, n = 48 * nb, n6 = 6 * G.N, np6 = 48 * G.dnbp, tid = threadIdx.x;
     double* rv = G.dvec;
     double* yv = G.dvec + n;
     double* sv = reinterpret_cast<double*>(g_smem + kSmWork);   // [48] the vector piece of this step, [48] its product
-    for (int i = tid_team(); i < n; i += nthr_team()) rv[i] = (i < n6) ? ldc(G.b + i) : 0.0;
+    for (int i = tid_team(); i < n; i += nthr_team())
+      rv[i] = (i < n6) ? ldc(G.b + i) : ((i >= np6 && i < np6 + 3 * G.dnbord) ? ldc(G.b + n6 + i - np6) : 0.0);
     team_barrier(c);
     for (int K = 0; K < nb; K++) {   // forward: y_K = L_KK^-1 r_K;  r_J -= L_JK y_K  (J > K)
       const double* Li = tile_at(G.Dinv, K);
@@ -3317,8 +3380,10 @@ struct Phase {
         if (c.rank == 0) yv[48 * K + tid] = v;
       }
       __syncthreads();
-      for (int row = 48 * (K + 1) + tid_team(); row < n; row += nthr_team()) {
-        const double* Lr = tile_at(G.Sd, dtile(row / 48, K)) + (row % 48) * kAcLd;
+      const int p0 = ldc(G.dcol_ptr + K), nr = 48 * (ldc(G.dcol_ptr + K + 1) - p0);
+      for (int e = tid_team(); e < nr; e += nthr_team()) {
+        const int tr = ldc(G.dcol_row + p0 + e / 48), row = 48 * tr + e % 48;
+        const double* Lr = tile_at(G.Sd, dtile(tr, K)) + (row % 48) * kAcLd;
         double v = ldc(rv + row);
         for (int m = 0; m < 48; m++) v -= ldc(Lr + m) * sv[48 + m];
         rv[row] = v;
@@ -3337,7 +3402,7 @@ struct Phase {
         if (c.rank == 0) rv[48 * K + tid] = v;
       }
       __syncthreads();
-      for (int row = tid_team(); row < 48 * K; row += nthr_team()) {
+      for (int row = 48 * ldc(G.dfirst + K) + tid_team(); row < 48 * K; row += nthr_team()) {
         const double* Lc = tile_at(G.Sd, dtile(K, row / 48)) + (row % 48);
         double v = ldc(yv + row);
         for (int m = 0; m < 48; m++) v -= ldc(Lc + m * kAcLd) * sv[48 + m];
