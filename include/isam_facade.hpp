@@ -480,6 +480,10 @@ class Slam {
   // of a bordered system, graphs of any size within its device-memory budget; see pus_set_linear_solver.
   enum LinearSolver { LINEAR_SOLVER_PCG = 0, LINEAR_SOLVER_DIRECT = 1, LINEAR_SOLVER_BAND = 2 };
   void set_linear_solver(LinearSolver kind) { detail::check(pus_set_linear_solver(_h, (int)kind)); }
+  // order of the band solve's pose tiles (LINEAR_SOLVER_BAND only): insertion order (the default) or nested dissection, which
+  // keeps the fill low where a loop closure re-observes earlier planes; see pus_set_direct_ordering
+  enum Ordering { ORDERING_INSERTION = 0, ORDERING_NESTED_DISSECTION = 1 };
+  void set_direct_ordering(Ordering order) { detail::check(pus_set_direct_ordering(_h, (int)order)); }
   void add_node(Pose3d_Node* n) { n->_attach(_h); _nodes.push_back(n); }            // Slam.cpp:91-94
   void add_node(Plane3d_Node* n) { n->_attach(_h); _nodes.push_back(n); }
   void add_factor(Factor* f) {                                                      // Slam.cpp:96-105

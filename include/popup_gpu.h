@@ -32,7 +32,8 @@
  *   - the dense direct linear solver (pus_set_linear_solver(h, 1)) handles at most 640 live poses (a dense reduced system
  *     of order 3 840, about 65 MB of device memory); a larger graph fails at upload with a message and launches nothing.
  *     The band direct solver (kind 2) takes any graph whose envelope fits 8 GiB of device memory (tiles, snapshots, pivot
- *     inverses, vectors and tables; there is no fill-reducing reordering); a larger one fails at upload with a message
+ *     inverses, vectors and tables), in insertion order by default or, with pus_set_direct_ordering(h, 1), whose
+ *     nested-dissection tile pattern fits the same budget; a larger one fails at upload with a message
  *     stating the need and launches nothing.  Neither spans ranks: the pus_span_* entry points refuse a direct-mode handle.
  *   - the error / Jacobian export (pus_weighted_errors .. pus_local_chi2) evaluates at the estimate only (iSAM's default
  *     Selector ESTIMATE; LINPOINT is not provided) and writes caller-owned host arrays only.  Its indices are int32: a
@@ -190,7 +191,7 @@ int pus_set_jacobian_mode(pus_handle h, int numeric);
  * Cholesky (ISAM/isamlib/Cholesky.cpp:68-147) solves the same damped system.  kind 2: exact as kind 1, on the envelope of
  * a bordered system -- the poses in insertion order, then the few planes seen from most of the trajectory (chosen by
  * observer span, at most 64) kept as unknowns instead of being eliminated; the tiles outside the envelope are never stored,
- * factored or read (DESIGN.md section 5.2).  Every linear solve is bit-identical across
+ * factored or read (DESIGN.md section 5.2); pus_set_direct_ordering picks the order of kind 2's pose tiles.  Every linear solve is bit-identical across
  * team sizes, barrier kinds and batch positions; the chi2 and |delta| of the trace come from the team reduction, whose order
  * follows the team size, so whole runs agree bit for bit as long as no accept / reject decision is a tie in the last bits.  It applies to pus_batch_optimize (LM and GN), pus_update, pus_solve_resident
  * and the _many forms; a batch may mix all kinds (PCG and direct handles run as launches of their own).  In direct mode
@@ -205,6 +206,17 @@ int pus_set_jacobian_mode(pus_handle h, int numeric);
  * the solution to their dl. */
 int pus_set_linear_solver(pus_handle h, int kind);
 int pus_get_linear_solver(pus_handle h);   /* the kind, or < 0 on error */
+/* Order of the band solve's pose tiles (kind 2 only; a handle setting, accepted at any time).  order 0 (default): insertion
+ * order, the envelope layout.  order 1: nested dissection -- the 8-pose tiles permuted by recursive bisection of the tile
+ * graph (separators last, the bordered planes chosen by the number of pose tiles that see them and ordered after every
+ * pose), stored as L's tile pattern and factored level by level of the elimination tree (DESIGN.md section 5.3).  It keeps
+ * the fill near linear where insertion order has a wide envelope, as on a map whose loop closure re-observes earlier
+ * planes.  Other values are refused.  Changing it lays the graph out again at the next upload.  Debug hooks in order 1:
+ * "Sdir" and stages 4 / 5 keep the bordered order (a stored "Sdir" must lie inside the pattern), "Ldir" is the factor of
+ * P S P^T in the permuted order; "ndtile" (new column -> original tile), "ndparent", "ndcptr" / "ndcrow" (L's pattern per
+ * column), "ndlevel", "ndtoff" / "ndtrow" / "ndtcol" (tile storage) and "nduptr" / "ndupd" (update lists) fetch the tables. */
+int pus_set_direct_ordering(pus_handle h, int order);
+int pus_get_direct_ordering(pus_handle h);   /* the order, or < 0 on error */
 int pus_get_solver_options(pus_handle h, pus_solver_options* out);
 int pus_set_solver_options(pus_handle h, const pus_solver_options* in);
 

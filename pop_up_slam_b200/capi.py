@@ -381,6 +381,16 @@ class GpuGraphAPI(GraphAPI):
     def linear_solver_is_direct(self):
         return self.linear_solver_kind() == 1
 
+    def set_direct_ordering(self, order):
+        """Order of the band solve's pose tiles (kind 2 only): 0 insertion order (the default), 1 nested dissection."""
+        if not isinstance(order, (int, np.integer)) or isinstance(order, bool) or int(order) not in (0, 1):
+            raise ValueError(f"direct ordering: expected 0 (insertion order) or 1 (nested dissection), got {order!r}")
+        self._chk(self.lib.pus_set_direct_ordering(self.h, int(order)))
+
+    def direct_ordering(self):
+        """0 = insertion order, 1 = nested dissection."""
+        return self._chk(self.lib.pus_get_direct_ordering(self.h))
+
     def get_solver_options(self):
         o = SolverOptions()
         self._chk(self.lib.pus_get_solver_options(self.h, C.byref(o)))

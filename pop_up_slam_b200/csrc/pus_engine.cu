@@ -55,6 +55,7 @@ struct Solver {
   double robust_b = 1.0;
   int jac_numeric = 0;
   int linear_solver = 0;       // 0: PCG, 1: exact dense Cholesky of the reduced pose system, 2: exact band Cholesky (pus_set_linear_solver)
+  int ordering = 0;            // kind 2: 0 insertion order, 1 nested dissection (pus_set_direct_ordering)
   pus_solver_options opt;
   Compiled c;
   DirectTables dt;             // (direct mode only)
@@ -239,7 +240,7 @@ static int upload(Solver* s) {
     s->recycle_device();
     std::string err;
     if (!compile_graph(s->g, s->c, err)) { g_err = err; return -1; }
-    if (s->linear_solver != 0 && !build_direct(s->c, s->dt, err, s->linear_solver)) { g_err = err; return -1; }
+    if (s->linear_solver != 0 && !build_direct(s->c, s->dt, err, s->linear_solver, s->ordering)) { g_err = err; return -1; }
     const Compiled& c = s->c;
     if (kSmRc + 6 * c.nc * 8 > kSmemBytes) { g_err = "graph too large for the coarse-space shared-memory buffer"; return -1; }
     DevGraph& d = s->hd;
@@ -314,9 +315,16 @@ static int upload(Solver* s) {
       UPD(dlp_ptr, dt.lp_ptr); UPD(dlp_a, dt.lp_a); UPD(dlp_b, dt.lp_b); UPD(dfp_ptr, dt.fp_ptr); UPD(dfp_f, dt.fp_f);
       UPD(dfirst, dt.first); UPD(dtoff, dt.toff); UPD(dpoff, dt.poff); UPD(dcol_ptr, dt.col_ptr); UPD(dcol_row, dt.col_row);
       UPD(dbord, dt.border); UPD(dbinc, dt.binc);
+      size_t ntile = 0;
+      if (dt.order == 1) {
+        UPD(dnd, dt.nd_dev);
+        ntile = dt.nd_cptr[nb];
+      } else {
+        ntile = dt.toff[nb];
+      }
 #undef UPD
       AL(Wd, ninc * 18, "Wd"); AL(Yd, ninc * 18, "Yd");
-      AL(Sd, (size_t)dt.toff[nb] * kAcTile, nullptr); AL(Dsnap, 2 * nb * kAcTile, nullptr); AL(Dinv, nb * kAcTile, nullptr);
+      AL(Sd, ntile * kAcTile, nullptr); AL(Dsnap, dt.order == 1 ? 1 : 2 * nb * kAcTile, nullptr); AL(Dinv, nb * kAcTile, nullptr);
       AL(dvec, 2 * 48 * nb, nullptr);
       if (s->dalloc(&d.dflag, 1) < 0) return -1;
     }
@@ -868,6 +876,17 @@ int pus_set_linear_solver(pus_handle h, int kind) {
   return 0;
 }
 int pus_get_linear_solver(pus_handle h) { NEED(h); return SV(h)->linear_solver; }
+int pus_set_direct_ordering(pus_handle h, int order) {
+  NEED(h);
+  Solver* s = SV(h);
+  if (order < 0 || order > 1) { g_err = "bad direct ordering (0 = insertion order, 1 = nested dissection)"; return -1; }
+  if (order != s->ordering) {   // (only kind 2 lays the graph out by it; the next upload of a kind-2 handle lays it out again)
+    s->ordering = order;
+    s->g.topo_version++;
+  }
+  return 0;
+}
+int pus_get_direct_ordering(pus_handle h) { NEED(h); return SV(h)->ordering; }
 static int refuse_direct_span(Solver* s, const char* fn) {
   if (s->linear_solver == 0) return 0;
   g_err = std::string(fn) + ": the direct linear solvers do not span ranks (set the PCG solver, kind 0)";
@@ -1655,6 +1674,13 @@ int pus_load_isam_dataset(pus_handle h, const char* path, int* n_poses, int* n_f
 // order of the direct solve's system without padding (6 N, then 3 per bordered plane), and row r's row in the padded layout
 static int direct_order(const Solver* s) { return 6 * s->c.N + 3 * (int)s->dt.border.size(); }
 static int direct_row(const Solver* s, int r) { return r < 6 * s->c.N ? r : 48 * s->dt.nbp + r - 6 * s->c.N; }
+// nested-dissection layout: row r's row in the permuted padded order, and the stored tile (i, j), i >= j, or -1 outside L's pattern
+static int nd_row(const Solver* s, int r) { const int p = direct_row(s, r); return 48 * s->dt.nd_pos[p / 48] + p % 48; }
+static long long nd_tile(const DirectTables& dt, int i, int j) {
+  const int* b = dt.nd_crow.data();
+  const int* at = std::lower_bound(b + dt.nd_cptr[j], b + dt.nd_cptr[j + 1], i);
+  return (at == b + dt.nd_cptr[j + 1] || *at != i) ? -1 : dt.nd_toff[j] + (at - (b + dt.nd_cptr[j]));
+}
 
 long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long cap) {
   NEED(h);
@@ -1701,6 +1727,18 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
   if (nm == "bborder") return ints(s->dt.border);
   if (nm == "bfirst") return ints(s->dt.first);
   if (nm == "bbytes") { if (cap >= 1) out[0] = (double)s->dt.bytes; return 1; }
+  // nested-dissection layout: the tile order (new column -> original tile), the elimination tree, L's pattern, the levels,
+  // the tile storage (per column its diagonal tile's index; per tile its row and column) and the update lists
+  if (nm == "ndtile") return ints(s->dt.nd_perm);
+  if (nm == "ndparent") return ints(s->dt.nd_parent);
+  if (nm == "ndcptr") return ints(s->dt.nd_cptr);
+  if (nm == "ndcrow") return ints(s->dt.nd_crow);
+  if (nm == "ndlevel") return ints(s->dt.nd_level);
+  if (nm == "ndtoff") return ints(s->dt.nd_toff);
+  if (nm == "ndtrow") return ints(s->dt.nd_trow);
+  if (nm == "ndtcol") return ints(s->dt.nd_tcol);
+  if (nm == "nduptr") return ints(s->dt.nd_uptr);
+  if (nm == "ndupd") return ints(s->dt.nd_upd);
   if (nm == "pf_i") return ints(c.pf_i);
   if (nm == "pf_j") return ints(c.pf_j);
   if (nm == "pl_pose") return ints(c.pl_pose);
@@ -1728,11 +1766,21 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
     if (s->linear_solver == 0) { g_err = "not in direct linear-solver mode"; return -1; }
     const DirectTables& dt = s->dt;
     const int n = direct_order(s);   // (band: 6 N pose rows, then 3 per bordered plane, padding stripped)
-    const size_t total = (size_t)dt.toff[dt.nb] * kAcTile;
+    const size_t total = (size_t)(dt.order == 1 ? dt.nd_cptr[dt.nb] : dt.toff[dt.nb]) * kAcTile;
     std::vector<double> tmp(total);
     if (cudaMemcpy(tmp.data(), s->hd.Sd, total * 8, cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
     const long long cnt = (long long)n * n;
-    if (cnt <= cap)
+    if (cnt <= cap && dt.order == 1) {   // Sdir in the bordered order; Ldir, the factor of P S P^T, in the permuted order
+      std::vector<int> nr(n), rows(n);
+      for (int r = 0; r < n; r++) { nr[r] = nd_row(s, r); rows[r] = r; }
+      if (nm == "Ldir") std::sort(rows.begin(), rows.end(), [&](int x, int y) { return nr[x] < nr[y]; });
+      for (int a = 0; a < n; a++)
+        for (int b = 0; b < n; b++) {
+          const int I = std::max(nr[rows[a]], nr[rows[b]]), J = std::min(nr[rows[a]], nr[rows[b]]);
+          const long long t = (b > a) ? -1 : nd_tile(dt, I / 48, J / 48);
+          out[(size_t)a * n + b] = t < 0 ? 0.0 : tmp[(size_t)t * kAcTile + (I % 48) * kAcLd + J % 48];
+        }
+    } else if (cnt <= cap)
       for (int r = 0; r < n; r++)
         for (int q = 0; q < n; q++) {
           const int pr = direct_row(s, r), pq = direct_row(s, q), ti = pr / 48, tj = pq / 48;
@@ -1790,6 +1838,32 @@ long long pus_debug_store(pus_handle h, const char* name, const double* in, long
     }
     std::vector<int> orig(48 * nb, -1);   // padded row -> row of the stored matrix (-1: padding)
     for (int r = 0; r < n; r++) orig[direct_row(s, r)] = r;
+    if (dt.order == 1) {   // nested dissection: tile (i, j) of the new order holds P S P^T, lower half
+      for (int r = 0; r < n; r++)
+        for (int q = 0; q < r; q++) {
+          const int I = std::max(nd_row(s, r), nd_row(s, q)), J = std::min(nd_row(s, r), nd_row(s, q));
+          if (in[(size_t)r * n + q] != 0.0 && nd_tile(dt, I / 48, J / 48) < 0) {
+            g_err = "Sdir: entry (" + std::to_string(r) + ", " + std::to_string(q) + ") lies outside the nested-dissection pattern";
+            return -1;
+          }
+        }
+      const int T = dt.nd_cptr[nb];
+      std::vector<double> tiles((size_t)T * kAcTile, 0.0);
+      for (int t = 0; t < T; t++) {
+        const int ti = dt.nd_trow[t], tj = dt.nd_tcol[t];
+        for (int er = 0; er < 48; er++)
+          for (int ec = 0; ec < 48; ec++) {
+            const int oi = orig[48 * dt.nd_perm[ti] + er], oj = orig[48 * dt.nd_perm[tj] + ec];
+            double v = 0.0;
+            if (ti == tj && ec > er) v = 0.0;
+            else if (oi < 0 || oj < 0) v = (ti == tj && er == ec) ? 1.0 : 0.0;   // identity padding
+            else v = in[(size_t)std::max(oi, oj) * n + std::min(oi, oj)];
+            tiles[(size_t)t * kAcTile + er * kAcLd + ec] = v;
+          }
+      }
+      if (cudaMemcpy(s->hd.Sd, tiles.data(), tiles.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) { g_err = "memcpy"; return -1; }
+      return count;
+    }
     for (int r = 0; r < n; r++)
       for (int q = 0; q < r; q++)
         if (in[(size_t)r * n + q] != 0.0 && direct_row(s, q) / 48 < dt.first[direct_row(s, r) / 48]) {
@@ -1834,7 +1908,7 @@ int pus_debug_compile(pus_handle h) {
   Solver* s = SV(h);
   std::string err;
   if (!compile_graph(s->g, s->c, err)) { g_err = err; return -1; }
-  if (s->linear_solver != 0 && !build_direct(s->c, s->dt, err, s->linear_solver)) { g_err = err; return -1; }
+  if (s->linear_solver != 0 && !build_direct(s->c, s->dt, err, s->linear_solver, s->ordering)) { g_err = err; return -1; }
   return 0;
 }
 

@@ -670,7 +670,246 @@ struct DirectTables {
   std::vector<int> col_ptr, col_row;    // per tile column K: the tile rows i > K with first[i] <= K, ascending
   std::vector<int> border, binc;        // bordered planes (ascending); [lo, hi) of each one's incidences
   long long bytes = 0;                  // device memory of the solve's tiles, vectors and tables
+  // nested-dissection layout (kind 2, order 1; empty otherwise): tile columns are numbered in the new order.  Tiles are stored
+  // level by level, the columns of a level ascending, each column's tiles row-ascending (its diagonal tile first).
+  int order = 0;                        // 0: insertion order (the envelope above), 1: nested dissection
+  int nlev = 0;                         // levels of the elimination tree
+  long long nupd = 0;                   // tile products of one factorization (update-list entries)
+  std::vector<int> nd_perm, nd_pos;     // new column -> original tile, original tile -> new column
+  std::vector<int> nd_parent, nd_level; // per column: elimination-tree parent (-1: a root), level (0: a leaf)
+  std::vector<int> nd_cptr, nd_crow;    // per column j: the tile rows i >= j of L's pattern, ascending
+  std::vector<int> nd_toff;             // per column: storage index of its diagonal tile (its tiles follow it)
+  std::vector<int> nd_lptr, nd_lcol, nd_ltptr;   // per level: its columns (ascending), its tile range
+  std::vector<int> nd_trow, nd_tcol;    // per stored tile: tile row, tile column
+  std::vector<int> nd_uptr, nd_upd;     // per stored tile (i, j): pairs (tile of L_iK, tile of L_jK), K < j ascending
+  std::vector<int> nd_rptr, nd_rtile;   // per tile row j: the tiles (j, K), K < j ascending
+  std::vector<int> nd_dev;              // the tables above that the device reads, packed (NdTable)
 };
+
+// ---- nested-dissection order of the pose tiles (kind 2, order 1) ----
+// Connected components one after another (by their lowest tile); a component is bisected by the BFS level structure from a
+// pseudo-peripheral tile: the separator is the tiles of the median level adjacent to the level after it, ordered after both
+// halves.  Parts of at most kNdLeaf tiles, and parts whose level structure has fewer than three levels, keep insertion order.
+constexpr int kNdLeaf = 4;
+// the ND tables the device reads, packed into one array (DirectTables::nd_dev): entry 0 the number of levels, entries 1 .. 13
+// the offsets of the tables
+enum NdTable { ND_NLEV = 0, ND_POS, ND_PERM, ND_LPTR, ND_LCOL, ND_LTPTR, ND_TOFF, ND_CPTR, ND_TROW, ND_TCOL, ND_UPTR, ND_UPD,
+               ND_RPTR, ND_RTILE, ND_HDR };
+
+struct NdOrder {
+  const std::vector<std::vector<int>>& adj;
+  std::vector<int> in, comp, seen, lev, out;
+  int stamp = 0, vstamp = 0;
+  explicit NdOrder(const std::vector<std::vector<int>>& a)
+      : adj(a), in(a.size(), 0), comp(a.size(), 0), seen(a.size(), 0), lev(a.size(), 0) {}
+
+  // BFS level structure from r inside the part stamped s: tiles level by level (each level ascending), level pointers
+  void bfs(int r, int s, std::vector<int>& q, std::vector<int>& lp) {
+    vstamp++;
+    q.assign(1, r); lp.assign(1, 0);
+    seen[r] = vstamp; lev[r] = 0;
+    size_t h = 0;
+    while (h < q.size()) {
+      const size_t e = q.size();
+      lp.push_back((int)e);
+      for (; h < e; h++)
+        for (int u : adj[q[h]])
+          if (in[u] == s && seen[u] != vstamp) { seen[u] = vstamp; lev[u] = lev[q[h]] + 1; q.push_back(u); }
+      std::sort(q.begin() + e, q.end());
+    }
+  }
+  void dissect(std::vector<int> S) {   // S ascending
+    if ((int)S.size() <= kNdLeaf) { out.insert(out.end(), S.begin(), S.end()); return; }
+    const int s = ++stamp;
+    for (int t : S) in[t] = s;
+    std::vector<int> q, lp;
+    {   // components
+      std::vector<std::vector<int>> comps;
+      for (int t : S) {
+        if (comp[t] == s) continue;
+        bfs(t, s, q, lp);
+        for (int u : q) comp[u] = s;
+        std::sort(q.begin(), q.end());
+        comps.push_back(q);
+      }
+      if (comps.size() > 1) { for (auto& cpt : comps) dissect(cpt); return; }
+    }
+    // pseudo-peripheral tile: from the lowest tile, move to the lowest tile of the last level while the depth grows
+    int v = S[0];
+    bfs(v, s, q, lp);
+    for (;;) {
+      const int h = (int)lp.size() - 1, u = q[lp[h - 1]];
+      std::vector<int> q2, lp2;
+      bfs(u, s, q2, lp2);
+      if ((int)lp2.size() - 1 <= h) { bfs(v, s, q, lp); break; }
+      v = u; q.swap(q2); lp.swap(lp2);
+    }
+    const int h = (int)lp.size() - 1;
+    if (h <= 2) { out.insert(out.end(), S.begin(), S.end()); return; }
+    int m = 0;   // the level holding the median tile, kept off both ends
+    while (2 * lp[m + 1] < (int)S.size()) m++;
+    m = std::max(1, std::min(h - 2, m));
+    std::vector<int> A, B, sep;
+    for (int k = 0; k < lp[m]; k++) A.push_back(q[k]);
+    for (int k = lp[m]; k < lp[m + 1]; k++) {
+      bool far = false;
+      for (int u : adj[q[k]]) if (in[u] == s && seen[u] == vstamp && lev[u] == m + 1) { far = true; break; }
+      (far ? sep : A).push_back(q[k]);
+    }
+    for (int k = lp[m + 1]; k < (int)q.size(); k++) B.push_back(q[k]);
+    std::sort(A.begin(), A.end()); std::sort(B.begin(), B.end());
+    dissect(A);
+    dissect(B);
+    out.insert(out.end(), sep.begin(), sep.end());
+  }
+};
+
+// Symbolic Cholesky at tile granularity of the matrix whose lower pattern is alow (per column j: rows i > j, any order):
+// column patterns (ascending, diagonal first), elimination-tree parents and levels.  Returns the number of levels.
+inline int nd_symbolic(int nb, std::vector<std::vector<int>>& alow, std::vector<int>& cptr, std::vector<int>& crow,
+                       std::vector<int>& parent, std::vector<int>& level) {
+  std::vector<std::vector<int>> kids(nb);
+  std::vector<int> mark(nb, -1), col;
+  cptr.assign(nb + 1, 0); crow.clear(); parent.assign(nb, -1); level.assign(nb, 0);
+  int nlev = 0;
+  for (int j = 0; j < nb; j++) {
+    col.assign(1, j); mark[j] = j;
+    for (int i : alow[j]) if (mark[i] != j) { mark[i] = j; col.push_back(i); }
+    for (int c : kids[j]) {
+      for (int p = cptr[c] + 1; p < cptr[c + 1]; p++) {
+        const int i = crow[p];
+        if (i != j && mark[i] != j) { mark[i] = j; col.push_back(i); }
+      }
+      level[j] = std::max(level[j], level[c] + 1);
+    }
+    std::sort(col.begin(), col.end());
+    crow.insert(crow.end(), col.begin(), col.end());
+    cptr[j + 1] = (int)crow.size();
+    if (col.size() > 1) { parent[j] = col[1]; kids[col[1]].push_back(j); }
+    nlev = std::max(nlev, level[j] + 1);
+  }
+  return nlev;
+}
+
+// The nested-dissection layout that borders the planes with bslot >= 0 (nbord of them): the tile order (new -> original),
+// L's pattern, and the device bytes it takes
+inline long long nd_layout(const Compiled& c, const std::vector<int>& inc_ptr, const std::vector<int>& inc_pose,
+                           const std::vector<int>& bslot, int nbord, DirectTables& d) {
+  const int N = c.N, M = c.M;
+  const int nbp = std::max(1, (6 * N + 47) / 48), nb = nbp + (3 * nbord + 47) / 48;
+  d.nbp = nbp; d.nb = nb;
+  // pose-tile graph: a pose-pose factor, or an eliminated plane seen from both tiles
+  std::vector<std::vector<int>> adj(nbp), bt(nb);   // bt[t]: pose tiles coupled to bordered tile t
+  long long lp = 0, fp = 0;
+  for (int f = 0; f < c.Epf; f++) {
+    if (c.pf_j[f] < 0) continue;
+    fp++;
+    const int u = c.pf_i[f] / 8, v = c.pf_j[f] / 8;
+    if (u != v) { adj[u].push_back(v); adj[v].push_back(u); }
+  }
+  std::vector<int> tl;
+  for (int l = 0; l < M; l++) {
+    const int n = inc_ptr[l + 1] - inc_ptr[l];
+    if (n == 0) continue;
+    tl.clear();
+    for (int i = inc_ptr[l]; i < inc_ptr[l + 1]; i++) if (tl.empty() || tl.back() != inc_pose[i] / 8) tl.push_back(inc_pose[i] / 8);
+    if (bslot[l] >= 0) {
+      std::vector<int>& b = bt[nbp + 3 * bslot[l] / 48];
+      b.insert(b.end(), tl.begin(), tl.end());
+      continue;
+    }
+    lp += (long long)n * (n + 1) / 2;
+    for (int u : tl)
+      for (int v : tl) if (u != v) adj[u].push_back(v);
+  }
+  for (auto& a : adj) { std::sort(a.begin(), a.end()); a.erase(std::unique(a.begin(), a.end()), a.end()); }
+  NdOrder nd(adj);
+  std::vector<int> all(nbp);
+  for (int t = 0; t < nbp; t++) all[t] = t;
+  nd.dissect(all);
+  d.nd_perm = nd.out;
+  for (int t = nbp; t < nb; t++) d.nd_perm.push_back(t);   // bordered tiles last: the root of the elimination tree
+  d.nd_pos.assign(nb, 0);
+  for (int j = 0; j < nb; j++) d.nd_pos[d.nd_perm[j]] = j;
+  std::vector<std::vector<int>> alow(nb);
+  auto couple = [&](int u, int v) {
+    const int a = d.nd_pos[u], b = d.nd_pos[v];
+    if (a > b) alow[b].push_back(a); else if (b > a) alow[a].push_back(b);
+  };
+  for (int u = 0; u < nbp; u++) for (int v : adj[u]) if (v > u) couple(u, v);
+  for (int t = nbp; t < nb; t++) for (int u : bt[t]) couple(t, u);
+  d.nlev = nd_symbolic(nb, alow, d.nd_cptr, d.nd_crow, d.nd_parent, d.nd_level);
+  const long long T = d.nd_cptr[nb];
+  d.nupd = 0;
+  for (int j = 0; j < nb; j++) { const long long m = d.nd_cptr[j + 1] - d.nd_cptr[j] - 1; d.nupd += m * (m + 1) / 2; }
+  const long long ninc = (long long)inc_pose.size();
+  const long long ints = 5ll * nb + 2ll * d.nlev + 132 * T + 2 * d.nupd + 2 * lp + fp + 3 * ninc + 3ll * nbord + 7 + ND_HDR;
+  return (T + nb) * kDirectTileBytes                                 // tiles, pivot inverses
+         + 8 * (2ll * 48 * nb + 36 * ninc + 3ll * nbord) + 4 * ints;   // solve vectors, W / Y per incidence, border rhs, tables
+}
+
+// the device tables of the chosen nested-dissection layout: tile storage by level, update lists, row lists
+inline void nd_tables(DirectTables& d) {
+  const int nb = d.nb;
+  d.nd_lptr.assign(d.nlev + 1, 0);
+  for (int j = 0; j < nb; j++) d.nd_lptr[d.nd_level[j] + 1]++;
+  for (int l = 0; l < d.nlev; l++) d.nd_lptr[l + 1] += d.nd_lptr[l];
+  d.nd_lcol.assign(nb, 0);
+  {
+    std::vector<int> fill(d.nd_lptr.begin(), d.nd_lptr.end() - 1);
+    for (int j = 0; j < nb; j++) d.nd_lcol[fill[d.nd_level[j]]++] = j;
+  }
+  const int T = d.nd_cptr[nb];
+  d.nd_toff.assign(nb, 0); d.nd_ltptr.assign(d.nlev + 1, 0);
+  d.nd_trow.assign(T, 0); d.nd_tcol.assign(T, 0);
+  int t = 0;
+  for (int l = 0; l < d.nlev; l++) {
+    d.nd_ltptr[l] = t;
+    for (int k = d.nd_lptr[l]; k < d.nd_lptr[l + 1]; k++) {
+      const int j = d.nd_lcol[k];
+      d.nd_toff[j] = t;
+      for (int p = d.nd_cptr[j]; p < d.nd_cptr[j + 1]; p++, t++) { d.nd_trow[t] = d.nd_crow[p]; d.nd_tcol[t] = j; }
+    }
+  }
+  d.nd_ltptr[d.nlev] = t;
+  auto tile = [&](int i, int j) {   // the stored tile (i, j), i >= j inside the pattern
+    const int* b = d.nd_crow.data();
+    return d.nd_toff[j] + (int)(std::lower_bound(b + d.nd_cptr[j], b + d.nd_cptr[j + 1], i) - (b + d.nd_cptr[j]));
+  };
+  d.nd_uptr.assign(T + 1, 0);
+  d.nd_rptr.assign(nb + 1, 0);
+  for (int pass = 0; pass < 2; pass++) {
+    std::vector<int> fill, rfill;
+    if (pass == 1) {
+      for (int q = 0; q < T; q++) d.nd_uptr[q + 1] += d.nd_uptr[q];
+      for (int j = 0; j < nb; j++) d.nd_rptr[j + 1] += d.nd_rptr[j];
+      d.nd_upd.assign(std::max(2, 2 * d.nd_uptr[T]), 0);
+      d.nd_rtile.assign(std::max(1, d.nd_rptr[nb]), 0);
+      fill.assign(d.nd_uptr.begin(), d.nd_uptr.end() - 1);
+      rfill.assign(d.nd_rptr.begin(), d.nd_rptr.end() - 1);
+    }
+    for (int K = 0; K < nb; K++) {   // ascending K: every list comes out K-ascending
+      const int p0 = d.nd_cptr[K] + 1, p1 = d.nd_cptr[K + 1], t0 = d.nd_toff[K] + 1 - p0;
+      for (int a = p0; a < p1; a++) {
+        const int i = d.nd_crow[a];
+        if (pass == 0) d.nd_rptr[i + 1]++; else d.nd_rtile[rfill[i]++] = t0 + a;
+        for (int b = p0; b <= a; b++) {
+          const int q = tile(i, d.nd_crow[b]);
+          if (pass == 0) d.nd_uptr[q + 1]++;
+          else { const int at = fill[q]++; d.nd_upd[2 * at] = t0 + a; d.nd_upd[2 * at + 1] = t0 + b; }
+        }
+      }
+    }
+  }
+  const std::vector<int>* tab[ND_HDR] = {nullptr, &d.nd_pos, &d.nd_perm, &d.nd_lptr, &d.nd_lcol, &d.nd_ltptr, &d.nd_toff,
+                                         &d.nd_cptr, &d.nd_trow, &d.nd_tcol, &d.nd_uptr, &d.nd_upd, &d.nd_rptr, &d.nd_rtile};
+  d.nd_dev.assign(ND_HDR, 0);
+  d.nd_dev[ND_NLEV] = d.nlev;
+  for (int k = 1; k < ND_HDR; k++) {
+    d.nd_dev[k] = (int)d.nd_dev.size();
+    d.nd_dev.insert(d.nd_dev.end(), tab[k]->begin(), tab[k]->end());
+  }
+}
 
 // first[] of a layout that borders the planes with bslot >= 0 (nbord of them), and the device bytes it takes
 inline long long band_envelope(const Compiled& c, const std::vector<int>& inc_ptr, const std::vector<int>& inc_pose,
@@ -711,8 +950,97 @@ inline long long band_envelope(const Compiled& c, const std::vector<int>& inc_pt
          + 8 * (2ll * 48 * nb + 36 * ninc + 3ll * nbord) + 4 * ints;   // solve vectors, W / Y per incidence, border rhs, tables
 }
 
-// kind 1: dense (at most kDirectMaxPoses poses); kind 2: band, within kBandBudgetBytes
-inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err, int kind = 1) {
+// kind 2, order 1: the nested-dissection layout.  Bordering: the k planes seen from the most distinct pose tiles (ties: lower
+// index), k = 0 .. min(M, 64), whichever k takes the fewest device bytes (ties: the smaller k).  A revisited plane has a wide
+// span but a small clique, so the span rule of the insertion order is the wrong measure here.
+inline bool build_nd(const Compiled& c, DirectTables& d, std::string& err, const std::vector<int>& inc_ptr) {
+  const int N = c.N, M = c.M;
+  std::vector<int> ntile(M, 0), order(M);
+  for (int l = 0; l < M; l++) {
+    int last = -1;
+    for (int i = inc_ptr[l]; i < inc_ptr[l + 1]; i++)
+      if (d.inc_pose[i] / 8 != last) { last = d.inc_pose[i] / 8; ntile[l]++; }
+    order[l] = l;
+  }
+  std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return ntile[x] > ntile[y]; });
+  long long best = -1;
+  int best_k = 0;
+  std::vector<int> bs(M, -1);
+  for (int k = 0; k <= std::min(M, kBandMaxBorder); k++) {
+    std::fill(bs.begin(), bs.end(), -1);
+    std::vector<int> chosen(order.begin(), order.begin() + k);
+    std::sort(chosen.begin(), chosen.end());
+    for (int q = 0; q < k; q++) bs[chosen[q]] = q;
+    DirectTables t;
+    const long long bytes = nd_layout(c, inc_ptr, d.inc_pose, bs, k, t);
+    if (best < 0 || bytes < best) { best = bytes; best_k = k; }
+  }
+  d.border.assign(order.begin(), order.begin() + best_k);
+  std::sort(d.border.begin(), d.border.end());
+  std::fill(bs.begin(), bs.end(), -1);
+  for (int q = 0; q < best_k; q++) bs[d.border[q]] = q;
+  d.bytes = nd_layout(c, inc_ptr, d.inc_pose, bs, best_k, d);
+  if (d.bytes > kBandBudgetBytes) {
+    err = "band linear solver (nested-dissection order): the graph needs " + std::to_string(d.bytes) + " bytes of device memory (" +
+          std::to_string(N) + " poses, " + std::to_string(best_k) + " bordered planes, " + std::to_string(d.nd_cptr[d.nb]) +
+          " tiles); the budget is " + std::to_string(kBandBudgetBytes) + " bytes (use the PCG solver, kind 0)";
+    return false;
+  }
+  for (int q = 0; q < best_k; q++) { d.binc.push_back(inc_ptr[d.border[q]]); d.binc.push_back(inc_ptr[d.border[q] + 1]); }
+  nd_tables(d);
+  // per-pose-pair lists: pair (a, b), a >= b in insertion order, of the stored tile t that holds it, at 64 t + 8 (a % 8) + b % 8
+  auto pair = [&](int a, int b) {
+    int i = d.nd_pos[a / 8], j = d.nd_pos[b / 8];
+    if (i < j) std::swap(i, j);
+    const int* r = d.nd_crow.data();
+    const int t = d.nd_toff[j] + (int)(std::lower_bound(r + d.nd_cptr[j], r + d.nd_cptr[j + 1], i) - (r + d.nd_cptr[j]));
+    return (size_t)64 * t + 8 * (a % 8) + b % 8;
+  };
+  const size_t np = (size_t)64 * d.nd_cptr[d.nb];
+  d.lp_ptr.assign(np + 1, 0);
+  for (int pass = 0; pass < 2; pass++) {
+    std::vector<int> fill;
+    if (pass == 1) {
+      for (size_t q = 0; q < np; q++) d.lp_ptr[q + 1] += d.lp_ptr[q];
+      d.lp_a.assign(std::max(1, d.lp_ptr[np]), 0);
+      d.lp_b.assign(std::max(1, d.lp_ptr[np]), 0);
+      fill.assign(d.lp_ptr.begin(), d.lp_ptr.end() - 1);
+    }
+    for (int l = 0; l < M; l++) {
+      if (bs[l] >= 0) continue;
+      for (int i = inc_ptr[l]; i < inc_ptr[l + 1]; i++)
+        for (int j = inc_ptr[l]; j <= i; j++) {
+          const size_t q = pair(d.inc_pose[i], d.inc_pose[j]);
+          if (pass == 0) d.lp_ptr[q + 1]++;
+          else { const int at = fill[q]++; d.lp_a[at] = i; d.lp_b[at] = j; }
+        }
+    }
+  }
+  d.fp_ptr.assign(np + 1, 0);
+  for (int pass = 0; pass < 2; pass++) {
+    std::vector<int> fill;
+    if (pass == 1) {
+      for (size_t q = 0; q < np; q++) d.fp_ptr[q + 1] += d.fp_ptr[q];
+      d.fp_f.assign(std::max(1, d.fp_ptr[np]), 0);
+      fill.assign(d.fp_ptr.begin(), d.fp_ptr.end() - 1);
+    }
+    for (int f = 0; f < c.Epf; f++) {
+      if (c.pf_j[f] < 0) continue;
+      for (int side = 0; side < 2; side++) {
+        const int a = side ? c.pf_j[f] : c.pf_i[f], b = side ? c.pf_i[f] : c.pf_j[f];
+        if (a < b) continue;
+        const size_t q = pair(a, b);
+        if (pass == 0) d.fp_ptr[q + 1]++;
+        else d.fp_f[fill[q]++] = f * 2 + side;
+      }
+    }
+  }
+  return true;
+}
+
+// kind 1: dense (at most kDirectMaxPoses poses); kind 2: band, within kBandBudgetBytes, in insertion order (order 0) or
+// nested-dissection order (order 1)
+inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err, int kind = 1, int order = 0) {
   d = DirectTables();
   const int N = c.N, M = c.M;
   if (kind == 1 && N > kDirectMaxPoses) {
@@ -729,6 +1057,11 @@ inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err, i
       s = e;
     }
     inc_ptr[l + 1] = (int)d.inc_pose.size();
+  }
+  if (kind == 2 && order == 1) {
+    d.order = 1;
+    if (!build_nd(c, d, err, inc_ptr)) { d = DirectTables(); return false; }
+    return true;
   }
   std::vector<int> bslot(M, -1);
   if (kind == 1) {

@@ -135,6 +135,9 @@ struct DevGraph {
   double *Dinv;          // [dnb] L_KK^-1
   double *dvec;          // [2][48 dnb] triangular-solve vectors
   unsigned* dflag;       // set when a pivot is not positive
+  // nested-dissection layout (null otherwise): its tables packed into one array (pus_graph.hpp, NdTable; nd(k) below); the
+  // pose-pair lists are indexed 64 t + 8 (a % 8) + b % 8 by the stored tile t of the pair; the envelope tables above are unused
+  const int* dnd;
 };
 
 // The graph descriptor of the solve in progress and the dynamic shared memory, named at namespace scope so that every
@@ -3053,6 +3056,7 @@ struct Phase {
   __device__ __forceinline__ static int dpair(int a, int b) { return ldc(G.dpoff + a) + b - 8 * ldc(G.dfirst + a / 8); }
   template <typename T>
   __device__ __forceinline__ static T* tile_at(T* base, int t) { return base + (size_t)t * kAcTile; }
+  __device__ __forceinline__ static const int* nd(int k) { return G.dnd + ldc(G.dnd + k); }   // table k of the ND layout
 
   // W_al = sum of the (pose a, plane l) edges' W blocks in slot order, Y_al = W_al Hll_d^-1
   __device__ void direct_wy() {
@@ -3077,7 +3081,55 @@ struct Phase {
   // a bordered plane's rows hold W_al^T against its observers and its damped Hll block on the diagonal (0 against the other
   // bordered planes).  Upper halves of diagonal tiles are 0, the padding is identity.  The first tile of each row also goes
   // to the pivot-column snapshot of the step that first reads it (step first[i], parity first[i] & 1).
+  // Entry (i, j), i >= j, of S in the bordered order, as direct_assemble forms it; q(a, b) is the index of the pose pair's lists.
+  // (The insertion-order assembly keeps its own copy of this formula inline, so that its kernel compiles as before.)
+  template <typename Pair>
+  __device__ __forceinline__ static double direct_entry(int i, int j, double lambda, Pair pair) {
+    const int n6 = 6 * G.N, np6 = 48 * G.dnbp;
+    double v = 0.0;
+    if (i >= np6) {   // a bordered plane's row
+      const int k = i - np6, kb = k / 3, m = k - kb * 3;
+      if (k >= 3 * G.dnbord) {
+        v = (i == j) ? 1.0 : 0.0;
+      } else if (j >= np6) {
+        if ((j - np6) / 3 == kb) {
+          const int cc = j - np6 - kb * 3;
+          v = ldc(G.Hll + (size_t)ldc(G.dbord + kb) * 9 + m * 3 + cc);
+          if (m == cc) v *= (1 + lambda);   // Cholesky.cpp:91-97
+        }
+      } else if (j < n6) {   // W_al of the incidence (pose b, plane): incidences are pose-ascending inside a plane
+        const int b = j / 6, r = j - b * 6;
+        int lo = ldc(G.dbinc + 2 * kb), hi = ldc(G.dbinc + 2 * kb + 1);
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          if (ldc(G.pl_pose + ldc(G.dinc_lo + mid)) < b) lo = mid + 1; else hi = mid;
+        }
+        if (lo < ldc(G.dbinc + 2 * kb + 1) && ldc(G.pl_pose + ldc(G.dinc_lo + lo)) == b) v = ldc(G.Wd + (size_t)lo * 18 + r * 3 + m);
+      }
+    } else if (i >= n6) {
+      v = (i == j) ? 1.0 : 0.0;
+    } else {
+      const int a = i / 6, r = i - a * 6, b = j / 6, cc = j - b * 6;
+      if (a == b) {
+        v = ldc(G.Hpp + (size_t)a * 36 + r * 6 + cc);
+        if (r == cc) v *= (1 + lambda);   // Cholesky.cpp:91-97
+      }
+      const size_t q = pair(a, b);
+      for (int k = G.dfp_ptr[q]; k < G.dfp_ptr[q + 1]; k++) {
+        const int fs = G.dfp_f[k], f = fs >> 1;
+        v += (fs & 1) ? ldc(G.PF + (size_t)f * 120 + 72 + cc * 6 + r) : ldc(G.PF + (size_t)f * 120 + 72 + r * 6 + cc);
+      }
+      for (int k = G.dlp_ptr[q]; k < G.dlp_ptr[q + 1]; k++) {
+        const double* y = G.Yd + (size_t)G.dlp_a[k] * 18 + r * 3;
+        const double* w = G.Wd + (size_t)G.dlp_b[k] * 18 + cc * 3;
+        v -= ldc(y) * ldc(w) + ldc(y + 1) * ldc(w + 1) + ldc(y + 2) * ldc(w + 2);
+      }
+    }
+    return v;
+  }
+
   __device__ void direct_assemble(double lambda) {
+    if (G.dnd) { nd_assemble(lambda); return; }
     const int nb = G.dnb, n6 = 6 * G.N, np6 = 48 * G.dnbp;
     const long long total = (long long)ldc(G.dtoff + nb) * 2304;
     int tprev = -1, ti = 0, tj = 0, f0 = 0;
@@ -3145,6 +3197,7 @@ struct Phase {
   // (a, a) holds exactly one record (q, q) per eliminated incidence q of pose a, plane-ascending.  (The dense solve forms b in
   // pose_phase, with every plane eliminated.)
   __device__ void direct_rhs() {
+    if (G.dnd) { nd_rhs(); return; }
     const int n6 = 6 * G.N;
     for (int i = tid_team(); i < n6; i += nthr_team()) {
       const int a = i / 6, r = i - a * 6, q = dpair(a, a);
@@ -3219,6 +3272,7 @@ struct Phase {
   // DESIGN.md section 5.1.)  Look-ahead: the owner of tile (K+1, K+1) updates it first (unless row K+1 starts at column
   // K+1), factors it and publishes L_{K+1}^-1; step 0's pivot is factored by every CTA from the snapshot.
   __device__ void direct_factor() {
+    if (G.dnd) { nd_factor(); return; }
     const int nb = G.dnb, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3;
     double* Li = reinterpret_cast<double*>(g_smem + kSmWork);
     double* Ci = Li + kAcTile;
@@ -3362,6 +3416,7 @@ struct Phase {
   // columns first[K] .. K-1 of row K.  dvec[0] = the running right-hand side / x, dvec[1] = y.  b holds 6 N pose entries,
   // then 3 per bordered plane.
   __device__ void direct_trsv() {
+    if (G.dnd) { nd_trsv(); return; }
     const int nb = G.dnb, n = 48 * nb, n6 = 6 * G.N, np6 = 48 * G.dnbp, tid = threadIdx.x;
     double* rv = G.dvec;
     double* yv = G.dvec + n;
@@ -3411,6 +3466,190 @@ struct Phase {
       __syncthreads();
       team_barrier(c);
     }
+  }
+
+  // ---- nested-dissection layout (DESIGN.md section 5.3): the stored tiles of L's pattern in the permuted order ----
+  // S tile by tile, each entry by one thread: tile (ti, tj) of the new order holds the original tiles (perm ti, perm tj); an
+  // entry above the original diagonal is read from its mirror (the pair lists hold the original orientation a >= b).
+  __device__ __noinline__ void nd_assemble(double lambda) {
+    const long long total = (long long)ldc(nd(ND_LTPTR) + ldc(G.dnd)) * 2304;
+    for (long long idx = tid_team(); idx < total; idx += nthr_team()) {
+      const int t = (int)(idx / 2304), e = (int)(idx - (long long)t * 2304), er = e / 48, ec = e - er * 48;
+      const int ti = ldc(nd(ND_TROW) + t), tj = ldc(nd(ND_TCOL) + t);
+      double v = 0.0;
+      if (ti != tj || ec <= er) {
+        int i = 48 * ldc(nd(ND_PERM) + ti) + er, j = 48 * ldc(nd(ND_PERM) + tj) + ec;
+        if (j > i) { const int x = i; i = j; j = x; }
+        v = direct_entry(i, j, lambda, [t](int a, int b) { return (size_t)64 * t + 8 * (a & 7) + (b & 7); });
+      }
+      tile_at(G.Sd, t)[er * kAcLd + ec] = v;
+    }
+  }
+
+  // the right-hand side of direct_rhs in the ND layout: the pair (a, a) of pose a lies in the diagonal tile of its tile
+  __device__ __noinline__ void nd_rhs() {
+    const int n6 = 6 * G.N;
+    for (int i = tid_team(); i < n6; i += nthr_team()) {
+      const int a = i / 6, r = i - a * 6;
+      const size_t q = (size_t)64 * ldc(nd(ND_TOFF) + ldc(nd(ND_POS) + a / 8)) + 9 * (a & 7);
+      double v = -ldc(G.gp + i);
+      for (int k = G.dlp_ptr[q]; k < G.dlp_ptr[q + 1]; k++) {
+        const int inc = G.dlp_a[k];
+        const double* y = G.Yd + (size_t)inc * 18 + r * 3;
+        const double* g = G.gl + (size_t)G.dinc_plane[inc] * 3;
+        v += ldc(y) * ldc(g) + ldc(y + 1) * ldc(g + 1) + ldc(y + 2) * ldc(g + 2);
+      }
+      G.b[i] = v;
+    }
+    for (int k = tid_team(); k < 3 * G.dnbord; k += nthr_team()) G.b[n6 + k] = -ldc(G.gl + (size_t)ldc(G.dbord + k / 3) * 3 + k % 3);
+  }
+
+  // S = L L^T in place, left-looking, level by level of the elimination tree (a column's children lie on lower levels, so
+  // every L_iK it reads is final).  Stored tile t belongs to CTA (t - first tile of its level) % tsize.  Per level:
+  //   (a) C_ij = A_ij - sum_K L_iK L_jK^T over the tile's update list, in list order, on the FP64 tensor cores; the owner of a
+  //       diagonal tile factors it (chol48) and publishes L_jj^-1;          team barrier
+  //   (b) panels L_ij = C_ij L_jj^-T;                                        team barrier
+  // Each product reads two final L tiles, so every CTA that forms a tile gets the same bits.
+  __device__ __noinline__ void nd_factor() {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3, T = c.tsize;
+    double* Li = reinterpret_cast<double*>(g_smem + kSmWork);
+    double* Xa = Li + kAcTile;
+    double* Xb = Xa + kAcTile;
+    auto frag = [&](int s, int& r, int& cc) {
+      const int q = warp + 16 * s;
+      r = 8 * (q / 6) + fr;
+      cc = 8 * (q % 6) + 2 * fc;
+      return q < 36;
+    };
+    for (int l = 0; l < ldc(G.dnd); l++) {
+      const int t0 = ldc(nd(ND_LTPTR) + l), t1 = ldc(nd(ND_LTPTR) + l + 1);
+      for (int t = t0 + c.rank; t < t1; t += T) {
+        double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+        double* tile = tile_at(G.Sd, t);
+        int r, cc;
+#pragma unroll
+        for (int s = 0; s < 3; s++)
+          if (frag(s, r, cc)) {
+            const double2 v = __ldcg(reinterpret_cast<const double2*>(tile + r * kAcLd + cc));
+            acc[s][0] = v.x; acc[s][1] = v.y;
+          }
+        for (int u = ldc(nd(ND_UPTR) + t); u < ldc(nd(ND_UPTR) + t + 1); u++) {
+          const double* A = tile_at(G.Sd, ldc(nd(ND_UPD) + 2 * u));
+          const double* B = tile_at(G.Sd, ldc(nd(ND_UPD) + 2 * u + 1));
+          __syncthreads();
+          for (int e = tid; e < 48 * 48; e += kThreads) {
+            const int o = (e / 48) * kAcLd + e % 48;
+            Xa[o] = -ldc(A + o);
+            Xb[o] = ldc(B + o);
+          }
+          __syncthreads();
+          mma48<true>(acc, Xa, Xb);
+        }
+        const int j = ldc(nd(ND_TCOL) + t);
+        if (ldc(nd(ND_TROW) + t) == j) {   // diagonal: factor it, publish L_jj and L_jj^-1
+          __syncthreads();
+#pragma unroll
+          for (int s = 0; s < 3; s++)
+            if (frag(s, r, cc)) *reinterpret_cast<double2*>(Xa + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+          const bool ok = chol48(Xa, Li);
+          if (!ok && tid == 0) *G.dflag = 1u;
+          store_tile(tile, Xa);
+          store_tile(tile_at(G.Dinv, j), Li);
+        } else {
+#pragma unroll
+          for (int s = 0; s < 3; s++)
+            if (frag(s, r, cc)) *reinterpret_cast<double2*>(tile + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+        }
+      }
+      __syncthreads();
+      team_barrier(c);
+      for (int t = t0 + c.rank; t < t1; t += T) {   // panels
+        const int j = ldc(nd(ND_TCOL) + t);
+        if (ldc(nd(ND_TROW) + t) == j) continue;
+        double* tile = tile_at(G.Sd, t);
+        __syncthreads();
+        load_tile(Xa, tile);
+        load_tile(Li, tile_at(G.Dinv, j));
+        __syncthreads();
+        double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+        mma48<true>(acc, Xa, Li);
+        int r, cc;
+#pragma unroll
+        for (int s = 0; s < 3; s++)
+          if (frag(s, r, cc)) *reinterpret_cast<double2*>(tile + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+      }
+      __syncthreads();
+      team_barrier(c);
+    }
+  }
+
+  // L y = b by ascending level, L^T x = y by descending level, one team barrier per level.  Groups of 48 threads own one
+  // column each (group g of CTA rank takes the level's columns rank * groups + g, then every tsize * groups-th); each entry
+  // is a gather in list order by one thread, then the product with L_jj^-1.  b is gathered into the new order first and x
+  // scattered back, so dvec[0] ends as in the envelope layout.
+  __device__ __noinline__ void nd_trsv() {
+    constexpr int kGroups = kThreads / 48;
+    const int nb = G.dnb, n = 48 * nb, n6 = 6 * G.N, np6 = 48 * G.dnbp, tid = threadIdx.x, g = tid / 48, r = tid - 48 * g;
+    double* rv = G.dvec;
+    double* yv = G.dvec + n;   // the vector in the new order: b, then y, then x, in place
+    double* sv = reinterpret_cast<double*>(g_smem + kSmWork) + 48 * g;
+    for (int i = tid_team(); i < n; i += nthr_team())
+      yv[48 * ldc(nd(ND_POS) + i / 48) + i % 48] =
+          (i < n6) ? ldc(G.b + i) : ((i >= np6 && i < np6 + 3 * G.dnbord) ? ldc(G.b + n6 + i - np6) : 0.0);
+    team_barrier(c);
+    for (int l = 0; l < ldc(G.dnd); l++) {   // forward: y_j = L_jj^-1 (b_j - sum_K L_jK y_K)
+      const int k1 = ldc(nd(ND_LPTR) + l + 1);
+      for (int base = ldc(nd(ND_LPTR) + l) + c.rank * kGroups; base < k1; base += c.tsize * kGroups) {
+        const bool act = g < kGroups && base + g < k1;
+        const int j = act ? ldc(nd(ND_LCOL) + base + g) : 0;
+        if (act) {
+          double v = ldc(yv + 48 * j + r);
+          for (int p = ldc(nd(ND_RPTR) + j); p < ldc(nd(ND_RPTR) + j + 1); p++) {
+            const int t = ldc(nd(ND_RTILE) + p), K = ldc(nd(ND_TCOL) + t);
+            const double* Lr = tile_at(G.Sd, t) + r * kAcLd;
+            for (int m = 0; m < 48; m++) v -= ldc(Lr + m) * ldc(yv + 48 * K + m);
+          }
+          sv[r] = v;
+        }
+        __syncthreads();
+        if (act) {
+          const double* Li = tile_at(G.Dinv, j);
+          double v = 0.0;
+          for (int m = 0; m <= r; m++) v += ldc(Li + r * kAcLd + m) * sv[m];
+          yv[48 * j + r] = v;
+        }
+        __syncthreads();
+      }
+      team_barrier(c);
+    }
+    for (int l = ldc(G.dnd) - 1; l >= 0; l--) {   // backward: x_j = L_jj^-T (y_j - sum_i L_ij^T x_i)
+      const int k1 = ldc(nd(ND_LPTR) + l + 1);
+      for (int base = ldc(nd(ND_LPTR) + l) + c.rank * kGroups; base < k1; base += c.tsize * kGroups) {
+        const bool act = g < kGroups && base + g < k1;
+        const int j = act ? ldc(nd(ND_LCOL) + base + g) : 0;
+        if (act) {
+          double v = ldc(yv + 48 * j + r);
+          const int d = ldc(nd(ND_TOFF) + j), cnt = ldc(nd(ND_CPTR) + j + 1) - ldc(nd(ND_CPTR) + j);
+          for (int t = d + 1; t < d + cnt; t++) {
+            const int i = ldc(nd(ND_TROW) + t);
+            const double* Lc = tile_at(G.Sd, t) + r;
+            for (int m = 0; m < 48; m++) v -= ldc(Lc + m * kAcLd) * ldc(yv + 48 * i + m);
+          }
+          sv[r] = v;
+        }
+        __syncthreads();
+        if (act) {
+          const double* Li = tile_at(G.Dinv, j);
+          double v = 0.0;
+          for (int m = r; m < 48; m++) v += ldc(Li + m * kAcLd + r) * sv[m];
+          yv[48 * j + r] = v;
+        }
+        __syncthreads();
+      }
+      team_barrier(c);
+    }
+    for (int i = tid_team(); i < n; i += nthr_team()) rv[i] = ldc(yv + 48 * ldc(nd(ND_POS) + i / 48) + i % 48);
+    team_barrier(c);
   }
 #endif
 };

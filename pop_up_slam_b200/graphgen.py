@@ -240,6 +240,13 @@ def make_corridor(seed=0, n_poses=5000, n_planes=500, obs_per_pose=10, step=0.1,
     pose, and wall / door-frame planes anchored every L/(M-1) metres of path on alternating sides; each pose
     observes the ground plus the obs_per_pose-1 nearest anchors (by arclength)."""
     rng = np.random.default_rng(seed)
+    T, planes, obs_pose, obs_plane, dist = _corridor_geometry(rng, n_poses, n_planes, obs_per_pose, step, aisle, radius)
+    return _finish(name, seed, T, planes, obs_pose, obs_plane, dist, rng, sigma_mode, plane_noise, odo_noise,
+                   outlier_frac, outlier_mag, robust_kind, robust_b, max_iterations, init_mode)
+
+
+def _corridor_geometry(rng, n_poses, n_planes, obs_per_pose, step, aisle, radius):
+    """truth poses, planes and observations of make_corridor"""
     L = n_poses * step
     n_aisles = int(np.floor(L / (aisle + np.pi * radius))) + 1
     centre = np.array([0.0, (n_aisles - 1) * radius])
@@ -287,6 +294,28 @@ def make_corridor(seed=0, n_poses=5000, n_planes=500, obs_per_pose=10, step=0.1,
     obs_plane = obs_plane.reshape(-1)
     cam = T[obs_pose, :3, 3]
     dist = np.where(obs_plane == 0, cam[:, 2], np.linalg.norm(anchors[obs_plane][:, :2] - cam[:, :2], axis=1))
+    return T, planes, obs_pose, obs_plane, dist
+
+
+def make_revisit(seed=0, n_poses=2000, n_planes=100, obs_per_pose=10, step=0.1, sigma_mode="consistent", plane_noise=0.01,
+                 odo_noise=(0.003, 0.0002), outlier_frac=0.0, outlier_mag=(0.05, 0.3), robust_kind=0, robust_b=1.0,
+                 max_iterations=20, name="revisit", init_mode="dead_reckoning", aisle=40.0, radius=2.5, offset=0.2):
+    """A corridor driven twice: the first n_poses - n_poses // 2 poses walk the make_corridor path with n_planes planes, the
+    rest walk it again from the start, `offset` metres to the side.  The odometry chain continues across the turn-back, and
+    the second pass re-observes the first pass's planes with fresh noise -- the graph a loop closure that merges a revisit's
+    planes into the first visit's (Mapper_mono::loopclose_merge, Mapping.cpp:637-704) leaves behind: pose a and pose
+    a + n_poses // 2 share planes for every a."""
+    rng = np.random.default_rng(seed)
+    n1 = n_poses - n_poses // 2
+    T1, planes, op1, ol1, dist1 = _corridor_geometry(rng, n1, n_planes, obs_per_pose, step, aisle, radius)
+    n2 = n_poses - n1
+    T2 = T1[:n2].copy()
+    T2[:, :3, 3] += offset * T2[:, :3, 0]   # (R_BASE: the camera x axis points across the path)
+    keep = op1 < n2
+    T = np.concatenate([T1, T2])
+    obs_pose = np.concatenate([op1, op1[keep] + n1])
+    obs_plane = np.concatenate([ol1, ol1[keep]])
+    dist = np.concatenate([dist1, dist1[keep]])
     return _finish(name, seed, T, planes, obs_pose, obs_plane, dist, rng, sigma_mode, plane_noise, odo_noise,
                    outlier_frac, outlier_mag, robust_kind, robust_b, max_iterations, init_mode)
 

@@ -1,16 +1,20 @@
-"""Direct linear solves (pus_set_linear_solver(h, 1) dense, (h, 2) band) against PCG: device-resident solves of the same
-graphs in each mode, timed by CUDA events on the library's stream with a 256 MiB L2 flush before every timed solve (as
-bench.py does).  Per workload: ms per solve and per LM trial step for each mode, the phase_ms split (11 assembly,
-12 factorization, 13 right-hand side, 14 triangular solves in the direct modes), and the largest difference between the
-estimates of PCG and each direct mode.  Workloads: configs 1 and 2, an 80-pose TUM-scale graph, the 600-pose Huber corridor,
-sphere400 (loop closures, no planes) -- dense and band side by side -- then, band only (over the dense solve's 640 poses),
-the 2 000-pose Huber corridor, sphere2500 and config 3; a batch of 64 config-2 graphs; with --config5, one band solve of
-config 5.  Prints the GPU's name and power limit first.
+"""Direct linear solves (pus_set_linear_solver(h, 1) dense, (h, 2) band in insertion order and in nested-dissection order
+"nd") against PCG: device-resident solves of the same graphs in each mode, timed by CUDA events on the library's stream with
+a 256 MiB L2 flush before every timed solve (as bench.py does).  Per workload: ms per solve and per LM trial step for each
+mode, the phase_ms split (11 assembly, 12 factorization, 13 right-hand side, 14 triangular solves in the direct modes), and
+the largest difference between the estimates of PCG and each direct mode; for the band and nd modes also the layout: stored
+tiles, tile products of one factorization (nd), dependent steps (band: tile columns; nd: levels), device bytes and the host
+time of the table build.  Workloads: configs 1 and 2, an 80-pose TUM-scale graph, the 600-pose Huber corridor, sphere400
+(loop closures, no planes) -- dense and band side by side -- then, band only (over the dense solve's 640 poses), the
+2 000-pose Huber corridor, sphere2500, config 3 and the revisited corridor (gg.make_revisit) at 2 000 and 5 000 poses; a batch
+of 64 config-2 graphs; with --config5, one band and one nd solve of config 5 and of a revisited corridor of config 5's size
+(or the refusal when a layout is over its budget).  Prints the GPU's name and power limit first.
 usage: python tools/direct_solve_bench.py [reps=5] [warmup=2] [--config5]      (one JSON line per workload)"""
 import json
 import os
 import subprocess
 import sys
+import time
 
 import numpy as np
 import torch
@@ -58,14 +62,18 @@ WORKLOADS = [
     ("huber2000", lambda: gg.make_config(3, seed=0, n_poses=2000, n_planes=200, max_iterations=8)),
     ("sphere2500", None),
     ("config3", lambda: gg.make_config(3, seed=0)),
+    ("revisit2000", lambda: gg.make_revisit(seed=0, n_poses=2000, n_planes=100, max_iterations=8)),
+    ("revisit5000", lambda: gg.make_revisit(seed=0, n_poses=5000, n_planes=250, max_iterations=8)),
 ]
+MODES = (("pcg", 0, 0), ("direct", 1, 0), ("band", 2, 0), ("nd", 2, 1))
 SPHERES = dict(sphere400=sphere400, sphere2500=sphere2500)
 
 
-def make(name, g, direct, stream):
+def make(name, g, direct, stream, order=0):
     a = GpuGraphAPI()
     a.set_stream(stream.cuda_stream)
     a.set_linear_solver(direct)
+    a.set_direct_ordering(order)
     if g is None:
         ids = SPHERES[name](a)
     else:
@@ -73,6 +81,34 @@ def make(name, g, direct, stream):
         gg.configure(a, g)
     a.upload()
     return a, ids
+
+
+def layout(a, order):
+    """the band / nd layout of an uploaded handle, and the host time of its table build (a recompile of the graph)"""
+    t0 = time.perf_counter()
+    a._chk(a.lib.pus_debug_compile(a.h))
+    out = dict(table_build_s=round(time.perf_counter() - t0, 3), device_bytes=int(a.debug_fetch("bbytes", 1)[0]),
+               bordered=len(a.debug_fetch("bborder", 1 << 16)))
+    if order == 0:
+        first = a.debug_fetch("bfirst", 1 << 24).astype(np.int64)
+        out.update(tiles=int(sum(i - first[i] + 1 for i in range(len(first)))), steps=len(first))
+    else:
+        cptr = a.debug_fetch("ndcptr", 1 << 24).astype(np.int64)
+        m = np.diff(cptr) - 1
+        out.update(tiles=int(cptr[-1]), tile_products=int((m * (m + 1) // 2).sum()),
+                   levels=int(a.debug_fetch("ndlevel", 1 << 24).max()) + 1)
+    return out
+
+
+def run_mode(name, g, kind, order, reps, warmup, stream, flush):
+    a, ids = make(name, g, kind, stream, order)
+    ms, its = timed(a.solve_resident, reps, warmup, stream, flush)
+    a.download()
+    r = dict(ms_per_solve=round(ms, 3), trial_steps=int(its[-1]), ms_per_trial_step=round(ms / max(1, its[-1]), 4),
+             phase_ms=[round(x, 3) for x in a.stats()["phase_ms"][:15]])
+    if kind == 2:
+        r.update(layout(a, order))
+    return a, ids, r
 
 
 def timed(fn, reps, warmup, stream, flush):
@@ -112,34 +148,36 @@ def main():
         g = mk() if mk else None
         row = dict(workload=name)
         est = {}
-        small = name not in ("huber2000", "sphere2500", "config3")   # (the dense solve takes at most 640 poses)
-        for mode, kind in (("pcg", 0), ("direct", 1), ("band", 2)):
+        small = name in ("config1", "config2", "tum80", "huber600", "sphere400")   # (the dense solve takes at most 640 poses)
+        for mode, kind, order in MODES:
             if kind == 1 and not small:
                 continue
-            a, ids = make(name, g, kind, stream)
-            ms, its = timed(a.solve_resident, reps, warmup, stream, flush)
-            a.download()
+            try:
+                a, ids, row[mode] = run_mode(name, g, kind, order, reps, warmup, stream, flush)
+            except capi.ApiError as e:   # (a layout over its device-memory budget)
+                row[mode] = dict(refused=str(e))
+                continue
             est[mode] = estimates(a, ids)
-            row[mode] = dict(ms_per_solve=round(ms, 3), trial_steps=int(its[-1]), ms_per_trial_step=round(ms / max(1, its[-1]), 4),
-                             phase_ms=[round(x, 3) for x in a.stats()["phase_ms"][:15]])
-        for mode in ("direct", "band"):
+        for mode in ("direct", "band", "nd"):
             if mode in est:
                 row[f"max_estimate_diff_pcg_{mode}"] = float(np.abs(est["pcg"] - est[mode]).max())
+        if "band" in est and "nd" in est:
+            row["max_estimate_diff_band_nd"] = float(np.abs(est["band"] - est["nd"]).max())
         if small:
             row["max_estimate_diff_direct_band"] = float(np.abs(est["direct"] - est["band"]).max())
         print(json.dumps(dict(row, **dev)), flush=True)
-    if config5:   # one timed band solve, when the graph fits the band solve's device-memory budget
-        g = gg.make_config(5, seed=0)
-        row = dict(workload="config5")
-        try:
-            a, ids = make("config5", g, 2, stream)
-            ms, its = timed(a.solve_resident, 1, 0, stream, flush)
-            row["band"] = dict(ms_per_solve=round(ms, 3), trial_steps=int(its[-1]), ms_per_trial_step=round(ms / max(1, its[-1]), 4),
-                               phase_ms=[round(x, 3) for x in a.stats()["phase_ms"][:15]],
-                               device_bytes=int(a.debug_fetch("bbytes", 1)[0]))
-        except capi.ApiError as e:
-            row["band"] = dict(refused=str(e))
-        print(json.dumps(dict(row, **dev)), flush=True)
+    if config5:   # one timed solve per layout, when the graph fits the layout's device-memory budget
+        for name, mk in (("config5", lambda: gg.make_config(5, seed=0)),
+                         ("revisit50000", lambda: gg.make_revisit(seed=0, n_poses=50000, n_planes=5000, obs_per_pose=20,
+                                                                  step=0.02, aisle=100.0, radius=2.0, max_iterations=50))):
+            g = mk()
+            row = dict(workload=name)
+            for mode, kind, order in MODES[2:]:
+                try:
+                    row[mode] = run_mode(name, g, kind, order, 1, 0, stream, flush)[2]
+                except capi.ApiError as e:
+                    row[mode] = dict(refused=str(e))
+            print(json.dumps(dict(row, **dev)), flush=True)
     # a batch of 64 config-2 graphs
     graphs = [gg.make_config(2, seed=s) for s in range(64)]
     row = dict(workload="batch64_config2")

@@ -4,6 +4,8 @@ thing print the same lines; run it once per library (PUS_LIBRARY=<path to libpop
 device-side counterpart of compile_graph_hash.cpp.
 
     python tools/solve_digest.py [--quick]      (--quick: skip the 12 000-pose graph and the full config-3 graph)
+
+The PCG paths come first; the dense and insertion-order band direct solves follow.
 """
 import hashlib
 import os
@@ -16,8 +18,9 @@ from pop_up_slam_b200 import capi, graphgen as gg   # noqa: E402
 from pop_up_slam_b200.capi import GpuGraphAPI       # noqa: E402
 
 
-def graph(g, flags=0, jac_numeric=False, **props):
+def graph(g, flags=0, jac_numeric=False, kind=0, **props):
     a = GpuGraphAPI()
+    a.set_linear_solver(kind)
     ids = gg.build_bulk(a, g)
     gg.configure(a, g, **props)
     if flags:
@@ -45,8 +48,8 @@ def solve(g, **kw):
     return [a]
 
 
-def updates(g):
-    a = graph(g, method=0)
+def updates(g, kind=0):
+    a = graph(g, kind=kind, method=0)
     for _ in range(3):   # relinearise + one Gauss-Newton step each
         a[0].update()
     return [a]
@@ -91,6 +94,15 @@ def main():
     ]
     if not quick:
         paths.append(("c3 bench graph", lambda: solve(gg.make_config(3, seed=0))))
+    # the exact direct solves: dense (kind 1) and band in insertion order (kind 2)
+    paths += [
+        ("c1 dense direct", lambda: solve(gg.make_config(1, seed=0), kind=1)),
+        ("c2 dense direct", lambda: solve(c2, kind=1)),
+        ("c2 band direct", lambda: solve(c2, kind=2)),
+        ("c3/900 band direct", lambda: solve(c3s, kind=2)),
+        ("c3/900 band direct, numeric Jacobians", lambda: solve(c3s, kind=2, jac_numeric=True)),
+        ("c2 dense direct update() x3", lambda: updates(gg.make_config(2, seed=1), kind=1)),
+    ]
     for name, run in paths:
         pcg, d = digest(run())
         print(f"{name:36s} pcg={pcg:7d} {d}", flush=True)
