@@ -442,6 +442,65 @@ struct SparseJacobian {
   std::vector<double> values, rhs;     // [nnz], [rows]
 };
 
+// isam::Covariances (ISAM/include/isam/Covariances.h:58-110), read through Slam::covariances(): Sigma = (J^T J)^-1 at the
+// current estimate, undamped, recovered on the device from the band solver's nested-dissection factor (the handle must use
+// LINEAR_SOLVER_BAND with ORDERING_NESTED_DISSECTION; see pus_marginal_covariances).  marginal(list) is the joint block over
+// the nodes in list order, each node's rows / columns in its tangent order; access(pairs) returns dim(first) x dim(second)
+// blocks, as Covariances.cpp:107-150 does.
+class Covariances {
+  pus_handle _h;
+ public:
+  typedef std::list<std::list<Node*> > node_lists_t;
+  typedef std::list<std::pair<Node*, Node*> > node_pair_list_t;
+  explicit Covariances(pus_handle h) : _h(h) {}
+  std::list<MatrixXd> access(const node_pair_list_t& pairs) const {                 // Covariances.cpp:107-150
+    std::vector<int> ids;
+    long long n = 0;
+    for (const auto& p : pairs) { ids.push_back(p.first->unique_id()); ids.push_back(p.second->unique_id()); n += p.first->dim() * p.second->dim(); }
+    std::vector<double> v((size_t)n + 1);
+    detail::check(pus_covariance_blocks(_h, (int)pairs.size(), ids.data(), v.data()) < 0 ? -1 : 0);
+    std::list<MatrixXd> out;
+    size_t o = 0;
+    for (const auto& p : pairs) {
+      const int r = p.first->dim(), c = p.second->dim();
+      MatrixXd m(r, c);
+      for (int i = 0; i < r; i++)
+        for (int j = 0; j < c; j++) m(i, j) = v[o + (size_t)i * c + j];
+      o += (size_t)r * c;
+      out.push_back(m);
+    }
+    return out;
+  }
+  std::list<MatrixXd> marginal(const node_lists_t& lists) const {                   // Covariances.cpp:70-99
+    // as covariance.cpp:135-144: the upper triangle is computed and mirrored, so the joint matrix is exactly symmetric
+    std::list<MatrixXd> out;
+    for (const auto& l : lists) {
+      const std::vector<Node*> v(l.begin(), l.end());
+      std::vector<int> at(v.size() + 1, 0);
+      node_pair_list_t pairs;
+      for (size_t a = 0; a < v.size(); a++) {
+        at[a + 1] = at[a] + v[a]->dim();
+        for (size_t b = a; b < v.size(); b++) pairs.push_back(std::make_pair(v[a], v[b]));
+      }
+      const std::list<MatrixXd> blocks = access(pairs);
+      MatrixXd m(at[v.size()], at[v.size()]);
+      auto it = blocks.begin();
+      for (size_t a = 0; a < v.size(); a++)
+        for (size_t b = a; b < v.size(); b++, ++it)
+          for (int i = 0; i < v[a]->dim(); i++)
+            for (int j = (a == b ? i : 0); j < v[b]->dim(); j++) {
+              const double x = mget(*it, i, j);
+              m(at[a] + i, at[b] + j) = x;
+              m(at[b] + j, at[a] + i) = x;
+            }
+      out.push_back(m);
+    }
+    return out;
+  }
+  MatrixXd marginal(const std::list<Node*>& nodes) const { return marginal(node_lists_t(1, nodes)).front(); }   // :101-105
+  std::list<MatrixXd> marginals(const node_lists_t& lists) const { return marginal(lists); }
+};
+
 // robust costs (ISAM/include/isam/robust.h:101-118); Slam::set_cost_function takes these tags
 struct cost_func_t { int kind; double b; };
 inline cost_func_t cost_huber_tag(double b) { return cost_func_t{1, b}; }
@@ -456,10 +515,12 @@ class Slam {
   std::list<Node*> _nodes;
   std::list<Factor*> _factors;
   int _step = 0;
+  Covariances _covariances{nullptr};
   Slam(const Slam&);
   Slam& operator=(const Slam&);
  public:
-  explicit Slam(int device = 0) { detail::check(pus_create(device, &_h)); }
+  explicit Slam(int device = 0) { detail::check(pus_create(device, &_h)); _covariances = Covariances(_h); }
+  const Covariances& covariances() { return _covariances; }                       // Slam.h:210
   ~Slam() { if (_h) pus_destroy(_h); }
   pus_handle handle() { return _h; }
   Properties properties() { return _prop; }                                         // Slam.h:92-94

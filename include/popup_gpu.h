@@ -27,8 +27,9 @@
  *   There is NO CPU fallback: if no CUDA device / kernel image is usable, calls fail.
  *
  * Limits (a solve fails with a message instead of producing a wrong answer):
- *   - Slam::update() only with mod_batch = 1 (what PPS sets); relative-parameterised plane factors, anchor nodes,
- *     dog-leg and covariance recovery are not provided.
+ *   - Slam::update() only with mod_batch = 1 (what PPS sets); relative-parameterised plane factors, anchor nodes and
+ *     dog-leg are not provided.  Covariances (pus_marginal_covariances, pus_covariance_blocks) are recovered only from the
+ *     band solver in nested-dissection order, undamped at the estimate, within the same 8 GiB budget.
  *   - the dense direct linear solver (pus_set_linear_solver(h, 1)) handles at most 640 live poses (a dense reduced system
  *     of order 3 840, about 65 MB of device memory); a larger graph fails at upload with a message and launches nothing.
  *     The band direct solver (kind 2) takes any graph whose envelope fits 8 GiB of device memory (tiles, snapshots, pivot
@@ -330,6 +331,33 @@ int pus_normalized_chi2(pus_handle h, double* out);
 /* double Slam::local_chi2(int last_n)  Slam.cpp:270-285: the sum of squares of the weighted errors of the last_n most recent
  * live factors (all of them when last_n exceeds their number; 0 when last_n <= 0) */
 int pus_local_chi2(pus_handle h, int last_n, double* out);
+
+/* ---- marginal covariances (isam::Covariances, Covariances.h:58-110; DESIGN.md section 5.4) ---------------------------- */
+/* Sigma = (J^T J)^-1 at the current estimate, undamped (lambda = 0), where J is the stacked whitened, robustified Jacobian
+ * that pus_jacobian exports: the same column order and tangent parameterisation as pus_node_start, and it follows
+ * pus_set_jacobian_mode.  This is what iSAM returns right after Slam::update() with mod_batch = 1 (Optimizer::relinearize
+ * factors undamped at the pre-step point, and Covariances reads that R).  After batch_optimization() iSAM's R is its last
+ * damped trial factor, so its covariances differ from these by O(lambda); that is not reproduced.
+ * Only a handle with pus_set_linear_solver(h, 2) and pus_set_direct_ordering(h, 1) recovers covariances; every other handle
+ * (PCG, dense kind 1, band in insertion order, and hence a pus_span_* handle) is refused with a message naming those calls.
+ * The first call at an estimate linearises, factors the reduced system undamped and inverts it on L's tile pattern by
+ * selected inversion (about the cost of one factorization); the Sigma tiles stay on the device, and later calls read them
+ * until a solve, pus_init_*, a measurement change, a structural edit, pus_set_robust or pus_set_jacobian_mode.  The calls
+ * never change the estimate, the trace or the solver's statistics other than kernel_ms.  A non-positive pivot (J^T J not
+ * positive definite, e.g. no pose prior: the gauge is free) fails the call with a message and stores nothing.  The Sigma tiles
+ * and the selected-inversion lists count against the band budget of 8 GiB together with the factorization; an over-budget
+ * graph is refused at the first call with the need stated, and nothing is launched.  Results are bit-identical across team
+ * sizes, barrier kinds and repeated calls (no floating-point atomics, fixed summation orders).
+ * Cost: the blocks of kept unknowns (poses, bordered planes) whose tile is stored, and every plane's own block, are read
+ * from Sigma (an eliminated plane's block sums over its observer pairs).  Any other block (two distant poses, a pose and a
+ * plane it does not co-observe, two eliminated planes) costs one pair of triangular solves with the factor per column of
+ * its right-hand node (6 for a pose, 3 for a plane), shared by every block of the call with that right-hand node. */
+/* Each node's own block (6 x 6 for a pose, 3 x 3 for a plane), full, row-major, packed in ids order; n may be every live
+ * node.  Returns the number of doubles written, or < 0. */
+int pus_marginal_covariances(pus_handle h, int n, const int* ids, double* out);
+/* The cross blocks Sigma_ab, dim(a) x dim(b) row-major, of the pairs (id_pairs[2 k], id_pairs[2 k + 1]), packed in pair
+ * order (Covariances::access).  Returns the number of doubles written, or < 0. */
+long long pus_covariance_blocks(pus_handle h, int n_pairs, const int* id_pairs, double* out);
 
 /* ---- one graph spanning several ranks (SURVEY.md 8e, second bullet) --------------------------- */
 /* Every rank holds the whole graph (build it identically on each) and runs its own persistent kernel; the PCG

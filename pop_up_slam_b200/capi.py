@@ -498,6 +498,45 @@ class GpuGraphAPI(GraphAPI):
         self._chk(self.lib.pus_local_chi2(self.h, int(last_n), C.byref(out)))
         return out.value
 
+    # -- marginal covariances at the current estimate (band solver in nested-dissection order only) --
+    def marginal_covariances(self, ids):
+        """Each node's own block of (J^T J)^-1 (6 x 6 per pose, 3 x 3 per plane), as a list of numpy arrays in ids order."""
+        ids = _i32(np.atleast_1d(ids))
+        dims = [self.node_dim(int(i)) for i in ids]
+        out = np.zeros(max(1, sum(d * d for d in dims)))
+        fn = self.lib.pus_marginal_covariances
+        fn.argtypes = [C.c_void_p, C.c_int, c_int_p, c_double_p]
+        self._chk(fn(self.h, len(ids), _ip(ids), _dp(out)))
+        res, o = [], 0
+        for d in dims:
+            res.append(out[o:o + d * d].reshape(d, d).copy())
+            o += d * d
+        return res
+
+    def covariance_blocks(self, pairs):
+        """The cross blocks Sigma_ab of the (a, b) node pairs, as a list of dim(a) x dim(b) numpy arrays."""
+        p = _i32(np.asarray(pairs).reshape(-1, 2))
+        dims = [(self.node_dim(int(a)), self.node_dim(int(b))) for a, b in p]
+        out = np.zeros(max(1, sum(a * b for a, b in dims)))
+        fn = self.lib.pus_covariance_blocks
+        fn.restype = C.c_longlong
+        fn.argtypes = [C.c_void_p, C.c_int, c_int_p, c_double_p]
+        self._chk(fn(self.h, len(p), _ip(np.ascontiguousarray(p.reshape(-1))), _dp(out)))
+        res, o = [], 0
+        for a, b in dims:
+            res.append(out[o:o + a * b].reshape(a, b).copy())
+            o += a * b
+        return res
+
+    def node_dim(self, id_):
+        """6 for a live pose, 3 for a live plane."""
+        buf = np.zeros(7)
+        if self.lib.pus_get_pose(self.h, int(id_), _dp(buf)) >= 0:
+            return 6
+        if self.lib.pus_get_plane(self.h, int(id_), _dp(buf)) >= 0:
+            return 3
+        raise ApiError(f"bad node id {id_}")
+
     def debug_fetch(self, name, cap):
         out = np.zeros(int(cap))
         n = self.lib.pus_debug_fetch(self.h, name.encode(), _dp(out), C.c_longlong(int(cap)))

@@ -211,6 +211,20 @@ __device__ void run_graph_impl(Ctx& c) {
     if (lead) { res->chi2_final = e; res->chi2_initial = e; res->chi2_evals = 1; }
     return;
   }
+#ifdef PUS_DIRECT
+  if (P.mode == MODE_COV) {   // marginal covariances (ND layout; DESIGN.md section 5.4).  debug_stage 1: Sigma first
+    if (P.debug_stage == 1) {   // linearise at the estimate, factor undamped, invert on the pattern
+      linearize(ph, c);
+      direct_setup(ph, c, 0.0, ft);
+      if (__ldcg(G.dflag) != 0u) return;   // a non-positive pivot: the host reports it and keeps nothing
+      ph.nd_selinv();
+    }
+    ph.cov_gather();
+    ph.cov_columns();
+    team_barrier(c);
+    return;
+  }
+#endif
   if (P.mode == MODE_DEBUG) {
     if (P.debug_stage == 9) {   // micro-benchmark: 1000 team barriers, 1000 team reductions (phase_ms[0], [1])
       tm.sync();

@@ -106,6 +106,14 @@ struct Solver {
     bool structure = false;               // d_row_ptr / d_col_idx filled for this layout
     cudaEvent_t ev_copy = nullptr;        // recorded after an export's device-to-host copies
   } xt;
+  // marginal covariances (pus_marginal_covariances / pus_covariance_blocks; kind 2 in ND order only): the tables of the layout,
+  // built by its first covariance call, and Sigma on the device, valid until the next launch, upload or change of the
+  // linearisation (any of them sets valid = false)
+  struct CovState {
+    CovTables t;
+    bool valid = false;
+    void* mem = nullptr; size_t bytes = 0;   // device: Sigma tiles, then the packed tables
+  } cov;
   std::map<std::string, std::pair<double*, size_t>> named;  // debug access to double buffers
   DevGraph hd;
   DevGraph* d_graph = nullptr;
@@ -226,6 +234,7 @@ static int sync_measurements_to_host(Solver* s) {
 // (re)build the HBM image of the graph.  Topology arrays are re-uploaded only after a structural edit;
 // vertex values always; measurements when pus_set_measurement touched them.
 static int upload(Solver* s) {
+  s->cov.valid = false;
   if (ensure_device(s) < 0) return -1;
   cudaEvent_t e0 = s->ev0, e1 = s->ev1;
   long long bytes = 0;
@@ -417,6 +426,8 @@ static int auto_team(const Solver* s, int limit) {
 // launch the persistent kernel over `n` solvers (all on the device / stream of the first)
 static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stage, double debug_lambda) {
   Solver* s0 = ss[0];
+  if (mode != MODE_COV)
+    for (int i = 0; i < n; i++) ss[i]->cov.valid = false;   // (a solve or a debug stage overwrites the factor)
   if (ensure_device(s0) < 0) return -1;
   for (int i = 0; i < n; i++) {
     if (!ss[i]->uploaded) { g_err = "graph not uploaded"; return -1; }
@@ -713,6 +724,7 @@ int pus_destroy(pus_handle h) {
   if (s->rt.mem) cudaFree(s->rt.mem);
   if (s->xt.mem) cudaFree(s->xt.mem);
   if (s->xt.ev_copy) cudaEventDestroy(s->xt.ev_copy);
+  if (s->cov.mem) cudaFree(s->cov.mem);
   if (s->scratch) cudaFree(s->scratch);
   if (s->ev0) cudaEventDestroy(s->ev0);
   if (s->ev1) cudaEventDestroy(s->ev1);
@@ -865,9 +877,9 @@ int pus_set_properties(pus_handle h, const pus_properties* in) { NEED(h); SV(h)-
 int pus_set_robust(pus_handle h, int kind, double b) {
   NEED(h);
   if (kind < 0 || kind > 2 || !(b > 0)) { g_err = "bad robust cost"; return -1; }
-  SV(h)->robust_kind = kind; SV(h)->robust_b = b; return 0;
+  SV(h)->robust_kind = kind; SV(h)->robust_b = b; SV(h)->cov.valid = false; return 0;
 }
-int pus_set_jacobian_mode(pus_handle h, int numeric) { NEED(h); SV(h)->jac_numeric = numeric ? 1 : 0; return 0; }
+int pus_set_jacobian_mode(pus_handle h, int numeric) { NEED(h); SV(h)->jac_numeric = numeric ? 1 : 0; SV(h)->cov.valid = false; return 0; }
 int pus_set_linear_solver(pus_handle h, int kind) {
   NEED(h);
   Solver* s = SV(h);
@@ -1131,6 +1143,7 @@ int pus_refresh_plane_measurements(pus_handle h, int n_frames, const int* frame_
   float* d_ps = sc.put<float>(nullptr, (size_t)n_rows * 4);
   double* d_out = sc.put<double>(nullptr, (size_t)n_map * 4);
   if (!d_fpose || !d_ptr || !d_rf || !d_segs || !d_K || !d_mrow || !d_mslot || !d_T || !d_ps || !d_out) { g_err = "scratch allocation failed"; return -1; }
+  s->cov.valid = false;   // (new measurements on the device)
   CUDA_OK(cudaMemsetAsync(d_ps, 0, (size_t)n_rows * 4 * sizeof(float), st));
   CUDA_OK(launch_refresh(st, n_frames, d_fpose, s->hd.pose_lin, d_ptr, d_rf, n_rows, d_segs, d_K, d_T, d_ps, n_map, d_mrow, d_mslot,
                          const_cast<double*>(s->hd.pp_meas), d_out));
@@ -1243,6 +1256,7 @@ int pus_refresh_run(pus_handle h, double* new_meas) {
   if (t.slot_topo != s->compiled_topo && refresh_slots(s) < 0) return -1;
   CUDA_OK(cudaSetDevice(s->device));
   cudaStream_t st = s->stream;
+  s->cov.valid = false;   // (new measurements on the device)
   CUDA_OK(cudaEventRecord(s->ev0, st));
   CUDA_OK(launch_refresh(st, t.n_frames, t.d_fpose, s->hd.pose_lin, t.d_ptr, t.d_rf, t.n_rows, t.d_segs, t.d_K, t.d_T, t.d_ps, t.n_map, t.d_mrow,
                          t.d_mslot, const_cast<double*>(s->hd.pp_meas), t.d_out));
@@ -1682,6 +1696,190 @@ static long long nd_tile(const DirectTables& dt, int i, int j) {
   return (at == b + dt.nd_cptr[j + 1] || *at != i) ? -1 : dt.nd_toff[j] + (at - (b + dt.nd_cptr[j]));
 }
 
+// ---- marginal covariances (DESIGN.md section 5.4) ----
+// Refuse every handle but kind 2 in ND order; re-upload as the exports do; build the layout's tables on the first call and
+// check them against the budget before anything is allocated or launched.
+static int cov_prepare(Solver* s, const char* fn) {
+  if (s->linear_solver != 2 || s->ordering != 1) {
+    g_err = std::string(fn) + ": covariances are recovered from the nested-dissection factor only; call pus_set_linear_solver(h, 2) "
+            "and pus_set_direct_ordering(h, 1) (this handle: linear solver kind " + std::to_string(s->linear_solver) +
+            ", ordering " + std::to_string(s->ordering) + ")";
+    return -1;
+  }
+  if (s->g.num_factors() == 0) { g_err = std::string(fn) + ": the graph has no live factors"; return -1; }
+  if (!s->uploaded || s->compiled_topo != s->g.topo_version || s->values_dirty || s->meas_dirty) {
+    if (upload(s) < 0) return -1;
+  } else if (ensure_device(s) < 0) {
+    return -1;
+  }
+  Solver::CovState& cv = s->cov;
+  if (cv.t.topo == s->compiled_topo) return 0;
+  cv.valid = false;
+  std::string err;
+  if (!build_cov(s->c, s->dt, cv.t, err)) { g_err = std::string(fn) + ": " + err; return -1; }
+  const size_t sig = (size_t)s->dt.nd_cptr[s->dt.nb] * kAcTile * 8, need = sig + cv.t.dev.size() * 4;
+  CUDA_OK(cudaSetDevice(s->device));
+  if (need > cv.bytes) {
+    if (cv.mem) { cudaStreamSynchronize(s->stream); cudaFree(cv.mem); cv.mem = nullptr; cv.bytes = 0; }
+    if (cudaMalloc(&cv.mem, need) != cudaSuccess) {
+      cudaGetLastError();
+      g_err = std::string(fn) + ": cannot allocate " + std::to_string(need) + " bytes for the Sigma tiles";
+      cv.t = CovTables();
+      return -1;
+    }
+    cv.bytes = need;
+  }
+  CUDA_OK(cudaMemcpyAsync(static_cast<char*>(cv.mem) + sig, cv.t.dev.data(), cv.t.dev.size() * 4, cudaMemcpyHostToDevice, s->stream));
+  CUDA_OK(cudaStreamSynchronize(s->stream));
+  cv.t.topo = s->compiled_topo;
+  return 0;
+}
+
+// One covariance launch: Sigma first when it is not valid, then the records `rec` (header, gather records, columns, column
+// records; see Phase::cov_gather / cov_columns) into nout doubles.  The handle's results, statistics and estimate are kept.
+static int cov_run(Solver* s, const char* fn, const std::vector<int>& rec, size_t nout, double* out) {
+  Solver::CovState& cv = s->cov;
+  Scratch sc{s, s->stream};
+  if (!sc.reserve(Scratch::al(4 * rec.size()) + Scratch::al(8 * std::max<size_t>(nout, 1)))) { g_err = "scratch allocation failed"; return -1; }
+  int* d_rec = sc.put(rec.data(), rec.size());
+  double* d_out = sc.put<double>(nullptr, nout);
+  if (!d_rec || !d_out) { g_err = "scratch allocation failed"; return -1; }
+  const bool compute = !cv.valid;
+  s->hd.Sig = static_cast<double*>(cv.mem);
+  s->hd.dcov = reinterpret_cast<const int*>(static_cast<char*>(cv.mem) + (size_t)s->dt.nd_cptr[s->dt.nb] * kAcTile * 8);
+  s->hd.crec = d_rec; s->hd.covout = d_out;
+  const LmResult res = s->res;
+  const pus_stats st = s->stats;
+  const int rc = launch(&s, 1, MODE_COV, 0, compute ? 1 : 0, 0.0);
+  const float ms = s->stats.kernel_ms;
+  s->res = res; s->stats = st; s->stats.kernel_ms = ms;
+  s->hd.crec = nullptr; s->hd.covout = nullptr;
+  if (rc < 0) { cv.valid = false; return -1; }
+  if (compute) {
+    unsigned flag = 0;
+    CUDA_OK(cudaMemcpy(&flag, s->hd.dflag, sizeof(flag), cudaMemcpyDeviceToHost));
+    if (flag) {
+      g_err = std::string(fn) + ": the undamped reduced system has a non-positive pivot, so J^T J is not positive definite at the "
+              "estimate (for example a graph without a pose prior, whose gauge is free); nothing is stored";
+      return -1;
+    }
+    cv.valid = true;
+  }
+  if (nout) CUDA_OK(cudaMemcpy(out, d_out, nout * 8, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// a live node: its compiled index, its dimension, its first row in the bordered order (-1: an eliminated plane)
+struct CovNode { bool pose; int idx, dim, row; };
+static bool cov_node(const Solver* s, int id, CovNode& n, const char* fn) {
+  const Graph& g = s->g;
+  if (id < 0 || id >= (int)g.nodes.size() || !g.nodes[id].alive) { g_err = std::string(fn) + ": bad node id " + std::to_string(id); return false; }
+  n.pose = g.nodes[id].kind == NODE_POSE;
+  n.idx = s->c.node_idx[id];
+  n.dim = n.pose ? 6 : 3;
+  n.row = cov_row(s->dt, n.pose, n.idx);
+  return true;
+}
+
+// records of the block (a, b), dim(a) x dim(b) row-major at out[o]: from Sigma's tiles when both nodes are kept and their tile
+// is stored, else one column solve per column of b (columns shared by every block with the same right-hand node)
+struct CovRecs {
+  std::vector<int> gather, cols, crec;
+  std::map<int, int> col_of;   // right-hand node id -> its first column
+};
+static void cov_block(const Solver* s, const CovNode& a, const CovNode& b, int bid, int o, CovRecs& R) {
+  const DirectTables& dt = s->dt;
+  const std::vector<int>& ip = s->cov.t.inc_ptr;
+  int tile = 0, off = 0, flag = 0;
+  if (a.row >= 0 && b.row >= 0 && cov_block_at(dt, a.row, b.row, tile, off, flag)) {
+    for (int p = 0; p < a.dim; p++)
+      for (int q = 0; q < b.dim; q++)
+        R.gather.insert(R.gather.end(), {0, o + p * b.dim + q, -1, tile, flag ? off + q * kAcLd + p : off + p * kAcLd + q, 0, 0, 0});
+    return;
+  }
+  auto it = R.col_of.find(bid);
+  if (it == R.col_of.end()) {
+    it = R.col_of.emplace(bid, (int)(R.cols.size() / 6)).first;
+    for (int q = 0; q < b.dim; q++) {
+      if (b.row >= 0) {
+        const int r = b.row + q;   // its entry of the right-hand side: 6 N pose rows, then 3 per bordered plane
+        R.cols.insert(R.cols.end(), {0, r < 6 * s->c.N ? r : 6 * s->c.N + r - 48 * dt.nbp, 0, 0, 0, 0});
+      } else {
+        R.cols.insert(R.cols.end(), {1, ip[b.idx], ip[b.idx + 1], q, 0, 0});
+      }
+    }
+  }
+  // (column records are grouped by column in cov_finish)
+  for (int q = 0; q < b.dim; q++)
+    for (int p = 0; p < a.dim; p++) {
+      const int col = it->second + q, oo = o + p * b.dim + q;
+      if (a.row >= 0) R.crec.insert(R.crec.end(), {col, 0, oo, a.row + p, 0, 0, 0});
+      else R.crec.insert(R.crec.end(), {col, 1, oo, ip[a.idx], ip[a.idx + 1], p, (!b.pose && b.row < 0 && b.idx == a.idx) ? a.idx * 9 + p * 3 + q : -1});
+    }
+}
+// the packed record array of cov_run: header, gather records, columns (with their record ranges), column records by column
+static std::vector<int> cov_finish(CovRecs& R) {
+  const int ncol = (int)(R.cols.size() / 6), ng = (int)(R.gather.size() / 8);
+  std::vector<std::vector<int>> by(ncol);
+  for (size_t k = 0; k < R.crec.size(); k += 7) by[R.crec[k]].insert(by[R.crec[k]].end(), R.crec.begin() + k + 1, R.crec.begin() + k + 7);
+  std::vector<int> out = {ng, ncol, 8, 0, 0, 0, 0, 0};
+  out.insert(out.end(), R.gather.begin(), R.gather.end());
+  out[3] = (int)out.size();
+  const size_t cbase = out.size();
+  out.insert(out.end(), R.cols.begin(), R.cols.end());
+  out[4] = (int)out.size();
+  int e = 0;
+  for (int k = 0; k < ncol; k++) {
+    out[cbase + 6 * k + 4] = e;
+    out.insert(out.end(), by[k].begin(), by[k].end());
+    e += (int)(by[k].size() / 6);
+    out[cbase + 6 * k + 5] = e;
+  }
+  return out;
+}
+
+int pus_marginal_covariances(pus_handle h, int n, const int* ids, double* out) {
+  NEED(h);
+  Solver* s = SV(h);
+  const char* fn = "pus_marginal_covariances";
+  if (n < 0) { g_err = std::string(fn) + ": n < 0"; return -1; }
+  if (cov_prepare(s, fn) < 0) return -1;
+  CovRecs R;
+  int o = 0;
+  for (int k = 0; k < n; k++) {
+    CovNode a;
+    if (!cov_node(s, ids[k], a, fn)) return -1;
+    if (a.row >= 0) {
+      cov_block(s, a, a, ids[k], o, R);
+    } else {   // an eliminated plane: entries r <= c, mirrored
+      for (int r = 0; r < 3; r++)
+        for (int cc = r; cc < 3; cc++) R.gather.insert(R.gather.end(), {1, o + 3 * r + cc, r == cc ? -1 : o + 3 * cc + r, a.idx, r, cc, 0, 0});
+    }
+    o += a.dim * a.dim;
+  }
+  if (cov_run(s, fn, cov_finish(R), (size_t)o, out) < 0) return -1;
+  return o;
+}
+
+long long pus_covariance_blocks(pus_handle h, int n_pairs, const int* id_pairs, double* out) {
+  NEED(h);
+  Solver* s = SV(h);
+  const char* fn = "pus_covariance_blocks";
+  if (n_pairs < 0) { g_err = std::string(fn) + ": n_pairs < 0"; return -1; }
+  if (cov_prepare(s, fn) < 0) return -1;
+  CovRecs R;
+  long long o = 0;
+  for (int k = 0; k < n_pairs; k++) {
+    CovNode a, b;
+    if (!cov_node(s, id_pairs[2 * k], a, fn) || !cov_node(s, id_pairs[2 * k + 1], b, fn)) return -1;
+    if (o + a.dim * b.dim > 0x7fffffffll) { g_err = std::string(fn) + ": more than 2^31 - 1 output values in one call"; return -1; }
+    cov_block(s, a, b, id_pairs[2 * k + 1], (int)o, R);
+    o += a.dim * b.dim;
+  }
+  if (cov_run(s, fn, cov_finish(R), (size_t)o, out) < 0) return -1;
+  return o;
+}
+
 long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long cap) {
   NEED(h);
   Solver* s = SV(h);
@@ -1739,6 +1937,20 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
   if (nm == "ndtcol") return ints(s->dt.nd_tcol);
   if (nm == "nduptr") return ints(s->dt.nd_uptr);
   if (nm == "ndupd") return ints(s->dt.nd_upd);
+  // marginal covariances of the ND layout (built here from the current tables): the selected-inversion list of every stored
+  // tile, the plane incidence ranges, the eliminated planes' observer-pair lists and the device bytes
+  if (nm.compare(0, 3, "cov") == 0) {
+    if (s->dt.order != 1) { g_err = nm + ": not a nested-dissection layout"; return -1; }
+    CovTables t;
+    std::string err;
+    if (!build_cov(c, s->dt, t, err)) { g_err = err; return -1; }
+    if (nm == "covsptr") return ints(t.sel_ptr);
+    if (nm == "covsel") return ints(t.sel);
+    if (nm == "covincptr") return ints(t.inc_ptr);
+    if (nm == "covpptr") return ints(t.pair_ptr);
+    if (nm == "covpair") return ints(t.pair);
+    if (nm == "covbytes") { if (cap >= 1) out[0] = (double)t.bytes; return 1; }
+  }
   if (nm == "pf_i") return ints(c.pf_i);
   if (nm == "pf_j") return ints(c.pf_j);
   if (nm == "pl_pose") return ints(c.pl_pose);
@@ -1825,6 +2037,7 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
 long long pus_debug_store(pus_handle h, const char* name, const double* in, long long count) {
   NEED(h);
   Solver* s = SV(h);
+  s->cov.valid = false;
   cudaSetDevice(s->device);
   if (std::string(name) == "Sdir") {   // direct mode: a dense row-major S (n x n) for debug stage 5, laid out as direct_assemble does
     if (s->linear_solver == 0) { g_err = "Sdir: not in direct linear-solver mode"; return -1; }

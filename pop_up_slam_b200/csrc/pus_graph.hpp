@@ -1159,4 +1159,119 @@ inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err, i
   return true;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Marginal covariances from the nested-dissection factor (DESIGN.md section 5.4), built by the first covariance call of a
+// layout.  Sigma = S^-1 is stored in the tiles of L's pattern (same storage index as L); in the new order, with
+// R_j = the tile rows i > j of column j:
+//   off-diagonal  Sigma_ij = -(sum_{k in R_j} Sigma_ik L_kj) L_jj^-1,     i in R_j
+//   diagonal      Sigma_jj = L_jj^-T (L_jj^-1 - sum_{k in R_j} L_kj^T Sigma_kj)
+// Every Sigma_ik read is a stored tile: i and k both lie in R_j, a clique of the pattern, so (max, min) is stored, and its
+// column min(i, k) is an ancestor of j (a higher level).  The diagonal tile's list is its column's own tiles, in storage
+// order; the off-diagonal tiles' lists are below.
+// ------------------------------------------------------------------------------------------------
+// the covariance tables the device reads, packed into one array (CovTables::dev): entries 0 .. 3 the offsets of the tables
+enum CovTable { COV_SPTR = 0, COV_SEL, COV_PPTR, COV_PAIR, COV_HDR };
+
+struct CovTables {
+  uint64_t topo = 0;                  // layout version the tables were built for (0: none)
+  std::vector<int> sel_ptr, sel;      // per stored tile (i, j), i > j: (Sigma tile (i,k) or (k,i)) * 2 + transposed, L tile (k, j),
+                                      // k in R_j ascending (empty for diagonal tiles)
+  std::vector<int> inc_ptr;           // per plane: its incidences [inc_ptr[l], inc_ptr[l + 1]) (plane-major, pose-ascending)
+  std::vector<int> pair_ptr, pair;    // per eliminated plane: its observer pairs (incidences qa >= qb), 4 ints each: qa, qb,
+                                      // Sigma tile, in-tile offset * 2 + transposed (the block Sigma_{pose qa, pose qb})
+  std::vector<int> dev;               // the tables above that the device reads, packed (CovTable)
+  long long nsel = 0;                 // list entries of the off-diagonal tiles
+  long long bytes = 0;                // device memory of the Sigma tiles and these tables
+};
+
+// The stored place of the block of Sigma whose rows start at row r0 and columns at c0 (both in the bordered order: 6 N pose
+// rows, then 3 per bordered plane from row 48 nbp), when its rows and columns each lie inside one tile: element (p, s) is at
+// tile * kAcTile + (flag ? off + s * ld + p : off + p * ld + s) with ld = 52.  False when the tile is not stored.
+inline bool cov_block_at(const DirectTables& d, int r0, int c0, int& tile, int& off, int& flag) {
+  const int ti = d.nd_pos[r0 / 48], tj = d.nd_pos[c0 / 48], er = r0 % 48, ec = c0 % 48;
+  const int hi = std::max(ti, tj), lo = std::min(ti, tj);
+  const int* b = d.nd_crow.data() + d.nd_cptr[lo];
+  const int n = d.nd_cptr[lo + 1] - d.nd_cptr[lo];
+  const int p = (int)(std::lower_bound(b, b + n, hi) - b);
+  if (p == n || b[p] != hi) return false;
+  tile = d.nd_toff[lo] + p;
+  flag = ti < tj ? 1 : 0;
+  off = flag ? ec * 52 + er : er * 52 + ec;
+  return true;
+}
+
+// The first row of a node's block in the bordered order, or -1 for an eliminated plane.  `pose`: compiled pose / plane index.
+inline int cov_row(const DirectTables& d, bool pose, int idx) {
+  if (pose) return 6 * idx;
+  const auto it = std::lower_bound(d.border.begin(), d.border.end(), idx);
+  if (it == d.border.end() || *it != idx) return -1;
+  return 48 * d.nbp + 3 * (int)(it - d.border.begin());
+}
+
+constexpr int kCovSelBytes = 8;   // bytes per off-diagonal list entry
+
+// Build the covariance tables of an ND layout; false (with a message) when the Sigma tiles, these tables and the layout's own
+// memory together exceed the band budget.
+inline bool build_cov(const Compiled& c, const DirectTables& d, CovTables& cv, std::string& err) {
+  cv = CovTables();
+  const int nb = d.nb, T = d.nd_cptr[nb], M = c.M;
+  cv.nsel = 0;
+  for (int j = 0; j < nb; j++) { const long long m = d.nd_cptr[j + 1] - d.nd_cptr[j] - 1; cv.nsel += m * m; }
+  cv.inc_ptr.assign(M + 1, 0);
+  for (int q = 0; q < (int)d.inc_plane.size(); q++) cv.inc_ptr[d.inc_plane[q] + 1]++;
+  for (int l = 0; l < M; l++) cv.inc_ptr[l + 1] += cv.inc_ptr[l];
+  std::vector<char> bord(M, 0);
+  for (int l : d.border) bord[l] = 1;
+  long long npair = 0;
+  for (int l = 0; l < M; l++)
+    if (!bord[l]) { const long long n = cv.inc_ptr[l + 1] - cv.inc_ptr[l]; npair += n * (n + 1) / 2; }
+  cv.bytes = (long long)T * kDirectTileBytes + kCovSelBytes * cv.nsel + 4ll * (T + 1) + 16 * npair + 4ll * (M + 1) + 4 * COV_HDR;
+  if (d.bytes + cv.bytes > kBandBudgetBytes) {
+    err = "marginal covariances: the graph needs " + std::to_string(d.bytes + cv.bytes) + " bytes of device memory (" +
+          std::to_string(d.bytes) + " for the factorization, " + std::to_string(cv.bytes) + " for the Sigma tiles and the selected-" +
+          "inversion lists, " + std::to_string(T) + " tiles); the budget is " + std::to_string(kBandBudgetBytes) + " bytes";
+    cv = CovTables();
+    return false;
+  }
+  cv.sel_ptr.assign(T + 1, 0);
+  cv.sel.reserve(2 * cv.nsel);
+  auto stored = [&](int i, int j) {   // storage index of tile (i, j), i >= j, inside the pattern
+    const int* b = d.nd_crow.data();
+    return d.nd_toff[j] + (int)(std::lower_bound(b + d.nd_cptr[j], b + d.nd_cptr[j + 1], i) - (b + d.nd_cptr[j]));
+  };
+  for (int t = 0; t < T; t++) {   // storage order
+    const int i = d.nd_trow[t], j = d.nd_tcol[t];
+    if (i != j) {
+      for (int p = d.nd_cptr[j] + 1; p < d.nd_cptr[j + 1]; p++) {
+        const int k = d.nd_crow[p];
+        cv.sel.push_back(2 * stored(std::max(i, k), std::min(i, k)) + (i < k ? 1 : 0));
+        cv.sel.push_back(d.nd_toff[j] + p - d.nd_cptr[j]);
+      }
+    }
+    cv.sel_ptr[t + 1] = (int)(cv.sel.size() / 2);
+  }
+  cv.pair_ptr.assign(M + 1, 0);
+  for (int l = 0; l < M; l++) {
+    if (!bord[l])
+      for (int qa = cv.inc_ptr[l]; qa < cv.inc_ptr[l + 1]; qa++)
+        for (int qb = cv.inc_ptr[l]; qb <= qa; qb++) {
+          int tile = 0, off = 0, flag = 0;
+          if (!cov_block_at(d, 6 * d.inc_pose[qa], 6 * d.inc_pose[qb], tile, off, flag)) {   // (eliminating l coupled them)
+            err = "marginal covariances: internal error: an observer pair of an eliminated plane lies outside L's pattern";
+            cv = CovTables();
+            return false;
+          }
+          cv.pair.insert(cv.pair.end(), {qa, qb, tile, 2 * off + flag});
+        }
+    cv.pair_ptr[l + 1] = (int)(cv.pair.size() / 4);
+  }
+  const std::vector<int>* tab[COV_HDR] = {&cv.sel_ptr, &cv.sel, &cv.pair_ptr, &cv.pair};
+  cv.dev.assign(COV_HDR, 0);
+  for (int k = 0; k < COV_HDR; k++) {
+    cv.dev[k] = (int)cv.dev.size();
+    cv.dev.insert(cv.dev.end(), tab[k]->begin(), tab[k]->end());
+  }
+  return true;
+}
+
 }  // namespace pus

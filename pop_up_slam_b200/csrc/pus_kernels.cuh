@@ -27,7 +27,7 @@ constexpr int kSlots = 5;  // pose blocks handled concurrently by one CTA (5 x 9
 constexpr int kTraceCap = 1024;
 constexpr int kMaxStage = 64;  // staged group members in the dense-block build
 
-enum KernelMode { MODE_BATCH = 0, MODE_UPDATE = 1, MODE_DEBUG = 2, MODE_CHI2 = 3 };
+enum KernelMode { MODE_BATCH = 0, MODE_UPDATE = 1, MODE_DEBUG = 2, MODE_CHI2 = 3, MODE_COV = 4 };
 
 struct LmParams {
   int method;  // 0 GN, 1 LM
@@ -138,6 +138,13 @@ struct DevGraph {
   // nested-dissection layout (null otherwise): its tables packed into one array (pus_graph.hpp, NdTable; nd(k) below); the
   // pose-pair lists are indexed 64 t + 8 (a % 8) + b % 8 by the stored tile t of the pair; the envelope tables above are unused
   const int* dnd;
+  // marginal covariances (pus::kdirect, ND layout; null otherwise, DESIGN.md section 5.4): Sigma in the tiles of L's pattern,
+  // the packed selected-inversion and plane-pair tables (pus_graph.hpp, CovTable; cov(k) below), and one call's records
+  // (header: gather records, columns, their offsets) and output
+  double* Sig;
+  const int* dcov;
+  const int* crec;
+  double* covout;
 };
 
 // The graph descriptor of the solve in progress and the dynamic shared memory, named at namespace scope so that every
@@ -3650,6 +3657,183 @@ struct Phase {
     }
     for (int i = tid_team(); i < n; i += nthr_team()) rv[i] = ldc(yv + 48 * ldc(nd(ND_POS) + i / 48) + i % 48);
     team_barrier(c);
+  }
+
+  // ---- marginal covariances from the ND factor (DESIGN.md section 5.4) ----
+  __device__ __forceinline__ static const int* cov(int k) { return G.dcov + ldc(G.dcov + k); }   // table k of CovTable
+
+  // Selected inversion: Sigma = S^-1 on L's tile pattern (in the new order), by descending level, with the tile ownership of
+  // nd_factor.  Per level:
+  //   (a) off-diagonal tiles  Sigma_ij = -(sum_k Sigma_ik L_kj) L_jj^-1 over the tile's list (k ascending); Sigma_ik is stored
+  //       at (i, k) or, transposed, at (k, i);                                team barrier
+  //   (b) diagonal tiles      Sigma_jj = L_jj^-T (L_jj^-1 - sum_k L_kj^T Sigma_kj) over the column's own tiles, stored as
+  //       (X + X^T) / 2;                                                       team barrier
+  // L_jj^-1 is applied once per output tile, after the sum, instead of forming L_kj L_jj^-1 per list entry: one product per
+  // tile instead of one per entry, and no staging buffer.  Every product reads final tiles in a fixed order, so every CTA
+  // that forms a tile gets the same bits.  L stays as it is (the column solves read it).
+  __device__ __noinline__ void nd_selinv() {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3, T = c.tsize;
+    double* Xa = reinterpret_cast<double*>(g_smem + kSmWork);
+    double* Xb = Xa + kAcTile;
+    auto frag = [&](int s, int& r, int& cc) {
+      const int q = warp + 16 * s;
+      r = 8 * (q / 6) + fr;
+      cc = 8 * (q % 6) + 2 * fc;
+      return q < 36;
+    };
+    auto load = [&](double* dst, const double* src, bool tr) {   // dst = src or src^T
+      for (int e = tid; e < 48 * 48; e += kThreads) {
+        const int r = e / 48, cc = e - r * 48;
+        dst[r * kAcLd + cc] = ldc(src + (tr ? cc * kAcLd + r : r * kAcLd + cc));
+      }
+    };
+    auto put = [&](double* dst, const double (&acc)[3][2], double sg) {
+      int r, cc;
+#pragma unroll
+      for (int s = 0; s < 3; s++)
+        if (frag(s, r, cc)) *reinterpret_cast<double2*>(dst + r * kAcLd + cc) = make_double2(sg * acc[s][0], sg * acc[s][1]);
+    };
+    for (int l = ldc(G.dnd) - 1; l >= 0; l--) {
+      const int t0 = ldc(nd(ND_LTPTR) + l), t1 = ldc(nd(ND_LTPTR) + l + 1);
+      for (int t = t0 + c.rank; t < t1; t += T) {   // (a)
+        const int j = ldc(nd(ND_TCOL) + t);
+        if (ldc(nd(ND_TROW) + t) == j) continue;
+        double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+        for (int u = ldc(cov(COV_SPTR) + t); u < ldc(cov(COV_SPTR) + t + 1); u++) {
+          const int sg = ldc(cov(COV_SEL) + 2 * u), lt = ldc(cov(COV_SEL) + 2 * u + 1);
+          __syncthreads();
+          load(Xa, tile_at(G.Sig, sg >> 1), sg & 1);
+          load(Xb, tile_at(G.Sd, lt), false);
+          __syncthreads();
+          mma48<false>(acc, Xa, Xb);
+        }
+        __syncthreads();
+        put(Xa, acc, -1.0);
+        load(Xb, tile_at(G.Dinv, j), false);
+        __syncthreads();
+        double out[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+        mma48<false>(out, Xa, Xb);
+        put(tile_at(G.Sig, t), out, 1.0);
+      }
+      __syncthreads();
+      team_barrier(c);
+      for (int t = t0 + c.rank; t < t1; t += T) {   // (b)
+        const int j = ldc(nd(ND_TCOL) + t);
+        if (ldc(nd(ND_TROW) + t) != j) continue;
+        const int cnt = ldc(nd(ND_CPTR) + j + 1) - ldc(nd(ND_CPTR) + j);
+        double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+        for (int k = t + 1; k < t + cnt; k++) {
+          __syncthreads();
+          load(Xa, tile_at(G.Sd, k), true);
+          load(Xb, tile_at(G.Sig, k), false);
+          __syncthreads();
+          mma48<false>(acc, Xa, Xb);
+        }
+        __syncthreads();
+        load(Xb, tile_at(G.Dinv, j), false);
+        load(Xa, tile_at(G.Dinv, j), true);
+        __syncthreads();
+        {
+          int r, cc;
+#pragma unroll
+          for (int s = 0; s < 3; s++)
+            if (frag(s, r, cc)) { Xb[r * kAcLd + cc] -= acc[s][0]; Xb[r * kAcLd + cc + 1] -= acc[s][1]; }
+        }
+        __syncthreads();
+        double out[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+        mma48<false>(out, Xa, Xb);
+        __syncthreads();
+        put(Xa, out, 1.0);
+        __syncthreads();
+        double* dst = tile_at(G.Sig, t);
+        for (int e = tid; e < 48 * 48; e += kThreads) {
+          const int r = e / 48, cc = e - r * 48;
+          dst[r * kAcLd + cc] = 0.5 * (Xa[r * kAcLd + cc] + Xa[cc * kAcLd + r]);
+        }
+      }
+      __syncthreads();
+      team_barrier(c);
+    }
+  }
+
+  // The gather records of one covariance call, one output entry per thread (crec header: [0] count, [2] offset; 8 ints each):
+  //   kind 0  out[o1] = Sigma element (tile, in-tile offset)                        (a pose or bordered plane inside the pattern)
+  //   kind 1  entry (r, c) of an eliminated plane l:  (Hll^-1)_rc + sum over its observer pairs (a >= b) of
+  //           (Y_a^T Sigma_ab Y_b)_rc, plus (Y_a^T Sigma_ab Y_b)_cr when a != b;  to out[o1] and out[o2] (o2 = -1: none)
+  __device__ __noinline__ void cov_gather() {
+    const int n = ldc(G.crec);
+    const int* rec = G.crec + ldc(G.crec + 2);
+    for (int k = tid_team(); k < n; k += nthr_team()) {
+      const int* e = rec + 8 * k;
+      const int o1 = ldc(e + 1), o2 = ldc(e + 2);
+      double v;
+      if (ldc(e) == 0) {
+        v = ldc(tile_at(G.Sig, ldc(e + 3)) + ldc(e + 4));
+      } else {
+        const int l = ldc(e + 3), r = ldc(e + 4), cc = ldc(e + 5);
+        v = ldc(G.Hinv + (size_t)l * 9 + r * 3 + cc);
+        for (int u = ldc(cov(COV_PPTR) + l); u < ldc(cov(COV_PPTR) + l + 1); u++) {
+          const int* q = cov(COV_PAIR) + 4 * u;
+          const int qa = ldc(q), qb = ldc(q + 1), code = ldc(q + 3);
+          const double* S = tile_at(G.Sig, ldc(q + 2)) + (code >> 1);
+          const double* ya = G.Yd + (size_t)qa * 18;
+          const double* yb = G.Yd + (size_t)qb * 18;
+          for (int p = 0; p < 6; p++)
+            for (int s = 0; s < 6; s++) {
+              const double sig = ldc(S + ((code & 1) ? s * kAcLd + p : p * kAcLd + s));
+              v += ldc(ya + p * 3 + r) * sig * ldc(yb + s * 3 + cc);
+              if (qa != qb) v += ldc(ya + p * 3 + cc) * sig * ldc(yb + s * 3 + r);
+            }
+        }
+      }
+      G.covout[o1] = v;
+      if (o2 >= 0) G.covout[o2] = v;
+    }
+  }
+
+  // Blocks outside the pattern, one column of the right-hand node at a time (crec header: [1] columns, [3] their offset,
+  // 6 ints each: kind, a, b, c, first and end record; [4] the records' offset, 6 ints each).  A column is x = S^-1 rhs by
+  // nd_trsv with rhs = e_a (kind 0: a pose or bordered plane, a its row of b) or -Y_{.l} column c (kind 1: an eliminated
+  // plane l, its incidences [a, b)); x is then the column of Sigma over the kept unknowns.  Records:
+  //   kind 0  out[o] = x[a]                                                          (a kept row)
+  //   kind 1  out[o] = -sum_{q in [a, b)} (Y_q^T x_pose(q))_c + (e >= 0 ? Hll^-1 entry e : 0)   (row c of an eliminated plane)
+  __device__ __noinline__ void cov_columns() {
+    const int ncol = ldc(G.crec + 1), nk = 6 * G.N + 3 * G.dnbord;
+    const int* col = G.crec + ldc(G.crec + 3);
+    const int* rec = G.crec + ldc(G.crec + 4);
+    for (int k = 0; k < ncol; k++) {
+      const int* cl = col + 6 * k;
+      const int kind = ldc(cl), a = ldc(cl + 1), b = ldc(cl + 2), cc = ldc(cl + 3);
+      for (int i = tid_team(); i < nk; i += nthr_team()) G.b[i] = 0.0;
+      team_barrier(c);
+      if (kind == 0) {
+        if (tid_team() == 0) G.b[a] = 1.0;
+      } else {
+        for (int q = a + tid_team(); q < b; q += nthr_team()) {
+          const int p = ldc(G.pl_pose + ldc(G.dinc_lo + q));
+          for (int r = 0; r < 6; r++) G.b[6 * p + r] = -ldc(G.Yd + (size_t)q * 18 + r * 3 + cc);
+        }
+      }
+      team_barrier(c);
+      nd_trsv();
+      for (int e = ldc(cl + 4) + tid_team(); e < ldc(cl + 5); e += nthr_team()) {
+        const int* x = rec + 6 * e;
+        double v;
+        if (ldc(x) == 0) {
+          v = ldc(G.dvec + ldc(x + 2));
+        } else {
+          const int m = ldc(x + 4), h = ldc(x + 5);
+          double s = 0.0;
+          for (int q = ldc(x + 2); q < ldc(x + 3); q++) {
+            const int p = ldc(G.pl_pose + ldc(G.dinc_lo + q));
+            for (int r = 0; r < 6; r++) s += ldc(G.Yd + (size_t)q * 18 + r * 3 + m) * ldc(G.dvec + 6 * p + r);
+          }
+          v = (h >= 0 ? ldc(G.Hinv + h) : 0.0) - s;
+        }
+        G.covout[ldc(x + 1)] = v;
+      }
+      team_barrier(c);
+    }
   }
 #endif
 };
