@@ -324,16 +324,10 @@ static int upload(Solver* s) {
       UPD(dlp_ptr, dt.lp_ptr); UPD(dlp_a, dt.lp_a); UPD(dlp_b, dt.lp_b); UPD(dfp_ptr, dt.fp_ptr); UPD(dfp_f, dt.fp_f);
       UPD(dfirst, dt.first); UPD(dtoff, dt.toff); UPD(dpoff, dt.poff); UPD(dcol_ptr, dt.col_ptr); UPD(dcol_row, dt.col_row);
       UPD(dbord, dt.border); UPD(dbinc, dt.binc);
-      size_t ntile = 0;
-      if (dt.order == 1) {
-        UPD(dnd, dt.nd_dev);
-        ntile = dt.nd_cptr[nb];
-      } else {
-        ntile = dt.toff[nb];
-      }
+      if (dt.order == 1) UPD(dnd, dt.nd_dev);
 #undef UPD
       AL(Wd, ninc * 18, "Wd"); AL(Yd, ninc * 18, "Yd");
-      AL(Sd, ntile * kAcTile, nullptr); AL(Dsnap, dt.order == 1 ? 1 : 2 * nb * kAcTile, nullptr); AL(Dinv, nb * kAcTile, nullptr);
+      AL(Sd, (size_t)dt.ntile() * kAcTile, nullptr); AL(Dsnap, dt.order == 1 ? 1 : 2 * nb * kAcTile, nullptr); AL(Dinv, nb * kAcTile, nullptr);
       AL(dvec, 2 * 48 * nb, nullptr);
       if (s->dalloc(&d.dflag, 1) < 0) return -1;
     }
@@ -1688,13 +1682,6 @@ int pus_load_isam_dataset(pus_handle h, const char* path, int* n_poses, int* n_f
 // order of the direct solve's system without padding (6 N, then 3 per bordered plane), and row r's row in the padded layout
 static int direct_order(const Solver* s) { return 6 * s->c.N + 3 * (int)s->dt.border.size(); }
 static int direct_row(const Solver* s, int r) { return r < 6 * s->c.N ? r : 48 * s->dt.nbp + r - 6 * s->c.N; }
-// nested-dissection layout: row r's row in the permuted padded order, and the stored tile (i, j), i >= j, or -1 outside L's pattern
-static int nd_row(const Solver* s, int r) { const int p = direct_row(s, r); return 48 * s->dt.nd_pos[p / 48] + p % 48; }
-static long long nd_tile(const DirectTables& dt, int i, int j) {
-  const int* b = dt.nd_crow.data();
-  const int* at = std::lower_bound(b + dt.nd_cptr[j], b + dt.nd_cptr[j + 1], i);
-  return (at == b + dt.nd_cptr[j + 1] || *at != i) ? -1 : dt.nd_toff[j] + (at - (b + dt.nd_cptr[j]));
-}
 
 // ---- marginal covariances (DESIGN.md section 5.4) ----
 // Refuse every handle but kind 2 in ND order; re-upload as the exports do; build the layout's tables on the first call and
@@ -1717,7 +1704,7 @@ static int cov_prepare(Solver* s, const char* fn) {
   cv.valid = false;
   std::string err;
   if (!build_cov(s->c, s->dt, cv.t, err)) { g_err = std::string(fn) + ": " + err; return -1; }
-  const size_t sig = (size_t)s->dt.nd_cptr[s->dt.nb] * kAcTile * 8, need = sig + cv.t.dev.size() * 4;
+  const size_t sig = (size_t)s->dt.ntile() * kAcTile * 8, need = sig + cv.t.dev.size() * 4;
   CUDA_OK(cudaSetDevice(s->device));
   if (need > cv.bytes) {
     if (cv.mem) { cudaStreamSynchronize(s->stream); cudaFree(cv.mem); cv.mem = nullptr; cv.bytes = 0; }
@@ -1746,7 +1733,7 @@ static int cov_run(Solver* s, const char* fn, const std::vector<int>& rec, size_
   if (!d_rec || !d_out) { g_err = "scratch allocation failed"; return -1; }
   const bool compute = !cv.valid;
   s->hd.Sig = static_cast<double*>(cv.mem);
-  s->hd.dcov = reinterpret_cast<const int*>(static_cast<char*>(cv.mem) + (size_t)s->dt.nd_cptr[s->dt.nb] * kAcTile * 8);
+  s->hd.dcov = reinterpret_cast<const int*>(static_cast<char*>(cv.mem) + (size_t)s->dt.ntile() * kAcTile * 8);
   s->hd.crec = d_rec; s->hd.covout = d_out;
   const LmResult res = s->res;
   const pus_stats st = s->stats;
@@ -1789,7 +1776,7 @@ struct CovRecs {
 };
 static void cov_block(const Solver* s, const CovNode& a, const CovNode& b, int bid, int o, CovRecs& R) {
   const DirectTables& dt = s->dt;
-  const std::vector<int>& ip = s->cov.t.inc_ptr;
+  const std::vector<int>& ip = dt.inc_ptr;
   int tile = 0, off = 0, flag = 0;
   if (a.row >= 0 && b.row >= 0 && cov_block_at(dt, a.row, b.row, tile, off, flag)) {
     for (int p = 0; p < a.dim; p++)
@@ -1946,7 +1933,7 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
     if (!build_cov(c, s->dt, t, err)) { g_err = err; return -1; }
     if (nm == "covsptr") return ints(t.sel_ptr);
     if (nm == "covsel") return ints(t.sel);
-    if (nm == "covincptr") return ints(t.inc_ptr);
+    if (nm == "covincptr") return ints(s->dt.inc_ptr);
     if (nm == "covpptr") return ints(t.pair_ptr);
     if (nm == "covpair") return ints(t.pair);
     if (nm == "covbytes") { if (cap >= 1) out[0] = (double)t.bytes; return 1; }
@@ -1978,27 +1965,21 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
     if (s->linear_solver == 0) { g_err = "not in direct linear-solver mode"; return -1; }
     const DirectTables& dt = s->dt;
     const int n = direct_order(s);   // (band: 6 N pose rows, then 3 per bordered plane, padding stripped)
-    const size_t total = (size_t)(dt.order == 1 ? dt.nd_cptr[dt.nb] : dt.toff[dt.nb]) * kAcTile;
+    const size_t total = (size_t)dt.ntile() * kAcTile;
     std::vector<double> tmp(total);
     if (cudaMemcpy(tmp.data(), s->hd.Sd, total * 8, cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
     const long long cnt = (long long)n * n;
-    if (cnt <= cap && dt.order == 1) {   // Sdir in the bordered order; Ldir, the factor of P S P^T, in the permuted order
+    if (cnt <= cap) {   // Sdir in the bordered order; Ldir, the factor of P S P^T, in the factor's order
       std::vector<int> nr(n), rows(n);
-      for (int r = 0; r < n; r++) { nr[r] = nd_row(s, r); rows[r] = r; }
+      for (int r = 0; r < n; r++) { nr[r] = dt.row(direct_row(s, r)); rows[r] = r; }
       if (nm == "Ldir") std::sort(rows.begin(), rows.end(), [&](int x, int y) { return nr[x] < nr[y]; });
       for (int a = 0; a < n; a++)
         for (int b = 0; b < n; b++) {
           const int I = std::max(nr[rows[a]], nr[rows[b]]), J = std::min(nr[rows[a]], nr[rows[b]]);
-          const long long t = (b > a) ? -1 : nd_tile(dt, I / 48, J / 48);
+          const int t = (b > a) ? -1 : dt.tile(I / 48, J / 48);
           out[(size_t)a * n + b] = t < 0 ? 0.0 : tmp[(size_t)t * kAcTile + (I % 48) * kAcLd + J % 48];
         }
-    } else if (cnt <= cap)
-      for (int r = 0; r < n; r++)
-        for (int q = 0; q < n; q++) {
-          const int pr = direct_row(s, r), pq = direct_row(s, q), ti = pr / 48, tj = pq / 48;
-          out[(size_t)r * n + q] = (q > r || tj < dt.first[ti]) ? 0.0
-                                   : tmp[(size_t)(dt.toff[ti] + tj - dt.first[ti]) * kAcTile + (pr % 48) * kAcLd + pq % 48];
-        }
+    }
     return cnt;
   }
   if (nm == "dflag") {   // direct mode: 1 when the last factorization met a non-positive pivot, else 0
@@ -2049,51 +2030,31 @@ long long pus_debug_store(pus_handle h, const char* name, const double* in, long
                                     : "Sdir: expected (6 N + 3 B)^2 = " + std::to_string((long long)n * n) + " elements";
       return -1;
     }
-    std::vector<int> orig(48 * nb, -1);   // padded row -> row of the stored matrix (-1: padding)
-    for (int r = 0; r < n; r++) orig[direct_row(s, r)] = r;
-    if (dt.order == 1) {   // nested dissection: tile (i, j) of the new order holds P S P^T, lower half
-      for (int r = 0; r < n; r++)
-        for (int q = 0; q < r; q++) {
-          const int I = std::max(nd_row(s, r), nd_row(s, q)), J = std::min(nd_row(s, r), nd_row(s, q));
-          if (in[(size_t)r * n + q] != 0.0 && nd_tile(dt, I / 48, J / 48) < 0) {
-            g_err = "Sdir: entry (" + std::to_string(r) + ", " + std::to_string(q) + ") lies outside the nested-dissection pattern";
-            return -1;
-          }
-        }
-      const int T = dt.nd_cptr[nb];
-      std::vector<double> tiles((size_t)T * kAcTile, 0.0);
-      for (int t = 0; t < T; t++) {
-        const int ti = dt.nd_trow[t], tj = dt.nd_tcol[t];
-        for (int er = 0; er < 48; er++)
-          for (int ec = 0; ec < 48; ec++) {
-            const int oi = orig[48 * dt.nd_perm[ti] + er], oj = orig[48 * dt.nd_perm[tj] + ec];
-            double v = 0.0;
-            if (ti == tj && ec > er) v = 0.0;
-            else if (oi < 0 || oj < 0) v = (ti == tj && er == ec) ? 1.0 : 0.0;   // identity padding
-            else v = in[(size_t)std::max(oi, oj) * n + std::min(oi, oj)];
-            tiles[(size_t)t * kAcTile + er * kAcLd + ec] = v;
-          }
-      }
-      if (cudaMemcpy(s->hd.Sd, tiles.data(), tiles.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) { g_err = "memcpy"; return -1; }
-      return count;
-    }
+    std::vector<int> orig(48 * nb, -1);   // row in the factor's order -> row of the stored matrix (-1: padding)
+    for (int r = 0; r < n; r++) orig[dt.row(direct_row(s, r))] = r;
     for (int r = 0; r < n; r++)
-      for (int q = 0; q < r; q++)
-        if (in[(size_t)r * n + q] != 0.0 && direct_row(s, q) / 48 < dt.first[direct_row(s, r) / 48]) {
-          g_err = "Sdir: entry (" + std::to_string(r) + ", " + std::to_string(q) + ") lies outside the band layout's envelope";
+      for (int q = 0; q < r; q++) {
+        const int pr = dt.row(direct_row(s, r)), pq = dt.row(direct_row(s, q));
+        if (in[(size_t)r * n + q] != 0.0 && dt.tile(std::max(pr, pq) / 48, std::min(pr, pq) / 48) < 0) {
+          g_err = "Sdir: entry (" + std::to_string(r) + ", " + std::to_string(q) + ") lies outside " +
+                  (dt.order == 1 ? "the nested-dissection pattern" : "the band layout's envelope");
           return -1;
         }
-    std::vector<double> tiles((size_t)dt.toff[nb] * kAcTile, 0.0);
+      }
+    std::vector<double> tiles((size_t)dt.ntile() * kAcTile, 0.0);   // the lower half, identity padding
     for (int ti = 0; ti < nb; ti++)
-      for (int tj = dt.first[ti]; tj <= ti; tj++) {
-        double* t = tiles.data() + (size_t)(dt.toff[ti] + tj - dt.first[ti]) * kAcTile;
+      for (int tj = 0; tj <= ti; tj++) {
+        const int t = dt.tile(ti, tj);
+        if (t < 0) continue;
         for (int er = 0; er < 48; er++)
           for (int ec = 0; ec < 48; ec++) {
             const int i = 48 * ti + er, j = 48 * tj + ec, oi = orig[i], oj = orig[j];
-            t[er * kAcLd + ec] = j > i ? 0.0 : ((oi < 0 || oj < 0) ? (i == j ? 1.0 : 0.0) : in[(size_t)oi * n + oj]);   // lower half, identity padding
+            tiles[(size_t)t * kAcTile + er * kAcLd + ec] =
+                j > i ? 0.0 : ((oi < 0 || oj < 0) ? (i == j ? 1.0 : 0.0) : in[(size_t)std::max(oi, oj) * n + std::min(oi, oj)]);
           }
       }
     if (cudaMemcpy(s->hd.Sd, tiles.data(), tiles.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) { g_err = "memcpy"; return -1; }
+    if (dt.order == 1) return count;
     for (int ti = 0; ti < nb; ti++) {   // a row's first tile is also the pivot-column snapshot of the step that first reads it
       const int f = dt.first[ti];
       if (cudaMemcpy(s->hd.Dsnap + ((size_t)(f & 1) * nb + ti) * kAcTile, tiles.data() + (size_t)dt.toff[ti] * kAcTile, kAcTile * 8,

@@ -665,6 +665,7 @@ struct DirectTables {
   int nb = 0;    // tile rows of the padded order 48 nb
   int nbp = 0;   // tile rows of the poses (>= 6 N / 48); the bordered planes' rows start at tile row nbp
   std::vector<int> inc_pose, inc_plane, inc_lo, inc_hi;
+  std::vector<int> inc_ptr;             // per plane l: its incidences [inc_ptr[l], inc_ptr[l + 1])
   std::vector<int> lp_ptr, lp_a, lp_b, fp_ptr, fp_f;
   std::vector<int> first, toff, poff;   // per tile row: first tile column, tile offset (+ total); per pose: first pair index
   std::vector<int> col_ptr, col_row;    // per tile column K: the tile rows i > K with first[i] <= K, ascending
@@ -684,6 +685,17 @@ struct DirectTables {
   std::vector<int> nd_uptr, nd_upd;     // per stored tile (i, j): pairs (tile of L_iK, tile of L_jK), K < j ascending
   std::vector<int> nd_rptr, nd_rtile;   // per tile row j: the tiles (j, K), K < j ascending
   std::vector<int> nd_dev;              // the tables above that the device reads, packed (NdTable)
+
+  // the storage index of tile (i, j), i >= j, of the factor's order, or -1 outside the stored pattern
+  int tile(int i, int j) const {
+    if (order != 1) return j < first[i] ? -1 : toff[i] + j - first[i];
+    const int* b = nd_crow.data() + nd_cptr[j];
+    const int n = nd_cptr[j + 1] - nd_cptr[j], p = (int)(std::lower_bound(b, b + n, i) - b);
+    return (p == n || b[p] != i) ? -1 : nd_toff[j] + p;
+  }
+  // padded row r of the bordered order -> its row in the factor's order (the identity in insertion order)
+  int row(int r) const { return order == 1 ? 48 * nd_pos[r / 48] + r % 48 : r; }
+  int ntile() const { return order == 1 ? nd_cptr[nb] : toff[nb]; }   // stored tiles
 };
 
 // ---- nested-dissection order of the pose tiles (kind 2, order 1) ----
@@ -872,10 +884,6 @@ inline void nd_tables(DirectTables& d) {
     }
   }
   d.nd_ltptr[d.nlev] = t;
-  auto tile = [&](int i, int j) {   // the stored tile (i, j), i >= j inside the pattern
-    const int* b = d.nd_crow.data();
-    return d.nd_toff[j] + (int)(std::lower_bound(b + d.nd_cptr[j], b + d.nd_cptr[j + 1], i) - (b + d.nd_cptr[j]));
-  };
   d.nd_uptr.assign(T + 1, 0);
   d.nd_rptr.assign(nb + 1, 0);
   for (int pass = 0; pass < 2; pass++) {
@@ -894,7 +902,7 @@ inline void nd_tables(DirectTables& d) {
         const int i = d.nd_crow[a];
         if (pass == 0) d.nd_rptr[i + 1]++; else d.nd_rtile[rfill[i]++] = t0 + a;
         for (int b = p0; b <= a; b++) {
-          const int q = tile(i, d.nd_crow[b]);
+          const int q = d.tile(i, d.nd_crow[b]);
           if (pass == 0) d.nd_uptr[q + 1]++;
           else { const int at = fill[q]++; d.nd_upd[2 * at] = t0 + a; d.nd_upd[2 * at + 1] = t0 + b; }
         }
@@ -950,79 +958,56 @@ inline long long band_envelope(const Compiled& c, const std::vector<int>& inc_pt
          + 8 * (2ll * 48 * nb + 36 * ninc + 3ll * nbord) + 4 * ints;   // solve vectors, W / Y per incidence, border rhs, tables
 }
 
-// kind 2, order 1: the nested-dissection layout.  Bordering: the k planes seen from the most distinct pose tiles (ties: lower
-// index), k = 0 .. min(M, 64), whichever k takes the fewest device bytes (ties: the smaller k).  A revisited plane has a wide
-// span but a small clique, so the span rule of the insertion order is the wrong measure here.
-inline bool build_nd(const Compiled& c, DirectTables& d, std::string& err, const std::vector<int>& inc_ptr) {
-  const int N = c.N, M = c.M;
-  std::vector<int> ntile(M, 0), order(M);
-  for (int l = 0; l < M; l++) {
-    int last = -1;
-    for (int i = inc_ptr[l]; i < inc_ptr[l + 1]; i++)
-      if (d.inc_pose[i] / 8 != last) { last = d.inc_pose[i] / 8; ntile[l]++; }
-    order[l] = l;
-  }
-  std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return ntile[x] > ntile[y]; });
+// Bordering: rank the planes by `key` (descending; ties: lower index) and border the k first, k = 0 .. min(M, 64), whichever
+// k takes the fewest device bytes (ties: the smaller k); bytes(bslot, k) is the device bytes of a layout.  Out: the bordered
+// planes (ascending) and each plane's slot among them (-1: eliminated).
+template <typename Bytes>
+inline void choose_border(const std::vector<int>& key, Bytes bytes, std::vector<int>& border, std::vector<int>& bslot) {
+  const int M = (int)key.size();
+  std::vector<int> order(M);
+  for (int l = 0; l < M; l++) order[l] = l;
+  std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return key[x] > key[y]; });
+  auto pick = [&](int k) {
+    border.assign(order.begin(), order.begin() + k);
+    std::sort(border.begin(), border.end());
+    bslot.assign(M, -1);
+    for (int q = 0; q < k; q++) bslot[border[q]] = q;
+  };
   long long best = -1;
   int best_k = 0;
-  std::vector<int> bs(M, -1);
   for (int k = 0; k <= std::min(M, kBandMaxBorder); k++) {
-    std::fill(bs.begin(), bs.end(), -1);
-    std::vector<int> chosen(order.begin(), order.begin() + k);
-    std::sort(chosen.begin(), chosen.end());
-    for (int q = 0; q < k; q++) bs[chosen[q]] = q;
-    DirectTables t;
-    const long long bytes = nd_layout(c, inc_ptr, d.inc_pose, bs, k, t);
-    if (best < 0 || bytes < best) { best = bytes; best_k = k; }
+    pick(k);
+    const long long b = bytes(bslot, k);
+    if (best < 0 || b < best) { best = b; best_k = k; }
   }
-  d.border.assign(order.begin(), order.begin() + best_k);
-  std::sort(d.border.begin(), d.border.end());
-  std::fill(bs.begin(), bs.end(), -1);
-  for (int q = 0; q < best_k; q++) bs[d.border[q]] = q;
-  d.bytes = nd_layout(c, inc_ptr, d.inc_pose, bs, best_k, d);
-  if (d.bytes > kBandBudgetBytes) {
-    err = "band linear solver (nested-dissection order): the graph needs " + std::to_string(d.bytes) + " bytes of device memory (" +
-          std::to_string(N) + " poses, " + std::to_string(best_k) + " bordered planes, " + std::to_string(d.nd_cptr[d.nb]) +
-          " tiles); the budget is " + std::to_string(kBandBudgetBytes) + " bytes (use the PCG solver, kind 0)";
-    return false;
-  }
-  for (int q = 0; q < best_k; q++) { d.binc.push_back(inc_ptr[d.border[q]]); d.binc.push_back(inc_ptr[d.border[q] + 1]); }
-  nd_tables(d);
-  // per-pose-pair lists: pair (a, b), a >= b in insertion order, of the stored tile t that holds it, at 64 t + 8 (a % 8) + b % 8
-  auto pair = [&](int a, int b) {
-    int i = d.nd_pos[a / 8], j = d.nd_pos[b / 8];
-    if (i < j) std::swap(i, j);
-    const int* r = d.nd_crow.data();
-    const int t = d.nd_toff[j] + (int)(std::lower_bound(r + d.nd_cptr[j], r + d.nd_cptr[j + 1], i) - (r + d.nd_cptr[j]));
-    return (size_t)64 * t + 8 * (a % 8) + b % 8;
-  };
-  const size_t np = (size_t)64 * d.nd_cptr[d.nb];
+  pick(best_k);
+}
+
+// The per-pose-pair assembly lists; pair(a, b) is the index of the pose pair (a, b), a >= b in insertion order.  lp: the
+// incidence pairs (i, j), i >= j, of every eliminated plane (incidences are pose-ascending inside a plane: i >= j gives
+// a >= b); fp: the pose-pose factors, f * 2 + side (side 1: a is the factor's second pose).
+template <typename Pair>
+inline void pair_lists(const Compiled& c, const std::vector<int>& bslot, size_t np, Pair pair, DirectTables& d) {
   d.lp_ptr.assign(np + 1, 0);
-  for (int pass = 0; pass < 2; pass++) {
-    std::vector<int> fill;
-    if (pass == 1) {
-      for (size_t q = 0; q < np; q++) d.lp_ptr[q + 1] += d.lp_ptr[q];
-      d.lp_a.assign(std::max(1, d.lp_ptr[np]), 0);
-      d.lp_b.assign(std::max(1, d.lp_ptr[np]), 0);
-      fill.assign(d.lp_ptr.begin(), d.lp_ptr.end() - 1);
-    }
-    for (int l = 0; l < M; l++) {
-      if (bs[l] >= 0) continue;
-      for (int i = inc_ptr[l]; i < inc_ptr[l + 1]; i++)
-        for (int j = inc_ptr[l]; j <= i; j++) {
-          const size_t q = pair(d.inc_pose[i], d.inc_pose[j]);
-          if (pass == 0) d.lp_ptr[q + 1]++;
-          else { const int at = fill[q]++; d.lp_a[at] = i; d.lp_b[at] = j; }
-        }
-    }
-  }
   d.fp_ptr.assign(np + 1, 0);
   for (int pass = 0; pass < 2; pass++) {
-    std::vector<int> fill;
+    std::vector<int> lfill, ffill;
     if (pass == 1) {
-      for (size_t q = 0; q < np; q++) d.fp_ptr[q + 1] += d.fp_ptr[q];
+      for (size_t q = 0; q < np; q++) { d.lp_ptr[q + 1] += d.lp_ptr[q]; d.fp_ptr[q + 1] += d.fp_ptr[q]; }
+      d.lp_a.assign(std::max(1, d.lp_ptr[np]), 0);
+      d.lp_b.assign(std::max(1, d.lp_ptr[np]), 0);
       d.fp_f.assign(std::max(1, d.fp_ptr[np]), 0);
-      fill.assign(d.fp_ptr.begin(), d.fp_ptr.end() - 1);
+      lfill.assign(d.lp_ptr.begin(), d.lp_ptr.end() - 1);
+      ffill.assign(d.fp_ptr.begin(), d.fp_ptr.end() - 1);
+    }
+    for (int l = 0; l < c.M; l++) {
+      if (bslot[l] >= 0) continue;
+      for (int i = d.inc_ptr[l]; i < d.inc_ptr[l + 1]; i++)
+        for (int j = d.inc_ptr[l]; j <= i; j++) {
+          const size_t q = pair(d.inc_pose[i], d.inc_pose[j]);
+          if (pass == 0) d.lp_ptr[q + 1]++;
+          else { const int at = lfill[q]++; d.lp_a[at] = i; d.lp_b[at] = j; }
+        }
     }
     for (int f = 0; f < c.Epf; f++) {
       if (c.pf_j[f] < 0) continue;
@@ -1031,10 +1016,39 @@ inline bool build_nd(const Compiled& c, DirectTables& d, std::string& err, const
         if (a < b) continue;
         const size_t q = pair(a, b);
         if (pass == 0) d.fp_ptr[q + 1]++;
-        else d.fp_f[fill[q]++] = f * 2 + side;
+        else d.fp_f[ffill[q]++] = f * 2 + side;
       }
     }
   }
+}
+
+// kind 2, order 1: the nested-dissection layout.  Bordering ranks the planes by the number of distinct pose tiles that observe
+// them: a revisited plane has a wide span but a small clique, so the span rule of the insertion order is the wrong measure here.
+inline bool build_nd(const Compiled& c, DirectTables& d, std::string& err) {
+  const int N = c.N, M = c.M;
+  std::vector<int> ntile(M, 0), bslot;
+  for (int l = 0; l < M; l++) {
+    int last = -1;
+    for (int i = d.inc_ptr[l]; i < d.inc_ptr[l + 1]; i++)
+      if (d.inc_pose[i] / 8 != last) { last = d.inc_pose[i] / 8; ntile[l]++; }
+  }
+  choose_border(ntile, [&](const std::vector<int>& bs, int k) { DirectTables t; return nd_layout(c, d.inc_ptr, d.inc_pose, bs, k, t); },
+                d.border, bslot);
+  const int nbord = (int)d.border.size();
+  d.bytes = nd_layout(c, d.inc_ptr, d.inc_pose, bslot, nbord, d);
+  if (d.bytes > kBandBudgetBytes) {
+    err = "band linear solver (nested-dissection order): the graph needs " + std::to_string(d.bytes) + " bytes of device memory (" +
+          std::to_string(N) + " poses, " + std::to_string(nbord) + " bordered planes, " + std::to_string(d.nd_cptr[d.nb]) +
+          " tiles); the budget is " + std::to_string(kBandBudgetBytes) + " bytes (use the PCG solver, kind 0)";
+    return false;
+  }
+  for (int l : d.border) { d.binc.push_back(d.inc_ptr[l]); d.binc.push_back(d.inc_ptr[l + 1]); }
+  nd_tables(d);
+  // pair (a, b) lies in the stored tile t that holds it, at 64 t + 8 (a % 8) + b % 8
+  pair_lists(c, bslot, (size_t)64 * d.nd_cptr[d.nb], [&](int a, int b) {
+    const int i = d.nd_pos[a / 8], j = d.nd_pos[b / 8];
+    return (size_t)64 * d.tile(std::max(i, j), std::min(i, j)) + 8 * (a % 8) + b % 8;
+  }, d);
   return true;
 }
 
@@ -1048,7 +1062,7 @@ inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err, i
           std::to_string(kDirectMaxPoses) + " (use the PCG solver, kind 0)";
     return false;
   }
-  std::vector<int> inc_ptr(M + 1, 0);
+  d.inc_ptr.assign(M + 1, 0);
   for (int l = 0; l < M; l++) {
     for (int s = c.pl_ptr[l]; s < c.pl_ptr[l + 1];) {
       int e = s + 1;
@@ -1056,50 +1070,36 @@ inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err, i
       d.inc_pose.push_back(c.pl_pose[s]); d.inc_plane.push_back(l); d.inc_lo.push_back(s); d.inc_hi.push_back(e);
       s = e;
     }
-    inc_ptr[l + 1] = (int)d.inc_pose.size();
+    d.inc_ptr[l + 1] = (int)d.inc_pose.size();
   }
   if (kind == 2 && order == 1) {
     d.order = 1;
-    if (!build_nd(c, d, err, inc_ptr)) { d = DirectTables(); return false; }
+    if (!build_nd(c, d, err)) { d = DirectTables(); return false; }
     return true;
   }
   std::vector<int> bslot(M, -1);
   if (kind == 1) {
     d.nbp = d.nb = std::max(1, (6 * N + 47) / 48);
     d.first.assign(d.nb, 0);
-  } else {
-    // border the k planes of widest observer span (pose order; ties: lower index), k = 0 .. min(M, 64), whichever k takes
-    // the fewest device bytes (ties: the smaller k)
-    std::vector<int> span(M, 0), order(M);
-    for (int l = 0; l < M; l++) {
-      if (inc_ptr[l + 1] > inc_ptr[l]) span[l] = d.inc_pose[inc_ptr[l + 1] - 1] - d.inc_pose[inc_ptr[l]];
-      order[l] = l;
-    }
-    std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return span[x] > span[y]; });
-    long long best = -1;
-    int best_k = 0;
-    std::vector<int> fk, bs(M, -1);
-    for (int k = 0; k <= std::min(M, kBandMaxBorder); k++) {
-      std::fill(bs.begin(), bs.end(), -1);
-      std::vector<int> chosen(order.begin(), order.begin() + k);
-      std::sort(chosen.begin(), chosen.end());
-      for (int q = 0; q < k; q++) bs[chosen[q]] = q;
+  } else {   // bordering ranks the planes by observer span (pose order)
+    std::vector<int> span(M, 0);
+    for (int l = 0; l < M; l++)
+      if (d.inc_ptr[l + 1] > d.inc_ptr[l]) span[l] = d.inc_pose[d.inc_ptr[l + 1] - 1] - d.inc_pose[d.inc_ptr[l]];
+    choose_border(span, [&](const std::vector<int>& bs, int k) {
+      std::vector<int> fk;
       int nbp = 0, nb = 0;
-      const long long bytes = band_envelope(c, inc_ptr, d.inc_pose, bs, k, fk, nbp, nb);
-      if (best < 0 || bytes < best) { best = bytes; best_k = k; }
-    }
-    d.border.assign(order.begin(), order.begin() + best_k);
-    std::sort(d.border.begin(), d.border.end());
-    for (int q = 0; q < best_k; q++) bslot[d.border[q]] = q;
-    d.bytes = band_envelope(c, inc_ptr, d.inc_pose, bslot, best_k, d.first, d.nbp, d.nb);
+      return band_envelope(c, d.inc_ptr, d.inc_pose, bs, k, fk, nbp, nb);
+    }, d.border, bslot);
+    const int nbord = (int)d.border.size();
+    d.bytes = band_envelope(c, d.inc_ptr, d.inc_pose, bslot, nbord, d.first, d.nbp, d.nb);
     if (d.bytes > kBandBudgetBytes) {
       err = "band linear solver: the graph needs " + std::to_string(d.bytes) + " bytes of device memory (" +
-            std::to_string(N) + " poses, " + std::to_string(best_k) + " bordered planes); the budget is " +
+            std::to_string(N) + " poses, " + std::to_string(nbord) + " bordered planes); the budget is " +
             std::to_string(kBandBudgetBytes) + " bytes (use the PCG solver, kind 0)";
       d = DirectTables();
       return false;
     }
-    for (int q = 0; q < best_k; q++) { d.binc.push_back(inc_ptr[d.border[q]]); d.binc.push_back(inc_ptr[d.border[q] + 1]); }
+    for (int l : d.border) { d.binc.push_back(d.inc_ptr[l]); d.binc.push_back(d.inc_ptr[l + 1]); }
   }
   const int nb = d.nb;
   d.toff.assign(nb + 1, 0);
@@ -1116,46 +1116,7 @@ inline bool build_direct(const Compiled& c, DirectTables& d, std::string& err, i
   }
   d.poff.assign(N + 1, 0);
   for (int a = 0; a < N; a++) d.poff[a + 1] = d.poff[a] + a - 8 * d.first[a / 8] + 1;
-  const size_t np = (size_t)d.poff[N];
-  auto pair = [&](int a, int b) { return (size_t)d.poff[a] + b - 8 * d.first[a / 8]; };
-  d.lp_ptr.assign(np + 1, 0);
-  for (int pass = 0; pass < 2; pass++) {
-    std::vector<int> fill;
-    if (pass == 1) {
-      for (size_t q = 0; q < np; q++) d.lp_ptr[q + 1] += d.lp_ptr[q];
-      d.lp_a.assign(std::max(1, d.lp_ptr[np]), 0);
-      d.lp_b.assign(std::max(1, d.lp_ptr[np]), 0);
-      fill.assign(d.lp_ptr.begin(), d.lp_ptr.end() - 1);
-    }
-    for (int l = 0; l < M; l++) {   // incidences are pose-ascending inside a plane: i >= j gives a >= b
-      if (bslot[l] >= 0) continue;
-      for (int i = inc_ptr[l]; i < inc_ptr[l + 1]; i++)
-        for (int j = inc_ptr[l]; j <= i; j++) {
-          const size_t q = pair(d.inc_pose[i], d.inc_pose[j]);
-          if (pass == 0) d.lp_ptr[q + 1]++;
-          else { const int at = fill[q]++; d.lp_a[at] = i; d.lp_b[at] = j; }
-        }
-    }
-  }
-  d.fp_ptr.assign(np + 1, 0);
-  for (int pass = 0; pass < 2; pass++) {
-    std::vector<int> fill;
-    if (pass == 1) {
-      for (size_t q = 0; q < np; q++) d.fp_ptr[q + 1] += d.fp_ptr[q];
-      d.fp_f.assign(std::max(1, d.fp_ptr[np]), 0);
-      fill.assign(d.fp_ptr.begin(), d.fp_ptr.end() - 1);
-    }
-    for (int f = 0; f < c.Epf; f++) {
-      if (c.pf_j[f] < 0) continue;
-      for (int side = 0; side < 2; side++) {
-        const int a = side ? c.pf_j[f] : c.pf_i[f], b = side ? c.pf_i[f] : c.pf_j[f];
-        if (a < b) continue;
-        const size_t q = pair(a, b);
-        if (pass == 0) d.fp_ptr[q + 1]++;
-        else d.fp_f[fill[q]++] = f * 2 + side;
-      }
-    }
-  }
+  pair_lists(c, bslot, (size_t)d.poff[N], [&](int a, int b) { return (size_t)d.poff[a] + b - 8 * d.first[a / 8]; }, d);
   return true;
 }
 
@@ -1176,7 +1137,6 @@ struct CovTables {
   uint64_t topo = 0;                  // layout version the tables were built for (0: none)
   std::vector<int> sel_ptr, sel;      // per stored tile (i, j), i > j: (Sigma tile (i,k) or (k,i)) * 2 + transposed, L tile (k, j),
                                       // k in R_j ascending (empty for diagonal tiles)
-  std::vector<int> inc_ptr;           // per plane: its incidences [inc_ptr[l], inc_ptr[l + 1]) (plane-major, pose-ascending)
   std::vector<int> pair_ptr, pair;    // per eliminated plane: its observer pairs (incidences qa >= qb), 4 ints each: qa, qb,
                                       // Sigma tile, in-tile offset * 2 + transposed (the block Sigma_{pose qa, pose qb})
   std::vector<int> dev;               // the tables above that the device reads, packed (CovTable)
@@ -1189,12 +1149,8 @@ struct CovTables {
 // tile * kAcTile + (flag ? off + s * ld + p : off + p * ld + s) with ld = 52.  False when the tile is not stored.
 inline bool cov_block_at(const DirectTables& d, int r0, int c0, int& tile, int& off, int& flag) {
   const int ti = d.nd_pos[r0 / 48], tj = d.nd_pos[c0 / 48], er = r0 % 48, ec = c0 % 48;
-  const int hi = std::max(ti, tj), lo = std::min(ti, tj);
-  const int* b = d.nd_crow.data() + d.nd_cptr[lo];
-  const int n = d.nd_cptr[lo + 1] - d.nd_cptr[lo];
-  const int p = (int)(std::lower_bound(b, b + n, hi) - b);
-  if (p == n || b[p] != hi) return false;
-  tile = d.nd_toff[lo] + p;
+  tile = d.tile(std::max(ti, tj), std::min(ti, tj));
+  if (tile < 0) return false;
   flag = ti < tj ? 1 : 0;
   off = flag ? ec * 52 + er : er * 52 + ec;
   return true;
@@ -1217,14 +1173,11 @@ inline bool build_cov(const Compiled& c, const DirectTables& d, CovTables& cv, s
   const int nb = d.nb, T = d.nd_cptr[nb], M = c.M;
   cv.nsel = 0;
   for (int j = 0; j < nb; j++) { const long long m = d.nd_cptr[j + 1] - d.nd_cptr[j] - 1; cv.nsel += m * m; }
-  cv.inc_ptr.assign(M + 1, 0);
-  for (int q = 0; q < (int)d.inc_plane.size(); q++) cv.inc_ptr[d.inc_plane[q] + 1]++;
-  for (int l = 0; l < M; l++) cv.inc_ptr[l + 1] += cv.inc_ptr[l];
   std::vector<char> bord(M, 0);
   for (int l : d.border) bord[l] = 1;
   long long npair = 0;
   for (int l = 0; l < M; l++)
-    if (!bord[l]) { const long long n = cv.inc_ptr[l + 1] - cv.inc_ptr[l]; npair += n * (n + 1) / 2; }
+    if (!bord[l]) { const long long n = d.inc_ptr[l + 1] - d.inc_ptr[l]; npair += n * (n + 1) / 2; }
   cv.bytes = (long long)T * kDirectTileBytes + kCovSelBytes * cv.nsel + 4ll * (T + 1) + 16 * npair + 4ll * (M + 1) + 4 * COV_HDR;
   if (d.bytes + cv.bytes > kBandBudgetBytes) {
     err = "marginal covariances: the graph needs " + std::to_string(d.bytes + cv.bytes) + " bytes of device memory (" +
@@ -1235,16 +1188,12 @@ inline bool build_cov(const Compiled& c, const DirectTables& d, CovTables& cv, s
   }
   cv.sel_ptr.assign(T + 1, 0);
   cv.sel.reserve(2 * cv.nsel);
-  auto stored = [&](int i, int j) {   // storage index of tile (i, j), i >= j, inside the pattern
-    const int* b = d.nd_crow.data();
-    return d.nd_toff[j] + (int)(std::lower_bound(b + d.nd_cptr[j], b + d.nd_cptr[j + 1], i) - (b + d.nd_cptr[j]));
-  };
   for (int t = 0; t < T; t++) {   // storage order
     const int i = d.nd_trow[t], j = d.nd_tcol[t];
     if (i != j) {
       for (int p = d.nd_cptr[j] + 1; p < d.nd_cptr[j + 1]; p++) {
         const int k = d.nd_crow[p];
-        cv.sel.push_back(2 * stored(std::max(i, k), std::min(i, k)) + (i < k ? 1 : 0));
+        cv.sel.push_back(2 * d.tile(std::max(i, k), std::min(i, k)) + (i < k ? 1 : 0));
         cv.sel.push_back(d.nd_toff[j] + p - d.nd_cptr[j]);
       }
     }
@@ -1253,8 +1202,8 @@ inline bool build_cov(const Compiled& c, const DirectTables& d, CovTables& cv, s
   cv.pair_ptr.assign(M + 1, 0);
   for (int l = 0; l < M; l++) {
     if (!bord[l])
-      for (int qa = cv.inc_ptr[l]; qa < cv.inc_ptr[l + 1]; qa++)
-        for (int qb = cv.inc_ptr[l]; qb <= qa; qb++) {
+      for (int qa = d.inc_ptr[l]; qa < d.inc_ptr[l + 1]; qa++)
+        for (int qb = d.inc_ptr[l]; qb <= qa; qb++) {
           int tile = 0, off = 0, flag = 0;
           if (!cov_block_at(d, 6 * d.inc_pose[qa], 6 * d.inc_pose[qb], tile, off, flag)) {   // (eliminating l coupled them)
             err = "marginal covariances: internal error: an observer pair of an eliminated plane lies outside L's pattern";

@@ -1001,6 +1001,30 @@ __device__ __forceinline__ void mma48(double (&acc)[3][2], const double* A, cons
     }
   }
 }
+// accumulator s of mma48 holds row r, columns cc and cc + 1 of the tile; false when the warp has no s-th output tile
+__device__ __forceinline__ bool mma48_frag(int s, int& r, int& cc) {
+  const int lane = threadIdx.x & 31, q = (threadIdx.x >> 5) + 16 * s;
+  r = 8 * (q / 6) + (lane >> 2);
+  cc = 8 * (q % 6) + 2 * (lane & 3);
+  return q < 36;
+}
+// dst (row stride kAcLd) <- sg acc, each accumulator at its place in the tile
+__device__ __forceinline__ void mma48_store(double* dst, const double (&acc)[3][2], double sg = 1.0) {
+  int r, cc;
+#pragma unroll
+  for (int s = 0; s < 3; s++)
+    if (mma48_frag(s, r, cc)) *reinterpret_cast<double2*>(dst + r * kAcLd + cc) = make_double2(sg * acc[s][0], sg * acc[s][1]);
+}
+// acc <- the tile src (row stride kAcLd, read through L2), each accumulator from its place in the tile
+__device__ __forceinline__ void mma48_load(double (&acc)[3][2], const double* src) {
+  int r, cc;
+#pragma unroll
+  for (int s = 0; s < 3; s++)
+    if (mma48_frag(s, r, cc)) {
+      const double2 v = __ldcg(reinterpret_cast<const double2*>(src + r * kAcLd + cc));
+      acc[s][0] = v.x; acc[s][1] = v.y;
+    }
+}
 
 // Pose3d_Plane3d_Factor2 edges are rare (disabled in the shipped demo): keep their extra arithmetic out of the
 // register allocation of the common path
@@ -3088,8 +3112,7 @@ struct Phase {
   // a bordered plane's rows hold W_al^T against its observers and its damped Hll block on the diagonal (0 against the other
   // bordered planes).  Upper halves of diagonal tiles are 0, the padding is identity.  The first tile of each row also goes
   // to the pivot-column snapshot of the step that first reads it (step first[i], parity first[i] & 1).
-  // Entry (i, j), i >= j, of S in the bordered order, as direct_assemble forms it; q(a, b) is the index of the pose pair's lists.
-  // (The insertion-order assembly keeps its own copy of this formula inline, so that its kernel compiles as before.)
+  // Entry (i, j), i >= j, of S in the bordered order; pair(a, b) is the index of the pose pair's lists.
   template <typename Pair>
   __device__ __forceinline__ static double direct_entry(int i, int j, double lambda, Pair pair) {
     const int n6 = 6 * G.N, np6 = 48 * G.dnbp;
@@ -3137,7 +3160,7 @@ struct Phase {
 
   __device__ void direct_assemble(double lambda) {
     if (G.dnd) { nd_assemble(lambda); return; }
-    const int nb = G.dnb, n6 = 6 * G.N, np6 = 48 * G.dnbp;
+    const int nb = G.dnb;
     const long long total = (long long)ldc(G.dtoff + nb) * 2304;
     int tprev = -1, ti = 0, tj = 0, f0 = 0;
     for (long long idx = tid_team(); idx < total; idx += nthr_team()) {
@@ -3154,60 +3177,20 @@ struct Phase {
         tprev = t;
       }
       const int i = 48 * ti + er, j = 48 * tj + ec;
-      double v = 0.0;
-      if (j > i) {
-        v = 0.0;
-      } else if (i >= np6) {   // a bordered plane's row
-        const int k = i - np6, kb = k / 3, m = k - kb * 3;
-        if (k >= 3 * G.dnbord) {
-          v = (i == j) ? 1.0 : 0.0;
-        } else if (j >= np6) {
-          if ((j - np6) / 3 == kb) {
-            const int cc = j - np6 - kb * 3;
-            v = ldc(G.Hll + (size_t)ldc(G.dbord + kb) * 9 + m * 3 + cc);
-            if (m == cc) v *= (1 + lambda);   // Cholesky.cpp:91-97
-          }
-        } else if (j < n6) {   // W_al of the incidence (pose b, plane): incidences are pose-ascending inside a plane
-          const int b = j / 6, r = j - b * 6;
-          int lo = ldc(G.dbinc + 2 * kb), hi = ldc(G.dbinc + 2 * kb + 1);
-          while (lo < hi) {
-            const int mid = (lo + hi) >> 1;
-            if (ldc(G.pl_pose + ldc(G.dinc_lo + mid)) < b) lo = mid + 1; else hi = mid;
-          }
-          if (lo < ldc(G.dbinc + 2 * kb + 1) && ldc(G.pl_pose + ldc(G.dinc_lo + lo)) == b) v = ldc(G.Wd + (size_t)lo * 18 + r * 3 + m);
-        }
-      } else if (i >= n6) {
-        v = (i == j) ? 1.0 : 0.0;
-      } else {
-        const int a = i / 6, r = i - a * 6, b = j / 6, cc = j - b * 6;
-        if (a == b) {
-          v = ldc(G.Hpp + (size_t)a * 36 + r * 6 + cc);
-          if (r == cc) v *= (1 + lambda);   // Cholesky.cpp:91-97
-        }
-        const size_t q = dpair(a, b);
-        for (int k = G.dfp_ptr[q]; k < G.dfp_ptr[q + 1]; k++) {
-          const int fs = G.dfp_f[k], f = fs >> 1;
-          v += (fs & 1) ? ldc(G.PF + (size_t)f * 120 + 72 + cc * 6 + r) : ldc(G.PF + (size_t)f * 120 + 72 + r * 6 + cc);
-        }
-        for (int k = G.dlp_ptr[q]; k < G.dlp_ptr[q + 1]; k++) {
-          const double* y = G.Yd + (size_t)G.dlp_a[k] * 18 + r * 3;
-          const double* w = G.Wd + (size_t)G.dlp_b[k] * 18 + cc * 3;
-          v -= ldc(y) * ldc(w) + ldc(y + 1) * ldc(w + 1) + ldc(y + 2) * ldc(w + 2);
-        }
-      }
+      const double v = j > i ? 0.0 : direct_entry(i, j, lambda, dpair);
       tile_at(G.Sd, t)[er * kAcLd + ec] = v;
       if (tj == f0) tile_at(G.Dsnap + (size_t)(tj & 1) * nb * kAcTile, ti)[er * kAcLd + ec] = v;
     }
   }
 
   // band layout: b = [-gp + sum over the eliminated planes of Y_al g_l ; -g_l of the bordered planes].  The list of the pair
-  // (a, a) holds exactly one record (q, q) per eliminated incidence q of pose a, plane-ascending.  (The dense solve forms b in
-  // pose_phase, with every plane eliminated.)
+  // (a, a) holds exactly one record (q, q) per eliminated incidence q of pose a, plane-ascending; in the ND layout that pair
+  // lies in the diagonal tile of a's tile.  (The dense solve forms b in pose_phase, with every plane eliminated.)
   __device__ void direct_rhs() {
-    if (G.dnd) { nd_rhs(); return; }
     const int n6 = 6 * G.N;
     for (int i = tid_team(); i < n6; i += nthr_team()) {
-      const int a = i / 6, r = i - a * 6, q = dpair(a, a);
+      const int a = i / 6, r = i - a * 6;
+      const size_t q = G.dnd ? (size_t)64 * ldc(nd(ND_TOFF) + ldc(nd(ND_POS) + a / 8)) + 9 * (a & 7) : (size_t)dpair(a, a);
       double v = -ldc(G.gp + i);
       for (int k = G.dlp_ptr[q]; k < G.dlp_ptr[q + 1]; k++) {
         const int inc = G.dlp_a[k];
@@ -3259,6 +3242,12 @@ struct Phase {
     return ok;
   }
 
+  // entry i of b in the padded bordered order (6 N pose entries, then 3 per bordered plane from row 48 nbp; 0 in the padding)
+  __device__ __forceinline__ static double padded_b(int i) {
+    const int n6 = 6 * G.N, np6 = 48 * G.dnbp;
+    return (i < n6) ? ldc(G.b + i) : ((i >= np6 && i < np6 + 3 * G.dnbord) ? ldc(G.b + n6 + i - np6) : 0.0);
+  }
+
   __device__ void load_tile(double* dst, const double* src) {
     for (int e = threadIdx.x; e < 48 * 48; e += kThreads) dst[(e / 48) * kAcLd + e % 48] = ldc(src + (e / 48) * kAcLd + e % 48);
   }
@@ -3280,45 +3269,27 @@ struct Phase {
   // K+1), factors it and publishes L_{K+1}^-1; step 0's pivot is factored by every CTA from the snapshot.
   __device__ void direct_factor() {
     if (G.dnd) { nd_factor(); return; }
-    const int nb = G.dnb, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3;
+    const int nb = G.dnb, tid = threadIdx.x;
     double* Li = reinterpret_cast<double*>(g_smem + kSmWork);
     double* Ci = Li + kAcTile;
     double* Ti = Ci + kAcTile;
     double* Cj = Ti + kAcTile;
     double* Md = Cj + kAcTile;
     const int T = c.tsize;
-    auto frag = [&](int s, int& r, int& cc) {
-      const int q = warp + 16 * s;
-      r = 8 * (q / 6) + fr;
-      cc = 8 * (q % 6) + 2 * fc;
-      return q < 36;
-    };
     auto form_T = [&]() {   // Ti = -L_iK = -(Ci Li^T)
       double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
       mma48<true>(acc, Ci, Li);
-      int r, cc;
-#pragma unroll
-      for (int s = 0; s < 3; s++)
-        if (frag(s, r, cc)) *reinterpret_cast<double2*>(Ti + r * kAcLd + cc) = make_double2(-acc[s][0], -acc[s][1]);
+      mma48_store(Ti, acc, -1.0);
     };
     auto update = [&](int i, int j, double (&acc)[3][2]) {   // Cj (loaded) <- L_jK = Cj Li^T, then acc = A_ij + Ti L_jK^T
-      int r, cc;
       {
         double l[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
         mma48<true>(l, Cj, Li);
         __syncthreads();
-#pragma unroll
-        for (int s = 0; s < 3; s++)
-          if (frag(s, r, cc)) *reinterpret_cast<double2*>(Cj + r * kAcLd + cc) = make_double2(l[s][0], l[s][1]);
+        mma48_store(Cj, l);
         __syncthreads();
       }
-      const double* tile = tile_at(G.Sd, dtile(i, j));
-#pragma unroll
-      for (int s = 0; s < 3; s++)
-        if (frag(s, r, cc)) {
-          const double2 v = __ldcg(reinterpret_cast<const double2*>(tile + r * kAcLd + cc));
-          acc[s][0] = v.x; acc[s][1] = v.y;
-        }
+      mma48_load(acc, tile_at(G.Sd, dtile(i, j)));
       mma48<true>(acc, Ti, Cj);
     };
     auto factor_pivot = [&](int d, bool publish) {   // Md holds A_dd: L_dd into the store, L_dd^-1 out
@@ -3352,10 +3323,7 @@ struct Phase {
           __syncthreads();
           double acc[3][2];
           update(d, d, acc);
-          int r, cc;
-#pragma unroll
-          for (int s = 0; s < 3; s++)
-            if (frag(s, r, cc)) *reinterpret_cast<double2*>(Md + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+          mma48_store(Md, acc);
         } else {   // row d starts at column d: its pivot is the assembled tile
           load_tile(Md, tile_at(G.Sd, dtile(d, d)));
         }
@@ -3391,25 +3359,17 @@ struct Phase {
             trowT = i;
           }
           double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
-          int r, cc;
           if (j == K) {   // panel: L_iK = C_i L_KK^-T
             mma48<true>(acc, Ci, Li);
-#pragma unroll
-            for (int s = 0; s < 3; s++)
-              if (frag(s, r, cc))
-                *reinterpret_cast<double2*>(tile_at(G.Sd, t0) + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+            mma48_store(tile_at(G.Sd, t0), acc);
             continue;
           }
           __syncthreads();
           load_tile(Cj, tile_at(snap, j));
           __syncthreads();
           update(i, j, acc);
-#pragma unroll
-          for (int s = 0; s < 3; s++) {
-            if (!frag(s, r, cc)) continue;
-            *reinterpret_cast<double2*>(tile_at(G.Sd, dtile(i, j)) + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
-            if (j == d) *reinterpret_cast<double2*>(tile_at(snapn, i) + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
-          }
+          mma48_store(tile_at(G.Sd, dtile(i, j)), acc);
+          if (j == d) mma48_store(tile_at(snapn, i), acc);
         }
       }
       __syncthreads();
@@ -3424,12 +3384,11 @@ struct Phase {
   // then 3 per bordered plane.
   __device__ void direct_trsv() {
     if (G.dnd) { nd_trsv(); return; }
-    const int nb = G.dnb, n = 48 * nb, n6 = 6 * G.N, np6 = 48 * G.dnbp, tid = threadIdx.x;
+    const int nb = G.dnb, n = 48 * nb, tid = threadIdx.x;
     double* rv = G.dvec;
     double* yv = G.dvec + n;
     double* sv = reinterpret_cast<double*>(g_smem + kSmWork);   // [48] the vector piece of this step, [48] its product
-    for (int i = tid_team(); i < n; i += nthr_team())
-      rv[i] = (i < n6) ? ldc(G.b + i) : ((i >= np6 && i < np6 + 3 * G.dnbord) ? ldc(G.b + n6 + i - np6) : 0.0);
+    for (int i = tid_team(); i < n; i += nthr_team()) rv[i] = padded_b(i);
     team_barrier(c);
     for (int K = 0; K < nb; K++) {   // forward: y_K = L_KK^-1 r_K;  r_J -= L_JK y_K  (J > K)
       const double* Li = tile_at(G.Dinv, K);
@@ -3493,24 +3452,6 @@ struct Phase {
     }
   }
 
-  // the right-hand side of direct_rhs in the ND layout: the pair (a, a) of pose a lies in the diagonal tile of its tile
-  __device__ __noinline__ void nd_rhs() {
-    const int n6 = 6 * G.N;
-    for (int i = tid_team(); i < n6; i += nthr_team()) {
-      const int a = i / 6, r = i - a * 6;
-      const size_t q = (size_t)64 * ldc(nd(ND_TOFF) + ldc(nd(ND_POS) + a / 8)) + 9 * (a & 7);
-      double v = -ldc(G.gp + i);
-      for (int k = G.dlp_ptr[q]; k < G.dlp_ptr[q + 1]; k++) {
-        const int inc = G.dlp_a[k];
-        const double* y = G.Yd + (size_t)inc * 18 + r * 3;
-        const double* g = G.gl + (size_t)G.dinc_plane[inc] * 3;
-        v += ldc(y) * ldc(g) + ldc(y + 1) * ldc(g + 1) + ldc(y + 2) * ldc(g + 2);
-      }
-      G.b[i] = v;
-    }
-    for (int k = tid_team(); k < 3 * G.dnbord; k += nthr_team()) G.b[n6 + k] = -ldc(G.gl + (size_t)ldc(G.dbord + k / 3) * 3 + k % 3);
-  }
-
   // S = L L^T in place, left-looking, level by level of the elimination tree (a column's children lie on lower levels, so
   // every L_iK it reads is final).  Stored tile t belongs to CTA (t - first tile of its level) % tsize.  Per level:
   //   (a) C_ij = A_ij - sum_K L_iK L_jK^T over the tile's update list, in list order, on the FP64 tensor cores; the owner of a
@@ -3518,28 +3459,16 @@ struct Phase {
   //   (b) panels L_ij = C_ij L_jj^-T;                                        team barrier
   // Each product reads two final L tiles, so every CTA that forms a tile gets the same bits.
   __device__ __noinline__ void nd_factor() {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3, T = c.tsize;
+    const int tid = threadIdx.x, T = c.tsize;
     double* Li = reinterpret_cast<double*>(g_smem + kSmWork);
     double* Xa = Li + kAcTile;
     double* Xb = Xa + kAcTile;
-    auto frag = [&](int s, int& r, int& cc) {
-      const int q = warp + 16 * s;
-      r = 8 * (q / 6) + fr;
-      cc = 8 * (q % 6) + 2 * fc;
-      return q < 36;
-    };
     for (int l = 0; l < ldc(G.dnd); l++) {
       const int t0 = ldc(nd(ND_LTPTR) + l), t1 = ldc(nd(ND_LTPTR) + l + 1);
       for (int t = t0 + c.rank; t < t1; t += T) {
         double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
         double* tile = tile_at(G.Sd, t);
-        int r, cc;
-#pragma unroll
-        for (int s = 0; s < 3; s++)
-          if (frag(s, r, cc)) {
-            const double2 v = __ldcg(reinterpret_cast<const double2*>(tile + r * kAcLd + cc));
-            acc[s][0] = v.x; acc[s][1] = v.y;
-          }
+        mma48_load(acc, tile);
         for (int u = ldc(nd(ND_UPTR) + t); u < ldc(nd(ND_UPTR) + t + 1); u++) {
           const double* A = tile_at(G.Sd, ldc(nd(ND_UPD) + 2 * u));
           const double* B = tile_at(G.Sd, ldc(nd(ND_UPD) + 2 * u + 1));
@@ -3555,17 +3484,13 @@ struct Phase {
         const int j = ldc(nd(ND_TCOL) + t);
         if (ldc(nd(ND_TROW) + t) == j) {   // diagonal: factor it, publish L_jj and L_jj^-1
           __syncthreads();
-#pragma unroll
-          for (int s = 0; s < 3; s++)
-            if (frag(s, r, cc)) *reinterpret_cast<double2*>(Xa + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+          mma48_store(Xa, acc);
           const bool ok = chol48(Xa, Li);
           if (!ok && tid == 0) *G.dflag = 1u;
           store_tile(tile, Xa);
           store_tile(tile_at(G.Dinv, j), Li);
         } else {
-#pragma unroll
-          for (int s = 0; s < 3; s++)
-            if (frag(s, r, cc)) *reinterpret_cast<double2*>(tile + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+          mma48_store(tile, acc);
         }
       }
       __syncthreads();
@@ -3580,10 +3505,7 @@ struct Phase {
         __syncthreads();
         double acc[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
         mma48<true>(acc, Xa, Li);
-        int r, cc;
-#pragma unroll
-        for (int s = 0; s < 3; s++)
-          if (frag(s, r, cc)) *reinterpret_cast<double2*>(tile + r * kAcLd + cc) = make_double2(acc[s][0], acc[s][1]);
+        mma48_store(tile, acc);
       }
       __syncthreads();
       team_barrier(c);
@@ -3596,13 +3518,11 @@ struct Phase {
   // scattered back, so dvec[0] ends as in the envelope layout.
   __device__ __noinline__ void nd_trsv() {
     constexpr int kGroups = kThreads / 48;
-    const int nb = G.dnb, n = 48 * nb, n6 = 6 * G.N, np6 = 48 * G.dnbp, tid = threadIdx.x, g = tid / 48, r = tid - 48 * g;
+    const int nb = G.dnb, n = 48 * nb, tid = threadIdx.x, g = tid / 48, r = tid - 48 * g;
     double* rv = G.dvec;
     double* yv = G.dvec + n;   // the vector in the new order: b, then y, then x, in place
     double* sv = reinterpret_cast<double*>(g_smem + kSmWork) + 48 * g;
-    for (int i = tid_team(); i < n; i += nthr_team())
-      yv[48 * ldc(nd(ND_POS) + i / 48) + i % 48] =
-          (i < n6) ? ldc(G.b + i) : ((i >= np6 && i < np6 + 3 * G.dnbord) ? ldc(G.b + n6 + i - np6) : 0.0);
+    for (int i = tid_team(); i < n; i += nthr_team()) yv[48 * ldc(nd(ND_POS) + i / 48) + i % 48] = padded_b(i);
     team_barrier(c);
     for (int l = 0; l < ldc(G.dnd); l++) {   // forward: y_j = L_jj^-1 (b_j - sum_K L_jK y_K)
       const int k1 = ldc(nd(ND_LPTR) + l + 1);
@@ -3672,26 +3592,14 @@ struct Phase {
   // tile instead of one per entry, and no staging buffer.  Every product reads final tiles in a fixed order, so every CTA
   // that forms a tile gets the same bits.  L stays as it is (the column solves read it).
   __device__ __noinline__ void nd_selinv() {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3, T = c.tsize;
+    const int tid = threadIdx.x, T = c.tsize;
     double* Xa = reinterpret_cast<double*>(g_smem + kSmWork);
     double* Xb = Xa + kAcTile;
-    auto frag = [&](int s, int& r, int& cc) {
-      const int q = warp + 16 * s;
-      r = 8 * (q / 6) + fr;
-      cc = 8 * (q % 6) + 2 * fc;
-      return q < 36;
-    };
     auto load = [&](double* dst, const double* src, bool tr) {   // dst = src or src^T
       for (int e = tid; e < 48 * 48; e += kThreads) {
         const int r = e / 48, cc = e - r * 48;
         dst[r * kAcLd + cc] = ldc(src + (tr ? cc * kAcLd + r : r * kAcLd + cc));
       }
-    };
-    auto put = [&](double* dst, const double (&acc)[3][2], double sg) {
-      int r, cc;
-#pragma unroll
-      for (int s = 0; s < 3; s++)
-        if (frag(s, r, cc)) *reinterpret_cast<double2*>(dst + r * kAcLd + cc) = make_double2(sg * acc[s][0], sg * acc[s][1]);
     };
     for (int l = ldc(G.dnd) - 1; l >= 0; l--) {
       const int t0 = ldc(nd(ND_LTPTR) + l), t1 = ldc(nd(ND_LTPTR) + l + 1);
@@ -3708,12 +3616,12 @@ struct Phase {
           mma48<false>(acc, Xa, Xb);
         }
         __syncthreads();
-        put(Xa, acc, -1.0);
+        mma48_store(Xa, acc, -1.0);
         load(Xb, tile_at(G.Dinv, j), false);
         __syncthreads();
         double out[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
         mma48<false>(out, Xa, Xb);
-        put(tile_at(G.Sig, t), out, 1.0);
+        mma48_store(tile_at(G.Sig, t), out);
       }
       __syncthreads();
       team_barrier(c);
@@ -3737,13 +3645,13 @@ struct Phase {
           int r, cc;
 #pragma unroll
           for (int s = 0; s < 3; s++)
-            if (frag(s, r, cc)) { Xb[r * kAcLd + cc] -= acc[s][0]; Xb[r * kAcLd + cc + 1] -= acc[s][1]; }
+            if (mma48_frag(s, r, cc)) { Xb[r * kAcLd + cc] -= acc[s][0]; Xb[r * kAcLd + cc + 1] -= acc[s][1]; }
         }
         __syncthreads();
         double out[3][2] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
         mma48<false>(out, Xa, Xb);
         __syncthreads();
-        put(Xa, out, 1.0);
+        mma48_store(Xa, out);
         __syncthreads();
         double* dst = tile_at(G.Sig, t);
         for (int e = tid; e < 48 * 48; e += kThreads) {

@@ -8,6 +8,10 @@
 // are the running node count), so that generated or dataset graphs can be hashed too:
 //   pose - | pose x y z qw qx qy qz          plane - | plane a b c d
 //   prior <pose> m[6] sinf[21]   odo <pose> <pose> m[6] sinf[21]   pp <pose> <plane> m[4] sinf[6]   lprior <plane> m[4] sinf[6]
+// With `--direct <kind> <order>` in front of either form it hashes the direct solve's host tables instead: build_direct, and
+// build_cov for order 1 (or the refusal text of a layout that is refused), so that a refactor of the direct layouts can be
+// checked the same way:
+//   /tmp/h_old --direct 2 1 2000 12 3;  /tmp/h_new --direct 2 1 --file graph.txt
 #include <chrono>
 #include <cstdio>
 #include <cstdint>
@@ -45,6 +49,32 @@ static uint64_t image_hash(const Compiled& c) {
   hash_overflow(c, 0);
   return H;
 }
+// the per-plane incidence pointer of a covariance layout: a CovTables member in older headers, a DirectTables one since
+template <typename C, typename D> auto inc_ptr_of(const C& cv, const D&, int) -> decltype((cv.inc_ptr)) { return cv.inc_ptr; }
+template <typename C, typename D> auto inc_ptr_of(const C&, const D& d, long) -> decltype((d.inc_ptr)) { return d.inc_ptr; }
+static void hll(long long x) { hi((int)(x & 0xffffffff)); hi((int)(x >> 32)); }
+// FNV hash of every DirectTables (and, for order 1, CovTables) member; the refusal text instead when a layout is refused
+static std::string direct_hash(const Compiled& c, int kind, int order) {
+  DirectTables d; CovTables cv; std::string err;
+  if (!build_direct(c, d, err, kind, order)) return "refused: " + err;
+  H = 1469598103934665603ull;
+  for (int x : {d.nb, d.nbp, d.order, d.nlev}) hi(x);
+  hll(d.bytes); hll(d.nupd);
+  hv(d.inc_pose); hv(d.inc_plane); hv(d.inc_lo); hv(d.inc_hi); hv(d.lp_ptr); hv(d.lp_a); hv(d.lp_b); hv(d.fp_ptr); hv(d.fp_f);
+  hv(d.first); hv(d.toff); hv(d.poff); hv(d.col_ptr); hv(d.col_row); hv(d.border); hv(d.binc);
+  hv(d.nd_perm); hv(d.nd_pos); hv(d.nd_parent); hv(d.nd_level); hv(d.nd_cptr); hv(d.nd_crow); hv(d.nd_toff); hv(d.nd_lptr);
+  hv(d.nd_lcol); hv(d.nd_ltptr); hv(d.nd_trow); hv(d.nd_tcol); hv(d.nd_uptr); hv(d.nd_upd); hv(d.nd_rptr); hv(d.nd_rtile); hv(d.nd_dev);
+  char buf[64];
+  snprintf(buf, sizeof(buf), "tables=%016llx", (unsigned long long)H);
+  std::string out = buf;
+  if (order != 1) return out;
+  if (!build_cov(c, d, cv, err)) return out + " cov refused: " + err;
+  H = 1469598103934665603ull;
+  hll((long long)cv.topo); hll(cv.nsel); hll(cv.bytes);
+  hv(cv.sel_ptr); hv(cv.sel); hv(inc_ptr_of(cv, d, 0)); hv(cv.pair_ptr); hv(cv.pair); hv(cv.dev);
+  snprintf(buf, sizeof(buf), " cov=%016llx", (unsigned long long)H);
+  return out + buf;
+}
 static bool read_graph(const char* path, Graph& g) {
   std::ifstream in(path);
   std::string line, op;
@@ -72,6 +102,11 @@ static bool read_graph(const char* path, Graph& g) {
 }
 
 int main(int argc, char** argv) {
+  int dkind = -1, dorder = 0;
+  if (argc > 3 && !strcmp(argv[1], "--direct")) {
+    dkind = atoi(argv[2]); dorder = atoi(argv[3]);
+    argv += 3; argc -= 3;
+  }
   if (argc > 2 && !strcmp(argv[1], "--file")) {
     Graph g;
     if (!read_graph(argv[2], g)) { printf("ok=0 cannot read %s: %s\n", argv[2], g.err.c_str()); return 1; }
@@ -80,6 +115,10 @@ int main(int argc, char** argv) {
     bool ok = compile_graph(g, c, err);
     const uint64_t h1 = ok ? image_hash(c) : 0;
     ok = compile_graph(g, c, err) && ok && image_hash(c) == h1;
+    if (ok && dkind >= 0) {
+      printf("file=%s direct kind=%d order=%d N=%d %s\n", argv[2], dkind, dorder, c.N, direct_hash(c, dkind, dorder).c_str());
+      return 0;
+    }
     printf("file=%s ok=%d E=%d hash=%016llx %s\n", argv[2], ok, c.Epl, (unsigned long long)H, err.c_str());
     return ok ? 0 : 1;
   }
@@ -118,6 +157,10 @@ int main(int argc, char** argv) {
   const double ms2 = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count();
   const uint64_t h2 = image_hash(c);
   ok = ok && (h1 == h2);   // the re-compile into the same object gives the same image
+  if (ok && dkind >= 0) {
+    printf("N=%d per=%d seed=%d direct kind=%d order=%d %s\n", N, per, seed, dkind, dorder, direct_hash(c, dkind, dorder).c_str());
+    return 0;
+  }
   H = h2;
   printf("N=%d per=%d seed=%d ok=%d E=%d hash=%016llx  (%.2f ms, again %.2f ms) %s\n", N, per, seed, ok, c.Epl, (unsigned long long)H, ms, ms2, err.c_str());
 }

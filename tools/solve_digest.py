@@ -5,7 +5,8 @@ device-side counterpart of compile_graph_hash.cpp.
 
     python tools/solve_digest.py [--quick]      (--quick: skip the 12 000-pose graph and the full config-3 graph)
 
-The PCG paths come first; the dense and insertion-order band direct solves follow.
+The PCG paths come first; the dense and band direct solves follow (band in insertion order and in nested-dissection (ND)
+order), then the ND covariances and a debug-stage-5 round trip of a stored S in every direct layout.
 """
 import hashlib
 import os
@@ -18,9 +19,11 @@ from pop_up_slam_b200 import capi, graphgen as gg   # noqa: E402
 from pop_up_slam_b200.capi import GpuGraphAPI       # noqa: E402
 
 
-def graph(g, flags=0, jac_numeric=False, kind=0, **props):
+def graph(g, flags=0, jac_numeric=False, kind=0, order=0, **props):
     a = GpuGraphAPI()
     a.set_linear_solver(kind)
+    if order:
+        a.set_direct_ordering(order)
     ids = gg.build_bulk(a, g)
     gg.configure(a, g, **props)
     if flags:
@@ -48,11 +51,48 @@ def solve(g, **kw):
     return [a]
 
 
-def updates(g, kind=0):
-    a = graph(g, kind=kind, method=0)
+def updates(g, kind=0, order=0):
+    a = graph(g, kind=kind, order=order, method=0)
     for _ in range(3):   # relinearise + one Gauss-Newton step each
         a[0].update()
     return [a]
+
+
+def covariances(g, h):
+    """ND solve, then every node's marginal and a seeded set of cross blocks (inside and outside L's pattern)"""
+    a, ids = graph(g, kind=2, order=1)
+    a.batch_optimize()
+    nodes = np.concatenate([ids["pose_ids"], ids["plane_ids"]]).astype(int)
+    rng = np.random.default_rng(7)
+    pairs = [(int(x), int(y)) for x, y in rng.choice(nodes, size=(48, 2))]
+    pairs += [(int(ids["pose_ids"][k]), int(ids["pose_ids"][k + 1])) for k in range(0, len(ids["pose_ids"]) - 1, 97)]
+    for blk in a.marginal_covariances(nodes) + a.covariance_blocks(pairs):
+        h.update(np.ascontiguousarray(blk).tobytes())
+    return [(a, ids)]
+
+
+def stage5(g, kind, order, h):
+    """S assembled by debug stage 4, fetched, stored back as Sdir, factored and solved by debug stage 5"""
+    a, ids = graph(g, kind=kind, order=order)
+    a.upload()
+    a.debug_run_stage(4, 1e-3)
+    n = 6 * len(ids["pose_ids"]) + 3 * len(a.debug_fetch("bborder", 1 << 16))
+    S = a.debug_fetch("Sdir", n * n)
+    a.debug_store("Sdir", S)
+    a.debug_store("b", np.random.default_rng(11).standard_normal(n))
+    a.debug_run_stage(5)
+    for v in (S, a.debug_fetch("dflag", 1), a.debug_fetch("Ldir", n * n), a.debug_fetch("x", n)):
+        h.update(np.ascontiguousarray(v).tobytes())
+    return [(a, ids)]
+
+
+def extra(run):
+    """a path whose run also feeds arrays of its own into the digest"""
+    def go():
+        h = hashlib.sha256()
+        apis = run(h)
+        return apis, h.hexdigest()
+    return go
 
 
 def span(g, world):
@@ -103,9 +143,24 @@ def main():
         ("c3/900 band direct, numeric Jacobians", lambda: solve(c3s, kind=2, jac_numeric=True)),
         ("c2 dense direct update() x3", lambda: updates(gg.make_config(2, seed=1), kind=1)),
     ]
+    # the band solve in nested-dissection order, its covariances, and a stored S through debug stage 5
+    rv = gg.make_revisit(seed=0, n_poses=2000, n_planes=100, max_iterations=3)
+    paths += [
+        ("c2 ND direct", lambda: solve(c2, kind=2, order=1)),
+        ("c3/900 ND direct", lambda: solve(c3s, kind=2, order=1)),
+        ("revisit/2000 ND direct", lambda: solve(rv, kind=2, order=1)),
+        ("c3/900 ND direct, numeric Jacobians", lambda: solve(c3s, kind=2, order=1, jac_numeric=True)),
+        ("c2 ND direct update() x3", lambda: updates(gg.make_config(2, seed=1), kind=2, order=1)),
+        ("c2 ND covariances", extra(lambda h: covariances(c2, h))),
+        ("revisit/2000 ND covariances", extra(lambda h: covariances(rv, h))),
+    ]
+    for kind, order, what in [(1, 0, "dense"), (2, 0, "band"), (2, 1, "ND")]:
+        paths.append((f"c2 {what} stored Sdir, stage 5", extra(lambda h, k=kind, o=order: stage5(c2, k, o, h))))
     for name, run in paths:
-        pcg, d = digest(run())
-        print(f"{name:36s} pcg={pcg:7d} {d}", flush=True)
+        out = run()
+        apis, more = out if isinstance(out, tuple) else (out, "")
+        pcg, d = digest(apis)
+        print(f"{name:36s} pcg={pcg:7d} {d}{' ' + more if more else ''}", flush=True)
 
 
 if __name__ == "__main__":
