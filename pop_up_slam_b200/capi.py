@@ -553,6 +553,17 @@ class GpuGraphAPI(GraphAPI):
     def debug_run_stage(self, stage, lam=0.0):
         self._chk(self.lib.pus_debug_run_stage(self.h, int(stage), float(lam)))
 
+    PATH_BITS = ("resident", "tma", "tma_ring", "apply_smem", "apply_l2", "l3_local", "cluster", "res_listed_heavy",
+                 "res_unlisted_heavy", "res_pose_pose_tail", "res_wide_block", "coarse_tail")
+
+    def pcg_path(self):
+        """The branches the kernel reported for the linear solve of the last debug launch: a dict of the PathBit flags
+        (pus_kernels.cuh) plus the team size, the preconditioner levels, the hat spacing SP and the most pose blocks a CTA owns."""
+        v = self.debug_fetch("path", 5).astype(int)
+        d = {name: bool(v[0] >> i & 1) for i, name in enumerate(self.PATH_BITS)}
+        d.update(team=int(v[1]), levels=int(v[2]), SP=int(v[3]), owned=int(v[4]))
+        return d
+
 
 def _handles(apis):
     arr = (C.c_void_p * len(apis))(*[a.h for a in apis])

@@ -53,6 +53,13 @@ __device__ double schur_solve(Phase& ph, Ctx& c, double lambda, int* its, Timer&
   // spanning solve: the PCG phases are split over the CTAs of all ranks (every rank keeps full copies of the vectors)
   span_view(c, true);
   const bool resident = G.prm.resident && !c.use_tma && !c.mirror;   // block-resident loop (pcg_resident): loads its own caches
+  if (G.prm.mode == MODE_DEBUG && threadIdx.x == 0) {   // path report (PathBit); the apply branches add theirs as they run
+    LmResult* res = G.res;
+    atomicOr(&res->status, (resident ? (int)kPathResident : 0) | (c.use_tma ? (int)kPathTma : 0) |
+                               (c.l3_local ? (int)kPathL3Local : 0) | (c.cluster ? (int)kPathCluster : 0));
+    atomicMax(&res->trace_n, (G.nblk - c.rank + c.tsize - 1) / c.tsize);   // owned pose blocks k = rank + tsize * i
+    if (c.rank == 0) { res->iterations = c.tsize; res->accepted = G.levels; res->chi2_evals = G.SP; }
+  }
   if (!c.use_tma && !resident) {   // (large graphs use that shared memory for the TMA staging buffers instead)
     ph.cache_blocks();
     c.smem_cache_ok = 1;

@@ -121,6 +121,7 @@ struct Solver {
   LmTrace* d_trace = nullptr;
   unsigned* d_bar = nullptr;
   LmResult res;
+  int path[5] = {0, 0, 0, 0, 0};   // the last debug launch's path report (PathBit flags, team size, levels, SP, owned blocks)
   LmTrace trace;
   pus_stats stats;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -588,6 +589,12 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
     } else {
       CUDA_OK(cudaMemcpyAsync(&s->res, s->d_res, sizeof(LmResult), cudaMemcpyDeviceToHost, s0->stream));
       CUDA_OK(cudaStreamSynchronize(s0->stream));
+    }
+    if (mode == MODE_DEBUG) {   // the path report rides in fields a debug launch leaves unused: moved aside, the statistics keep 0
+      LmResult& r = s->res;
+      const int rep[5] = {r.status, r.iterations, r.accepted, r.chi2_evals, r.trace_n};
+      std::memcpy(s->path, rep, sizeof(rep));
+      r.status = r.iterations = r.accepted = r.chi2_evals = r.trace_n = 0;
     }
     pus_stats& st = s->stats;
     st.lm_iterations = s->res.iterations; st.accepted = s->res.accepted; st.relinearizations = s->res.relin;
@@ -1948,6 +1955,10 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
     if (cap >= 14) { out[12] = c.SP; out[13] = c.nc_pad; }
     if (cap >= 18) { out[14] = c.levels; out[15] = c.nc2; out[16] = c.ng2; out[17] = c.nce2; }
     return cap >= 18 ? 18 : (cap >= 14 ? 14 : 12);
+  }
+  if (nm == "path") {   // what the kernel reported of the last debug launch: PathBit flags, team size, levels, SP, most owned blocks
+    for (int k = 0; k < 5 && k < cap; k++) out[k] = (double)s->path[k];
+    return 5;
   }
   if (!s->uploaded) { g_err = "nothing uploaded"; return -1; }
   if (nm == "W" || nm == "Wt") {  // de-tiled: [slots][18] in pose-major slot order (W) or plane-major order (Wt)

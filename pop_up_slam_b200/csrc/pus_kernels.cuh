@@ -29,6 +29,24 @@ constexpr int kMaxStage = 64;  // staged group members in the dense-block build
 
 enum KernelMode { MODE_BATCH = 0, MODE_UPDATE = 1, MODE_DEBUG = 2, MODE_CHI2 = 3, MODE_COV = 4 };
 
+// MODE_DEBUG only: the branches the linear solve took, OR-ed into LmResult::status by the code that took them
+// (pus_debug_fetch "path"; LmResult::iterations / accepted / chi2_evals / trace_n then hold the team size, the preconditioner
+// levels, the hat spacing SP and the largest number of pose blocks one CTA owns)
+enum PathBit {
+  kPathResident = 1,       // block-resident loop (pcg_resident)
+  kPathTma = 2,            // W / Wt tiles staged by TMA
+  kPathTmaRing = 4,        // dense blocks applied from the three-stage bulk-copy ring
+  kPathApplySmem = 8,      // dense blocks applied from the shared-memory cache (plain loop)
+  kPathApplyL2 = 16,       // dense blocks applied straight from L2 (plain loop)
+  kPathL3Local = 32,       // three levels, level 3 applied by every CTA itself
+  kPathCluster = 64,       // the team is one thread-block cluster
+  kPathResListed = 128,    // resident loop: heavy planes summed once per CTA
+  kPathResUnlisted = 256,  // resident loop: heavy planes past kResHeavy, summed by a warp of their block
+  kPathResTail = 512,      // resident loop: pose-pose factors past the first two neighbours (loop closures)
+  kPathResWide = 1024,     // resident loop: a pose block with more than 96 plane groups
+  kPathCoarseTail = 2048,  // two levels: coarse residual over more than 8 blocks per hat interval
+};
+
 struct LmParams {
   int method;  // 0 GN, 1 LM
   double eps2, eps_abs, eps_rel;
@@ -2509,6 +2527,7 @@ struct Phase {
   #pragma unroll
           for (int t = 0; t < 8; t++) acc += va[side][t] - alpha * vq[side][t];
         if (bpn > 8) {  // (spacing > 128 poses: rare large graphs) remaining blocks, plain loop
+          if (G.prm.mode == MODE_DEBUG && i == 0) atomicOr(&G.res->status, (int)kPathCoarseTail);
           for (int side = 0; side < 2; side++) {
             int cint = node - side;
             if (cint < 0) continue;
@@ -2544,6 +2563,7 @@ struct Phase {
       // (loads of three rounds in flight together), then (B) stream the owned dense blocks Binv[k] through the
       // two 72 KB staging buffers with one bulk async copy each (the next block in flight while this one is applied).
       double* sR = reinterpret_cast<double*>(g_smem + sr_off);
+      if (G.prm.mode == MODE_DEBUG && tid == 0) atomicOr(&G.res->status, (int)kPathTmaRing);
       __syncthreads();
       for (int rd0 = 0; rd0 < nrd; rd0 += 3) {
         double vr[3], vp[3], vq[3], vx[3];
@@ -2642,11 +2662,13 @@ struct Phase {
         // dense block: z_local = Binv[k] r_block (symmetric: read column u)
         const int ci = slot + kSlots * rd;
         const double* rv = sA + slot * kBlockDim;
-        const double zl = (ci < kCacheBlocks && c.smem_cache_ok)
+        const bool cached = ci < kCacheBlocks && c.smem_cache_ok;
+        const double zl = cached
                               ? packed_row_dot<LdS>(reinterpret_cast<const double*>(g_smem + kSmCache) + (size_t)ci * kPackedBlock, u, rv)
                               : packed_row_dot<LdL2>(G.Binv + (size_t)k * kPackedBlock, u, rv);   // straight from L2
         put(c, &G.z[(size_t)p * 6 + row], zl);
         dot += rn * zl;
+        if (G.prm.mode == MODE_DEBUG && u == 0) atomicOr(&G.res->status, (int)(cached ? kPathApplySmem : kPathApplyL2));
       }
     }
     lap(15);
@@ -2765,7 +2787,7 @@ struct Phase {
     // partial count.  (More than kResHeavy distinct ones: the rest keep the per-block warp loop.)
     int* hvl = reinterpret_cast<int*>(g_smem + L.hdr + 64);   // [kResHeavy][4] = {plane, first partial, count, -}
     if (tid == 0) {
-      int nh = 0;
+      int nh = 0, unlisted = 0;
       for (int s = 0; s < nown; s++) {
         int4* gs = reinterpret_cast<int4*>(g_smem + L.slot0 + s * L.stride + L.o_gi);
         for (int g = 0; g < hdr[8 + s]; g++) {
@@ -2774,7 +2796,7 @@ struct Phase {
           int h = 0;
           while (h < nh && hvl[h * 4] != q.x) h++;
           if (h == nh) {
-            if (nh == kResHeavy) continue;
+            if (nh == kResHeavy) { unlisted = 1; continue; }
             hvl[h * 4] = q.x; hvl[h * 4 + 1] = q.y; hvl[h * 4 + 2] = q.z;
             nh++;
           }
@@ -2782,6 +2804,11 @@ struct Phase {
         }
       }
       hdr[7] = nh;
+      if (G.prm.mode == MODE_DEBUG) atomicOr(&G.res->status, (nh ? (int)kPathResListed : 0) | (unlisted ? (int)kPathResUnlisted : 0));
+    }
+    if (G.prm.mode == MODE_DEBUG) {
+      if (on && nr.y > nr.x) atomicOr(&G.res->status, (int)kPathResTail);
+      if (live && u == 0 && hdr[8 + slot] > kBlockDim) atomicOr(&G.res->status, (int)kPathResWide);
     }
     __syncthreads();
     const int ng = live ? hdr[8 + slot] : 0;
@@ -3032,7 +3059,10 @@ struct Phase {
       beta = rz_new / rz;
       rz = rz_new;
     }
-    if (on) G.x[o] = x_u;
+    if (on) {
+      G.x[o] = x_u;
+      if (G.prm.mode == MODE_DEBUG) { G.r[o] = r_u; G.z[o] = z_u; G.q[o] = q_u; }   // the exit state, as the general loop leaves it
+    }
     team_barrier(c);
     return it;
   }
