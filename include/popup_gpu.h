@@ -263,6 +263,38 @@ int pus_popup_fit_frames(int device, int n_frames, const int* seg_ptr, const flo
                          const float* Ts, float dist_thre, int mode, float* planes_world, float* planes_sensor,
                          float* dist, int* good);
 
+/* ---- dense plane clouds (float32) ------------------------------------------------------------------ */
+/* popup_plane::generate_cloud (PUW/libs/popup_plane.cpp:807-863) with closed_polygons_homo_pts (:81-116) and
+ * matrixToCloud (:925-985), batched over frames and their good planes, on the device:
+ *   plane_ptr[n_frames+1]   CSR offsets of the frames' planes, in the caller's order; the first plane of every frame is the
+ *                           ground (label 255), the others walls (label 0), as in pus_popup_fit_frames' rows
+ *   poly_ptr[n_planes+1], polys[n_vertices][2]   each plane's closed 2-D polygon (float pixels); an empty one gives no points
+ *   planes_sensor[n_planes][4]   the plane in the sensor frame (pus_popup_fit_frames' planes_sensor rows)
+ *   Ts[n_frames][16] row-major camera-to-world, invK[9] row-major
+ *   images[n_frames][height][width][3]   packed BGR, or NULL (colour 0, no border rule); width and height are needed either way
+ *   downsample   halve the polygon, fill, double the pixel coordinates (generate_cloud's downsample_poly)
+ * Per pixel: the polygon (halved when downsampling) is truncated to integer points, filled on its bounding box with
+ * cv::fillConvexPoly's rule (OpenCV 4.13, LINE_8, shift 0; non-convex, degenerate and partly off-image polygons included) and
+ * listed in cv::findNonZero order.  ray = invK (x, y, 1), p_s = -d / (n . ray) ray (ray_plane_interact), p_w = R p_s + t.
+ * Points with p_s.z < 0, p_s.z > depth_thre or p_w.z < -0.2 are dropped, z is clamped to ceiling_threshold, and with
+ * 960-wide images pixels with x < 4 or y < 4 are dropped.
+ * Outputs (any may be NULL): counts[n_planes] kept points per plane, offsets[n_planes] their first index; xyz[total][3] and
+ * rgb[total][3] (r, g, b) the per-plane clouds back to back, which is also the frame's mixed cloud; capacity is their room in
+ * points (xyz = rgb = NULL is a size query, too small a capacity fails with a message); labels[n_frames][height][width]
+ * 127 void / 255 ground / 0 wall, with the nearest-neighbour 0.5x / 2x resize in downsample mode (even sizes only).
+ * Returns the total number of points.  The outputs are deterministic: repeated calls and any split of the batch give the
+ * same bytes.  Two deviations from the reference, where it is undefined: pixels outside the image keep their points with
+ * colour 0 and are not written to the label image (the reference reads and writes out of bounds), and a call without images
+ * gives colour 0 (the reference keeps the previous point's colour).  The fill is pinned to OpenCV 4.13; differences of older
+ * OpenCV releases are not reproduced.  Polygons have at most PUS_POPUP_MAX_VERTICES vertices and coordinates of magnitude
+ * at most PUS_POPUP_MAX_COORD. */
+#define PUS_POPUP_MAX_VERTICES 256
+#define PUS_POPUP_MAX_COORD 1048576.0f
+long long pus_popup_clouds(int device, int n_frames, const int* plane_ptr, const int* poly_ptr, const float* polys,
+                           const float* planes_sensor, const float* Ts, const float* invK, const unsigned char* images,
+                           int width, int height, int downsample, float depth_thre, float ceiling_threshold, int* counts,
+                           long long* offsets, float* xyz, unsigned char* rgb, long long capacity, unsigned char* labels);
+
 /* ---- device-resident measurement refresh and polygon re-projection (SURVEY.md 8f.1) -------- */
 /* Mapper_mono::update_plane_measurement (pop_planar_slam/src/Mapping.cpp:590-607): after a solve every past
  * frame re-pops its wall planes from its ground segments with the frame's LATEST pose estimate

@@ -631,3 +631,57 @@ def popup_fit_frames(lib, seg_ptr, segs, invK, Ts, dist_thre=10.0, mode=0, prefi
     if rc < 0:
         raise ApiError("popup_fit_frames failed")
     return pw, ps, dist, good
+
+
+def popup_clouds(lib, plane_ptr, poly_ptr, polys, planes_sensor, Ts, invK, width, height, images=None, downsample=True,
+                 depth_thre=5.0, ceiling_threshold=2.8, labels=False, points=True, capacity=None, prefix="pus_", device=0):
+    """popup_plane::generate_cloud batched over frames and their planes (pus_popup_clouds, include/popup_gpu.h).
+
+    plane_ptr [n_frames+1] and poly_ptr [n_planes+1] are CSR offsets; polys [n_vertices, 2] float pixels; planes_sensor
+    [n_planes, 4]; Ts [n_frames, 4, 4] camera-to-world; images [n_frames, height, width, 3] uint8 BGR or None.
+    Returns a dict: counts [n_planes] int32, offsets [n_planes] int64, xyz [total, 3] float32 and rgb [total, 3] uint8
+    (absent with points=False: a size query), labels [n_frames, height, width] uint8 (with labels=True).  Without a
+    capacity (in points) a size query runs first; with one, a single call fills buffers of that size."""
+    plane_ptr = _i32(plane_ptr)
+    nf = len(plane_ptr) - 1
+    npl = int(plane_ptr[-1])
+    poly_ptr = _i32(poly_ptr)
+    polys = np.ascontiguousarray(polys, dtype=np.float32).reshape(-1, 2)
+    planes_sensor = np.ascontiguousarray(planes_sensor, dtype=np.float32).reshape(-1, 4)
+    Ts = np.ascontiguousarray(Ts, dtype=np.float32).reshape(nf, 4, 4)
+    invK = np.ascontiguousarray(invK, dtype=np.float32).reshape(3, 3)
+    u8p = C.POINTER(C.c_ubyte)
+    img = None if images is None else np.ascontiguousarray(images, dtype=np.uint8).reshape(nf, height, width, 3)
+    counts = np.zeros(npl, np.int32)
+    offsets = np.zeros(npl, np.int64)
+    lab = np.zeros((nf, height, width), np.uint8) if labels else None
+    fn = getattr(lib, prefix + "popup_clouds")
+    fn.restype = C.c_longlong
+    fn.argtypes = [C.c_int, C.c_int, c_int_p, c_int_p, c_float_p, c_float_p, c_float_p, c_float_p, u8p, C.c_int, C.c_int,
+                   C.c_int, C.c_float, C.c_float, c_int_p, C.POINTER(C.c_longlong), c_float_p, u8p, C.c_longlong, u8p]
+    err = getattr(lib, prefix + "last_error", None) or getattr(lib, prefix + "popup_last_error")
+    err.restype = C.c_char_p
+
+    def call(xyz, rgb, cap):
+        n = fn(device, nf, _ip(plane_ptr), _ip(poly_ptr), polys.ctypes.data_as(c_float_p),
+               planes_sensor.ctypes.data_as(c_float_p), Ts.ctypes.data_as(c_float_p), invK.ctypes.data_as(c_float_p),
+               None if img is None else img.ctypes.data_as(u8p), int(width), int(height), int(bool(downsample)),
+               float(depth_thre), float(ceiling_threshold), _ip(counts), offsets.ctypes.data_as(C.POINTER(C.c_longlong)),
+               None if xyz is None else xyz.ctypes.data_as(c_float_p), None if rgb is None else rgb.ctypes.data_as(u8p),
+               int(cap), None if lab is None else lab.ctypes.data_as(u8p))
+        if n < 0:
+            raise ApiError((err() or b"?").decode())
+        return n
+
+    out = {"counts": counts, "offsets": offsets}
+    if not points:
+        total = call(None, None, 0)
+    else:
+        cap = call(None, None, 0) if capacity is None else int(capacity)
+        xyz, rgb = np.empty((cap, 3), np.float32), np.empty((cap, 3), np.uint8)
+        total = call(xyz, rgb, cap)
+        out.update(xyz=xyz[:total], rgb=rgb[:total])
+    out["total"] = total
+    if labels:
+        out["labels"] = lab
+    return out
