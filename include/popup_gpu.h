@@ -295,6 +295,36 @@ long long pus_popup_clouds(int device, int n_frames, const int* plane_ptr, const
                            int width, int height, int downsample, float depth_thre, float ceiling_threshold, int* counts,
                            long long* offsets, float* xyz, unsigned char* rgb, long long capacity, unsigned char* labels);
 
+/* ---- closed wall and ground polygons (float32) ------------------------------------------------------------------ */
+/* popup_plane::find_2d_3d_closed_polygon (PUW/libs/popup_plane.cpp:120-406, simple_polygon_mode = false) with
+ * direction_hit_boundary and cut_wall_polygons (PUW/libs/matrix_utils.cpp:229-270, 506-713), batched over frames, on the
+ * device.  The step between get_plane_equation (pus_popup_fit_frames) and generate_cloud (pus_popup_clouds):
+ *   seg_ptr[n_frames+1], segs   the frames' connected ground segments, as pus_popup_fit_frames
+ *   K[9], invK[9] row-major, Ts[n_frames][16] row-major camera-to-world; width, height the image size
+ *   ceiling_threshold   the cut height; walllength_threshold   the cut length from the ground endpoint nearer the camera
+ *                       (negative: height only, as cut_wall_polygons tests it)
+ * Rows as pus_popup_fit_frames': n_seg(f) + 1 per frame at seg_ptr[f] + f, row 0 the ground.  Per row:
+ *   bound2d   the closed 2-D polygon out to the image border (all_closed_2d_bound_polygons)
+ *   world3d   a wall's polygon on its plane in the world frame, cut (all_3d_bound_polygons_world); empty for the ground,
+ *             which the reference never assigns
+ *   cut2d     world3d projected back through K (all_closed_2d_cutted_polygons); the ground's is its bound polygon
+ * Counts per row ([n_rows] each) are always written; the vertices are packed in row order (2 or 3 floats each), so both
+ * 2-D sets are the poly_ptr / polys input of pus_popup_clouds.  bound2d = cut2d = world3d = NULL is a size query; the
+ * capacities are in vertices, and too small a one fails with a message.  Frames without segments give empty rows.
+ * The planes and world ground endpoints come from the same device code as pus_popup_fit_frames (mode 0).  The cut follows
+ * OpenCV 4.13's cv::convexHull (start vertex, orientation, dropped collinear and duplicate points) and cv::pointPolygonTest
+ * on Point2f; point sets with three points collinear only up to float rounding are outside that guarantee (OpenCV's
+ * result there depends on how its build contracts the orientation test).  Deviations: the camera inverse is
+ * [R^T | -R^T t] in closed form (Eigen's general inverse may differ in the last bit); float -> int truncations follow x86
+ * (NaN or out of range gives INT_MIN); where find_correct_ground_seq would index past its hull the uncut polygon is kept,
+ * as when it finds no sequence; nothing is printed.  Deterministic: repeated calls and any split of the batch give the
+ * same bytes.  There is no CPU fallback. */
+#define PUS_POPUP_MAX_SEGMENTS (PUS_POPUP_MAX_VERTICES - 6)   /* a ground polygon has n + 6 vertices at most */
+int pus_popup_polygons(int device, int n_frames, const int* seg_ptr, const float* segs, const float* K, const float* invK,
+                       const float* Ts, int width, int height, float ceiling_threshold, float walllength_threshold,
+                       int* bound_counts, int* cut_counts, int* world_counts, float* bound2d, float* cut2d, float* world3d,
+                       long long bound_capacity, long long cut_capacity, long long world_capacity);
+
 /* ---- device-resident measurement refresh and polygon re-projection (SURVEY.md 8f.1) -------- */
 /* Mapper_mono::update_plane_measurement (pop_planar_slam/src/Mapping.cpp:590-607): after a solve every past
  * frame re-pops its wall planes from its ground segments with the frame's LATEST pose estimate

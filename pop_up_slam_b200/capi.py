@@ -685,3 +685,51 @@ def popup_clouds(lib, plane_ptr, poly_ptr, polys, planes_sensor, Ts, invK, width
     if labels:
         out["labels"] = lab
     return out
+
+
+def popup_polygons(lib, seg_ptr, segs, K, invK, Ts, width, height, ceiling_threshold=2.5, walllength_threshold=3.0,
+                   vertices=True, capacity=None, prefix="pus_", device=0):
+    """popup_plane::find_2d_3d_closed_polygon batched over frames (pus_popup_polygons, include/popup_gpu.h).
+
+    seg_ptr [n_frames+1] CSR offsets, segs [n_seg, 4] float pixels, K and invK [3, 3], Ts [n_frames, 4, 4]
+    camera-to-world.  Rows as popup_fit_frames'.  Returns a dict with, for each of "bound" (2-D, to the image border),
+    "cut" (2-D, the cut polygon projected back) and "world" (3-D, cut, on the wall): <name>_counts [n_rows] int32,
+    <name>_ptr [n_rows+1] int32 CSR offsets and, unless vertices=False (a size query), <name> [total, 2 or 3] float32.
+    bound_ptr / bound or cut_ptr / cut are the poly_ptr / polys of popup_clouds.  capacity = (bound, cut, world) in
+    vertices fills buffers of that size instead of the queried ones."""
+    seg_ptr = _i32(seg_ptr)
+    nf = len(seg_ptr) - 1
+    n_rows = int(seg_ptr[-1]) + nf
+    segs = np.ascontiguousarray(segs, dtype=np.float32).reshape(-1, 4)
+    K = np.ascontiguousarray(K, dtype=np.float32).reshape(3, 3)
+    invK = np.ascontiguousarray(invK, dtype=np.float32).reshape(3, 3)
+    Ts = np.ascontiguousarray(Ts, dtype=np.float32).reshape(nf, 4, 4)
+    cnt = {k: np.zeros(n_rows, np.int32) for k in ("bound", "cut", "world")}
+    fn = getattr(lib, prefix + "popup_polygons")
+    fn.restype = C.c_int
+    fn.argtypes = [C.c_int, C.c_int, c_int_p, c_float_p, c_float_p, c_float_p, c_float_p, C.c_int, C.c_int, C.c_float,
+                   C.c_float, c_int_p, c_int_p, c_int_p, c_float_p, c_float_p, c_float_p, C.c_longlong, C.c_longlong,
+                   C.c_longlong]
+    err = getattr(lib, prefix + "last_error", None) or getattr(lib, prefix + "popup_last_error")
+    err.restype = C.c_char_p
+
+    def call(out, caps):
+        rc = fn(device, nf, _ip(seg_ptr), segs.ctypes.data_as(c_float_p), K.ctypes.data_as(c_float_p),
+                invK.ctypes.data_as(c_float_p), Ts.ctypes.data_as(c_float_p), int(width), int(height),
+                float(ceiling_threshold), float(walllength_threshold), _ip(cnt["bound"]), _ip(cnt["cut"]), _ip(cnt["world"]),
+                *[None if o is None else o.ctypes.data_as(c_float_p) for o in out], *[int(c) for c in caps])
+        if rc < 0:
+            raise ApiError((err() or b"?").decode())
+
+    call((None, None, None), (0, 0, 0))
+    res = {}
+    for k in cnt:
+        res[k + "_counts"] = cnt[k].copy()
+        res[k + "_ptr"] = np.concatenate([[0], np.cumsum(cnt[k])]).astype(np.int32)
+    if vertices:
+        tot = [int(res[k + "_ptr"][-1]) for k in cnt]
+        cap = tot if capacity is None else [int(c) for c in capacity]
+        out = (np.empty((cap[0], 2), np.float32), np.empty((cap[1], 2), np.float32), np.empty((cap[2], 3), np.float32))
+        call(out, cap)
+        res.update(bound=out[0][:tot[0]], cut=out[1][:tot[1]], world=out[2][:tot[2]])
+    return res

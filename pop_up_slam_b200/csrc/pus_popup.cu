@@ -13,6 +13,7 @@
 #include <climits>
 #include <cmath>
 #include <cstdint>
+#include <cstring>
 #include <string>
 #include <vector>
 
@@ -37,7 +38,7 @@ __device__ __forceinline__ float seg_dist(const float* b, const float* e, const 
 __global__ void popup_kernel(int n_frames, const int* __restrict__ seg_ptr, const int* __restrict__ row_frame,
                              int n_rows, const float* __restrict__ segs, const float* __restrict__ invK,
                              const float* __restrict__ Ts, float dist_thre, int mode, float* planes_world,
-                             float* planes_sensor, float* dist, int* good) {
+                             float* planes_sensor, float* dist, int* good, float* ends_world = nullptr) {
   int row = blockIdx.x * blockDim.x + threadIdx.x;
   if (row >= n_rows) return;
   const int f = row_frame[row];
@@ -82,6 +83,9 @@ __global__ void popup_kernel(int n_frames, const int* __restrict__ seg_ptr, cons
   }
   if (mode == 0) {
     Pw[0][2] = 0.f; Pw[1][2] = 0.f;
+    if (ends_world)   // the world ground endpoints (get_plane_equation's ground_seg3d_lines_world row)
+      for (int k = 0; k < 2; k++)
+        for (int i = 0; i < 3; i++) ends_world[(size_t)row * 6 + 3 * k + i] = Pw[k][i];
     float t1[3] = {Pw[1][0] - Pw[0][0], Pw[1][1] - Pw[0][1], Pw[1][2] - Pw[0][2]};
     float t2[3] = {gw[0], gw[1], gw[2]};
     float nrm[3] = {t1[1] * t2[2] - t1[2] * t2[1], t1[2] * t2[0] - t1[0] * t2[2], t1[0] * t2[1] - t1[1] * t2[0]};
@@ -679,4 +683,596 @@ extern "C" long long pus_popup_clouds(int device, int n_frames, const int* plane
   }
   CCHK(cudaDeviceSynchronize());
   return total;
+}
+
+// ---- closed wall and ground polygons (pus_popup_polygons) -------------------------------------------------------------
+// popup_plane::find_2d_3d_closed_polygon (popup_plane.cpp:120-406) with direction_hit_boundary, polygon_overlap_func,
+// find_correct_ground_seq and cut_wall_polygons (matrix_utils.cpp:229-270, 506-713), and OpenCV 4.13's cv::convexHull and
+// cv::pointPolygonTest on Point2f.  One thread per (frame, plane) row; the polygons go to fixed per-row slots, and a second
+// pass packs the slots in row order at offsets scanned from the counts.
+namespace pus {
+namespace poly {
+constexpr int kBoundSlot = PUS_POPUP_MAX_VERTICES;   // the ground polygon has n + 6 vertices at most, a wall's 7
+constexpr int kWallMax = 7;
+constexpr int kHullMax = 34;                          // 6 x 4 edge crossings + 10 corners
+constexpr int kCutSlot = kHullMax + 1;
+
+struct P2 { float x, y; };
+struct P3 { float x, y, z; };
+
+// x86 cvttss2si, which the reference's (int) casts compile to: NaN or out of range gives INT_MIN (cvt.rzi saturates)
+__device__ __forceinline__ int trunc_i(float v) { return (v >= -2147483648.f && v < 2147483648.f) ? __float2int_rz(v) : INT_MIN; }
+__device__ __forceinline__ int sgnf(float a) { return (a > 0.f) - (a < 0.f); }
+
+__device__ int sklansky(const P2* p, const int* ord, int start, int end, int* stack, int nsign, int sign2) {
+  const int incr = end > start ? 1 : -1;
+  int pprev = start, pcur = pprev + incr, pnext = pcur + incr;
+  int stacksize = 3;
+  if (start == end || (p[ord[start]].x == p[ord[end]].x && p[ord[start]].y == p[ord[end]].y)) {
+    stack[0] = start;
+    return 1;
+  }
+  stack[0] = pprev;
+  stack[1] = pcur;
+  stack[2] = pnext;
+  end += incr;
+  while (pnext != end) {
+    const float cury = p[ord[pcur]].y, nexty = p[ord[pnext]].y, by = nexty - cury;
+    if (sgnf(by) != nsign) {
+      const float ax = p[ord[pcur]].x - p[ord[pprev]].x, bx = p[ord[pnext]].x - p[ord[pcur]].x, ay = cury - p[ord[pprev]].y;
+      const float convexity = ay * bx - ax * by;
+      if (sgnf(convexity) == sign2 && (ax != 0 || ay != 0)) {
+        pprev = pcur;
+        pcur = pnext;
+        pnext += incr;
+        stack[stacksize] = pnext;
+        stacksize++;
+      } else if (pprev == start) {
+        pcur = pnext;
+        stack[1] = pcur;
+        pnext += incr;
+        stack[2] = pnext;
+      } else {
+        stack[stacksize - 2] = pnext;
+        pcur = pprev;
+        pprev = stack[stacksize - 4];
+        stacksize--;
+      }
+    } else {
+      pnext += incr;
+      stack[stacksize - 1] = pnext;
+    }
+  }
+  return --stacksize;
+}
+
+// cv::convexHull(points, hull, clockwise = false, returnPoints = true); n <= kHullMax.  The sort is an insertion sort on
+// OpenCV's order (x, y, then position), a total order, so it gives std::sort's result.
+__device__ int convex_hull(const P2* p, int n, P2* out) {
+  if (n <= 0) return 0;
+  int ord[kHullMax], stack[kHullMax + 2], hull[kHullMax];
+  for (int i = 0; i < n; i++) ord[i] = i;
+  for (int i = 1; i < n; i++) {
+    const int k = ord[i];
+    int j = i - 1;
+    while (j >= 0) {
+      const P2 a = p[ord[j]], b = p[k];
+      const bool greater = a.x != b.x ? b.x < a.x : a.y != b.y ? b.y < a.y : k < ord[j];
+      if (!greater) break;
+      ord[j + 1] = ord[j];
+      j--;
+    }
+    ord[j + 1] = k;
+  }
+  int miny = 0, maxy = 0;
+  for (int i = 1; i < n; i++) {
+    const float y = p[ord[i]].y;
+    if (p[ord[miny]].y > y) miny = i;
+    if (p[ord[maxy]].y < y) maxy = i;
+  }
+  int nout = 0;
+  if (p[ord[0]].x == p[ord[n - 1]].x && p[ord[0]].y == p[ord[n - 1]].y) {
+    hull[nout++] = ord[0];
+  } else {
+    // upper half, right chain first (clockwise = false)
+    int tlc = sklansky(p, ord, 0, maxy, stack, -1, 1);
+    int* tr = stack;
+    int* tl = stack + tlc;
+    int trc = tlc;
+    tlc = sklansky(p, ord, n - 1, maxy, tl, -1, -1);
+    for (int i = 0; i < tlc - 1; i++) hull[nout++] = ord[tl[i]];
+    for (int i = trc - 1; i > 0; i--) hull[nout++] = ord[tr[i]];
+    const int stop = trc > 2 ? tr[1] : tlc > 2 ? tl[tlc - 2] : -1;
+    int* bl = stack;
+    int blc = sklansky(p, ord, 0, miny, bl, 1, -1);
+    int* br = stack + blc;
+    int brc = sklansky(p, ord, n - 1, miny, br, 1, 1);
+    if (stop >= 0) {
+      const int check = blc > 2 ? bl[1] : blc + brc > 2 ? br[2 - blc] : -1;
+      if (check == stop || (check >= 0 && p[ord[check]].x == p[ord[stop]].x && p[ord[check]].y == p[ord[stop]].y)) {
+        blc = min(blc, 2);
+        brc = min(brc, 2);
+      }
+    }
+    for (int i = 0; i < blc - 1; i++) hull[nout++] = ord[bl[i]];
+    for (int i = brc - 1; i > 0; i--) hull[nout++] = ord[br[i]];
+    if (nout >= 3) {   // the cyclic shift that makes the indices ascending or descending where one exists
+      int min_idx = 0, max_idx = 0, lt = 0;
+      for (int i = 1; i < nout; i++) {
+        const int idx = hull[i];
+        lt += hull[i - 1] < idx;
+        if (lt > 1 && lt <= i - 2) break;
+        if (idx < hull[min_idx]) min_idx = i;
+        if (idx > hull[max_idx]) max_idx = i;
+      }
+      const int mmdist = abs(max_idx - min_idx);
+      if ((mmdist == 1 || mmdist == nout - 1) && (lt <= 1 || lt >= nout - 2)) {
+        const int ascending = (max_idx + 1) % nout == min_idx;
+        const int i0 = ascending ? min_idx : max_idx;
+        int j = i0;
+        if (i0 > 0) {
+          int i;
+          for (i = 0; i < nout; i++) {
+            const int cur = stack[i] = hull[j];
+            const int next = hull[j + 1 < nout ? j + 1 : 0];
+            if (i < nout - 1 && (ascending != (cur < next))) break;
+            if (++j >= nout) j = 0;
+          }
+          if (i == nout)
+            for (int k = 0; k < nout; k++) hull[k] = stack[k];
+        }
+      }
+    }
+  }
+  for (int i = 0; i < nout; i++) out[i] = p[hull[i]];
+  return nout;
+}
+
+// cv::pointPolygonTest(contour, pt, measureDist = false): 1 inside, 0 on the outline, -1 outside
+__device__ int point_polygon_test(const P2* c, int n, P2 pt) {
+  if (n == 0) return -1;
+  int counter = 0;
+  P2 v = c[n - 1];
+  for (int i = 0; i < n; i++) {
+    const P2 v0 = v;
+    v = c[i];
+    if ((v0.y <= pt.y && v.y <= pt.y) || (v0.y > pt.y && v.y > pt.y) || (v0.x < pt.x && v.x < pt.x)) {
+      if (pt.y == v.y && (pt.x == v.x || (pt.y == v0.y && ((v0.x <= pt.x && pt.x <= v.x) || (v.x <= pt.x && pt.x <= v0.x)))))
+        return 0;
+      continue;
+    }
+    // products of two floats are exact in double, so only the difference rounds
+    double dist = (double)(pt.y - v0.y) * (double)(v.x - v0.x) - (double)(pt.x - v0.x) * (double)(v.y - v0.y);
+    if (dist == 0) return 0;
+    if (v.y < v0.y) dist = -dist;
+    counter += dist > 0;
+  }
+  return counter % 2 == 0 ? -1 : 1;
+}
+
+// direction_hit_boundary (nobottom = false); its lambdas are double expressions rounded to float
+__device__ P2 hit_boundary(P2 pt, P2 d, int w, int h) {
+  if (d.y < 0) {
+    const float l = (float)((0.0 - (double)pt.y) / (double)d.y);
+    if (l >= 0) {
+      const P2 q{pt.x + l * d.x, pt.y + l * d.y};
+      if (0 <= trunc_i(q.x) && trunc_i(q.x) <= w - 1) return q;
+    }
+  }
+  if (d.y > 0) {
+    const float l = (float)(((double)h - 1.0 - (double)pt.y) / (double)d.y);
+    if (l >= 0) {
+      const P2 q{pt.x + l * d.x, pt.y + l * d.y};
+      if (0 <= trunc_i(q.x) && trunc_i(q.x) <= w - 1) return q;
+    }
+  }
+  if (d.x > 0) {
+    const float l = (float)(((double)w - 1.0 - (double)pt.x) / (double)d.x);
+    if (l >= 0) {
+      const P2 q{pt.x + l * d.x, pt.y + l * d.y};
+      if (0 <= trunc_i(q.y) && trunc_i(q.y) <= h - 1) return q;
+    }
+  }
+  if (d.x < 0) {
+    const float l = (float)((0.0 - (double)pt.x) / (double)d.x);
+    if (l >= 0) {
+      const P2 q{pt.x + l * d.x, pt.y + l * d.y};
+      if (0 <= trunc_i(q.y) && trunc_i(q.y) <= h - 1) return q;
+    }
+  }
+  return P2{-1.f, -1.f};
+}
+
+// A (p, 1) for a row-major 4x4 A, divided by its fourth component (homo_to_real_coord)
+__device__ __forceinline__ P3 xform(const float* A, P3 p) {
+  float h[4];
+#pragma unroll
+  for (int i = 0; i < 4; i++) h[i] = A[i * 4 + 0] * p.x + A[i * 4 + 1] * p.y + A[i * 4 + 2] * p.z + A[i * 4 + 3] * 1.0f;
+  return P3{h[0] / h[3], h[1] / h[3], h[2] / h[3]};
+}
+__device__ __forceinline__ P2 project(const float* K, P3 p) {
+  float q[3];
+#pragma unroll
+  for (int i = 0; i < 3; i++) q[i] = K[i * 3 + 0] * p.x + K[i * 3 + 1] * p.y + K[i * 3 + 2] * p.z;
+  return P2{q[0] / q[2], q[1] / q[2]};
+}
+__device__ __forceinline__ float norm3(P3 a) { return sqrtf(a.x * a.x + a.y * a.y + a.z * a.z); }
+
+// polygon_overlap_func: the hull of the corners inside both closed polygons and of their edges' crossings
+// (lineSegmentIntersect_f2); a has at most kWallMax vertices, b is the 5-vertex cut box
+__device__ int overlap(const P2* a, int na, const P2* b, int nb, P2* out) {
+  P2 sect[kHullMax], inside[kHullMax];
+  int ns = 0, ni = 0;
+  for (int i = 0; i + 1 < na; i++)
+    for (int j = 0; j + 1 < nb; j++) {
+      const float X2_X1 = a[i + 1].x - a[i].x, Y2_Y1 = a[i + 1].y - a[i].y;
+      const float X4_X3 = b[j + 1].x - b[j].x, Y4_Y3 = b[j + 1].y - b[j].y;
+      const float X1_X3 = a[i].x - b[j].x, Y1_Y3 = a[i].y - b[j].y;
+      const float ua = (X4_X3 * Y1_Y3 - Y4_Y3 * X1_X3) / (Y4_Y3 * X2_X1 - X4_X3 * Y2_Y1);
+      const float ub = (X2_X1 * Y1_Y3 - Y2_Y1 * X1_X3) / (Y4_Y3 * X2_X1 - X4_X3 * Y2_Y1);
+      const float ix = a[i].x + X2_X1 * ua, iy = a[i].y + Y2_Y1 * ua;
+      const float ib = (float)((ua >= 0) && (ua <= 1) && (ub >= 0) && (ub <= 1));
+      if ((ua >= 0) && (ua <= 1) && (ub >= 0) && (ub <= 1)) sect[ns++] = P2{ix * ib, iy * ib};
+    }
+  for (int k = 0; k < (na - 1) + (nb - 1); k++) {
+    const P2 c = k < na - 1 ? a[k] : b[k - (na - 1)];
+    if (point_polygon_test(a, na, c) >= 0 && point_polygon_test(b, nb, c) >= 0) inside[ni++] = c;
+  }
+  for (int k = 0; k < ns; k++) inside[ni++] = sect[k];
+  return convex_hull(inside, ni, out);
+}
+
+// find_correct_ground_seq; 0 = none.  Where the reference would index past its hull (one of the two ground vertices
+// missing and the other not next to the wrap) this also returns 0, i.e. the uncut polygon.
+__device__ int ground_seq(const P2* q, int n, bool originkept, int* seq) {
+  int first = -1, second = -1;
+  for (int i = 0; i < n; i++)
+    if ((double)fabsf(q[i].y) < 1e-3) {
+      if (originkept) {
+        if ((double)fabsf(q[i].x) < 1e-3) first = i;
+        else second = i;
+      } else {
+        if (first == -1) first = i;
+        else second = i;
+      }
+    }
+  if (!(abs(first - second) == 1 || abs(first - second) == n - 1)) return 0;
+  int inc = second - first;
+  if (first == 0 && second == n - 1) inc = -1;
+  if (first == n - 1 && second == 0) inc = 1;
+  for (int j = 0; j < n + 1; j++) {
+    int cur = first + j * inc;
+    if (cur > n - 1) cur -= n;
+    if (cur < 0) cur += n;
+    if (cur < 0 || cur > n - 1) return 0;
+    seq[j] = cur;
+  }
+  return n + 1;
+}
+
+// cut_wall_polygons (matrix_utils.cpp:642-713): the wall polygon P (world frame, closed) cut to the box of height
+// [-1, ceiling] and, with walllength >= 0, of that length from the ground endpoint nearer the camera
+__device__ int cut_wall(const P3* P, int m, float ceiling, float walllength, P3 cam, P3* out) {
+  const P3 d{P[1].x - P[0].x, P[1].y - P[0].y, P[1].z - P[0].z};
+  const float z = d.x * d.x + d.y * d.y + d.z * d.z;
+  P3 dir = d;
+  if (z > 0) {   // Eigen's normalized()
+    const float s = sqrtf(z);
+    dir = P3{d.x / s, d.y / s, d.z / s};
+  }
+  const float L = norm3(d);
+  P2 poly[kWallMax];
+  for (int i = 0; i < m; i++) {
+    const P3 r{P[i].x - P[0].x, P[i].y - P[0].y, P[i].z - P[0].z};
+    poly[i] = P2{r.x * dir.x + r.y * dir.y + r.z * dir.z, P[i].z};
+  }
+  const bool height_only = walllength < 0;
+  float x0 = -1.f, x1 = L + 1;
+  if (!height_only) {
+    const float s0 = norm3(P3{cam.x - P[0].x, cam.y - P[0].y, cam.z - P[0].z});
+    const float s1 = norm3(P3{cam.x - P[1].x, cam.y - P[1].y, cam.z - P[1].z});
+    if (s0 < s1) {
+      x1 = walllength;
+    } else {
+      x0 = poly[1].x - walllength;
+      x1 = poly[1].x + 1;
+    }
+  }
+  const P2 box[5] = {{x0, -1.f}, {x1, -1.f}, {x1, ceiling}, {x0, ceiling}, {x0, -1.f}};
+  P2 hull[kHullMax];
+  const int nh = overlap(poly, m, box, 5, hull);
+  int seq[kCutSlot];
+  const int ns = ground_seq(hull, nh, height_only, seq);
+  if (ns == 0) {   // the reference prints "BAD cut_wall_polygons1" and keeps the uncut polygon
+    for (int i = 0; i < m; i++) out[i] = P[i];
+    return m;
+  }
+  for (int i = 0; i < ns; i++) {
+    const P2 h = hull[seq[i]];
+    out[i] = P3{(P[0].x + h.x * dir.x) + h.y * 0.f, (P[0].y + h.x * dir.y) + h.y * 0.f, (P[0].z + h.x * dir.z) + h.y * 1.f};
+  }
+  return ns;
+}
+
+struct Params {
+  const int* seg_ptr;
+  const int* row_frame;
+  int n_rows;
+  const float* segs;
+  const float* K;
+  const float* invK;
+  const float* Ts;
+  const float* planes;   // [n_rows][4] sensor frame, from popup_kernel
+  const float* ends;     // [n_rows][6] world ground endpoints of the wall rows, from popup_kernel
+  int width, height;
+  float ceiling, walllength;
+  float* bound;          // [n_rows][kBoundSlot][2]
+  float* cut;            // [n_rows][kCutSlot][2]
+  float* world;          // [n_rows][kCutSlot][3]
+  int* counts;           // [3][n_rows]: bound, cut, world
+};
+
+// the up image direction of a world vertical at ground endpoint k of the frame's segment s (popup_plane.cpp:127-143)
+__device__ P2 up_direction(const Params& P, const float* K, const float* iT, int row_of_seg, int k) {
+  const float* e = P.ends + (size_t)row_of_seg * 6 + 3 * k;
+  const P3 v0{e[0], e[1], e[2]}, v1{e[0] + 0.f, e[1] + 0.f, e[2] + 2.f};
+  const P2 i0 = project(K, xform(iT, v0)), i1 = project(K, xform(iT, v1));
+  P2 dir{i1.x - i0.x, i1.y - i0.y};
+  if (dir.y > 0) dir = P2{-dir.x, -dir.y};
+  return dir;
+}
+
+__global__ void polygon_kernel(Params P) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= P.n_rows) return;
+  const int f = P.row_frame[row];
+  const int s0 = P.seg_ptr[f];
+  const int n = P.seg_ptr[f + 1] - s0;
+  const int j = row - (s0 + f);
+  int* cnt = P.counts;
+  if (n <= 0) {
+    cnt[row] = cnt[P.n_rows + row] = cnt[2 * P.n_rows + row] = 0;
+    return;
+  }
+  float T[16], K[9], iT[16];
+#pragma unroll
+  for (int i = 0; i < 16; i++) T[i] = P.Ts[(size_t)f * 16 + i];
+#pragma unroll
+  for (int i = 0; i < 9; i++) K[i] = P.K[i];
+  // the camera inverse in closed form, [R^T | -R^T t]
+#pragma unroll
+  for (int i = 0; i < 3; i++) {
+#pragma unroll
+    for (int c = 0; c < 3; c++) iT[i * 4 + c] = T[c * 4 + i];
+    iT[i * 4 + 3] = -(T[0 * 4 + i] * T[3] + T[1 * 4 + i] * T[7] + T[2 * 4 + i] * T[11]);
+  }
+  iT[12] = 0.f; iT[13] = 0.f; iT[14] = 0.f; iT[15] = 1.f;
+  const float W1 = (float)(P.width - 1), H1 = (float)(P.height - 1);
+  const float* S = P.segs + (size_t)s0 * 4;
+  float* B = P.bound + (size_t)row * kBoundSlot * 2;
+  int nb = 0;
+  auto push = [&](P2 q) { B[2 * nb] = q.x; B[2 * nb + 1] = q.y; nb++; };
+  if (j == 0) {   // ground polygon (popup_plane.cpp:158-196)
+    for (int s = 0; s < n; s++) push(P2{S[4 * s], S[4 * s + 1]});
+    const float* l = S + 4 * (n - 1);
+    push(P2{l[2], l[3]});
+    if (l[3] == H1 && l[2] < W1) {
+    } else if (l[2] == W1 && l[3] <= H1) {
+      push(P2{W1, H1});
+    } else {
+      const P2 u = up_direction(P, K, iT, s0 + f + n, 1);
+      const P2 eh = hit_boundary(P2{l[2], l[3]}, P2{-u.x, -u.y}, P.width, P.height);
+      if (eh.x == W1) { push(eh); push(P2{W1, H1}); }
+      if (0 <= eh.x && eh.x < W1) push(eh);
+    }
+    const float* g = S;
+    if (g[1] == H1 && g[0] > 0) {
+    } else if (g[0] == 0 && g[1] <= H1) {
+      push(P2{0.f, H1});
+    } else {
+      const P2 ub = up_direction(P, K, iT, s0 + f + 1, 0), ue = up_direction(P, K, iT, s0 + f + 1, 1);
+      const P2 bh = hit_boundary(P2{g[0], g[1]}, P2{-ub.x, -ub.y}, P.width, P.height);
+      const P2 eh = hit_boundary(P2{g[2], g[3]}, P2{-ue.x, -ue.y}, P.width, P.height);
+      if (bh.x == W1) { push(P2{0.f, H1}); push(eh); }   // the reference pushes the end's hit in both cases
+      if (0 <= bh.x && bh.x < W1) push(eh);
+    }
+    push(P2{B[0], B[1]});
+    cnt[row] = nb;
+    cnt[P.n_rows + row] = nb;   // the cut polygon of the ground is its bound polygon, packed from the bound slot
+    cnt[2 * P.n_rows + row] = 0;
+    return;
+  }
+  // wall polygon (popup_plane.cpp:198-344)
+  const int s = j - 1;
+  const float* g = S + 4 * s;
+  P2 p[kWallMax];
+  int m = 0;
+  p[m++] = P2{g[0], g[1]};
+  p[m++] = P2{g[2], g[3]};
+  const P2 ub = up_direction(P, K, iT, row, 0), ue = up_direction(P, K, iT, row, 1);
+  const P2 bh = hit_boundary(P2{g[0], g[1]}, ub, P.width, P.height);
+  const P2 eh = hit_boundary(P2{g[2], g[3]}, ue, P.width, P.height);
+  auto general = [&]() {
+    if (bh.x == W1 && eh.x == W1) { p[m++] = eh; p[m++] = bh; }
+    if (0 < bh.x && bh.x < W1 && eh.x == W1) { p[m++] = eh; p[m++] = P2{W1, 0.f}; p[m++] = bh; }
+    if (0 < bh.x && bh.x < W1 && 0 < eh.x && eh.x < W1) { p[m++] = eh; p[m++] = bh; }
+    if (bh.x == 0 && 0 < eh.x && eh.x < W1) { p[m++] = eh; p[m++] = P2{0.f, 0.f}; p[m++] = bh; }
+    if (bh.x == 0 && eh.x == 0) { p[m++] = eh; p[m++] = bh; }
+  };
+  auto right_begin = [&]() {
+    if (bh.x == W1) p[m++] = bh;
+    if (0 < bh.x && bh.x < W1) { p[m++] = P2{W1, 0.f}; p[m++] = bh; }
+    if (bh.x == 0) { p[m++] = P2{W1, 0.f}; p[m++] = P2{0.f, 0.f}; p[m++] = bh; }
+  };
+  auto left_end = [&]() {
+    if (eh.x == W1) { p[m++] = eh; p[m++] = P2{W1, 0.f}; p[m++] = P2{0.f, 0.f}; }
+    if (0 < eh.x && eh.x < W1) { p[m++] = eh; p[m++] = P2{0.f, 0.f}; }
+    if (eh.x == 0) p[m++] = eh;
+  };
+  if (s == n - 1) {   // rightmost
+    if (g[3] == H1 && g[2] < W1) { p[m++] = P2{W1, H1}; right_begin(); }
+    else if (g[2] == W1 && g[3] <= H1) right_begin();
+    else general();
+  } else if (0 < s && s < n - 1) {
+    general();
+  } else {            // leftmost
+    if (g[1] == H1 && g[0] > 0) { left_end(); p[m++] = P2{0.f, H1}; }
+    else if (g[0] == 0 && g[1] <= H1) left_end();
+    else general();
+  }
+  p[m++] = P2{g[0], g[1]};
+  for (int i = 0; i < m; i++) push(p[i]);
+  // onto the wall plane, to the world frame, cut, and back into the image (popup_plane.cpp:346-404)
+  float invK[9], pl[4];
+#pragma unroll
+  for (int i = 0; i < 9; i++) invK[i] = P.invK[i];
+#pragma unroll
+  for (int i = 0; i < 4; i++) pl[i] = P.planes[(size_t)row * 4 + i];
+  P3 Q[kWallMax];
+  for (int i = 0; i < m; i++) {
+    float ray[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) ray[k] = invK[k * 3 + 0] * p[i].x + invK[k * 3 + 1] * p[i].y + invK[k * 3 + 2] * 1.0f;
+    const float frac = -pl[3] / (pl[0] * ray[0] + pl[1] * ray[1] + pl[2] * ray[2]);
+    Q[i] = xform(T, P3{frac * ray[0], frac * ray[1], frac * ray[2]});
+  }
+  Q[0].z = 0.f;
+  Q[1].z = 0.f;
+  P3 out[kCutSlot];
+  const int nc = cut_wall(Q, m, P.ceiling, P.walllength, P3{T[3], T[7], T[11]}, out);
+  float* C = P.cut + (size_t)row * kCutSlot * 2;
+  float* Wd = P.world + (size_t)row * kCutSlot * 3;
+  for (int i = 0; i < nc; i++) {
+    const P2 q = project(K, xform(iT, out[i]));
+    C[2 * i] = q.x; C[2 * i + 1] = q.y;
+    Wd[3 * i] = out[i].x; Wd[3 * i + 1] = out[i].y; Wd[3 * i + 2] = out[i].z;
+  }
+  cnt[row] = nb;
+  cnt[P.n_rows + row] = nc;
+  cnt[2 * P.n_rows + row] = nc;
+}
+
+// pack every row's slots at its offsets (off[3][n_rows], exclusive scans of the counts); the ground's cut polygon is its
+// bound polygon
+__global__ void pack_kernel(int n_rows, const int* row_frame, const int* seg_ptr, const int* counts, const long long* off,
+                            const float* bound, const float* cut, const float* world, float* ob, float* oc, float* ow) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= n_rows) return;
+  const int f = row_frame[row];
+  const bool ground = row == seg_ptr[f] + f;
+  const float* b = bound + (size_t)row * kBoundSlot * 2;
+  if (ob)
+    for (int i = 0; i < 2 * counts[row]; i++) ob[2 * off[row] + i] = b[i];
+  if (oc) {
+    const float* c = ground ? b : cut + (size_t)row * kCutSlot * 2;
+    for (int i = 0; i < 2 * counts[n_rows + row]; i++) oc[2 * off[n_rows + row] + i] = c[i];
+  }
+  if (ow)
+    for (int i = 0; i < 3 * counts[2 * n_rows + row]; i++) ow[3 * off[2 * n_rows + row] + i] = world[(size_t)row * kCutSlot * 3 + i];
+}
+}  // namespace poly
+}  // namespace pus
+
+#define GCHK(call)                                                                                          \
+  do {                                                                                                      \
+    cudaError_t e__ = (call);                                                                               \
+    if (e__ != cudaSuccess) { g_err = std::string("pus_popup_polygons: ") + #call + ": " + cudaGetErrorString(e__); return -1; } \
+  } while (0)
+
+extern "C" int pus_popup_polygons(int device, int n_frames, const int* seg_ptr, const float* segs, const float* K,
+                                  const float* invK, const float* Ts, int width, int height, float ceiling_threshold,
+                                  float walllength_threshold, int* bound_counts, int* cut_counts, int* world_counts,
+                                  float* bound2d, float* cut2d, float* world3d, long long bound_capacity,
+                                  long long cut_capacity, long long world_capacity) {
+  using namespace pus::poly;
+  auto refuse = [](const char* why) { g_err = std::string("pus_popup_polygons: ") + why; return -1; };
+  auto finite = [](const float* a, size_t n) {
+    for (size_t i = 0; i < n; i++)
+      if (!std::isfinite(a[i])) return false;
+    return true;
+  };
+  if (n_frames < 0) return refuse("n_frames < 0");
+  if (!seg_ptr || seg_ptr[0] != 0) return refuse("seg_ptr must be given and start at 0");
+  for (int f = 0; f < n_frames; f++) {
+    const int n = seg_ptr[f + 1] - seg_ptr[f];
+    if (n < 0) return refuse("seg_ptr is not ascending");
+    if (n > PUS_POPUP_MAX_SEGMENTS) return refuse("a frame has more than PUS_POPUP_MAX_SEGMENTS segments");
+  }
+  if (width < 2 || height < 2) return refuse("width and height must be at least 2");
+  const int n_seg = seg_ptr[n_frames];
+  const int n_rows = n_seg + n_frames;
+  if (n_seg > 0 && !segs) return refuse("segs must be given");
+  for (long long i = 0; i < 4LL * n_seg; i++)
+    if (!(std::fabs(segs[i]) <= PUS_POPUP_MAX_COORD)) return refuse("a segment coordinate is not finite or exceeds PUS_POPUP_MAX_COORD");
+  if (!K || !invK || !finite(K, 9) || !finite(invK, 9)) return refuse("K and invK must be given and finite");
+  if (n_frames > 0 && (!Ts || !finite(Ts, (size_t)n_frames * 16))) return refuse("Ts must be given and finite");
+  if (!bound_counts || !cut_counts || !world_counts) return refuse("the count arrays must be given");
+  if (n_frames == 0) return 0;
+  std::vector<int> rf(n_rows);
+  for (int f = 0; f < n_frames; f++)
+    for (int r = seg_ptr[f] + f; r < seg_ptr[f + 1] + f + 1; r++) rf[r] = f;
+  {
+    int ndev = 0;
+    cudaError_t de = cudaGetDeviceCount(&ndev);
+    if (de != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
+      return refuse("no CUDA device usable; libpopup_gpu has no CPU fallback");
+  }
+  GCHK(cudaSetDevice(device));
+  DevBuf<int> d_ptr, d_rf, d_cnt;
+  DevBuf<float> d_segs, d_K, d_iK, d_T, d_pl, d_ends, d_b, d_c, d_w, d_ob, d_oc, d_ow;
+  DevBuf<long long> d_off;
+  GCHK(d_ptr.alloc(n_frames + 1));
+  GCHK(d_rf.alloc(n_rows));
+  GCHK(d_segs.alloc((size_t)n_seg * 4));
+  GCHK(d_K.alloc(9));
+  GCHK(d_iK.alloc(9));
+  GCHK(d_T.alloc((size_t)n_frames * 16));
+  GCHK(d_pl.alloc((size_t)n_rows * 4));
+  GCHK(d_ends.alloc((size_t)n_rows * 6));
+  GCHK(d_b.alloc((size_t)n_rows * kBoundSlot * 2));
+  GCHK(d_c.alloc((size_t)n_rows * kCutSlot * 2));
+  GCHK(d_w.alloc((size_t)n_rows * kCutSlot * 3));
+  GCHK(d_cnt.alloc((size_t)n_rows * 3));
+  GCHK(d_off.alloc((size_t)n_rows * 3));
+  GCHK(cudaMemcpy(d_ptr.p, seg_ptr, (n_frames + 1) * sizeof(int), cudaMemcpyHostToDevice));
+  GCHK(cudaMemcpy(d_rf.p, rf.data(), n_rows * sizeof(int), cudaMemcpyHostToDevice));
+  if (n_seg > 0) GCHK(cudaMemcpy(d_segs.p, segs, (size_t)n_seg * 4 * sizeof(float), cudaMemcpyHostToDevice));
+  GCHK(cudaMemcpy(d_K.p, K, 9 * sizeof(float), cudaMemcpyHostToDevice));
+  GCHK(cudaMemcpy(d_iK.p, invK, 9 * sizeof(float), cudaMemcpyHostToDevice));
+  GCHK(cudaMemcpy(d_T.p, Ts, (size_t)n_frames * 16 * sizeof(float), cudaMemcpyHostToDevice));
+  // the planes and the world ground endpoints: get_plane_equation, as pus_popup_fit_frames runs it (mode 0)
+  popup_kernel<<<(n_rows + 255) / 256, 256>>>(n_frames, d_ptr.p, d_rf.p, n_rows, d_segs.p, d_iK.p, d_T.p, 0.f, 0, nullptr,
+                                               d_pl.p, nullptr, nullptr, d_ends.p);
+  GCHK(cudaGetLastError());
+  Params P{d_ptr.p, d_rf.p, n_rows, d_segs.p, d_K.p, d_iK.p, d_T.p, d_pl.p, d_ends.p, width, height, ceiling_threshold,
+           walllength_threshold, d_b.p, d_c.p, d_w.p, d_cnt.p};
+  polygon_kernel<<<(n_rows + 127) / 128, 128>>>(P);
+  GCHK(cudaGetLastError());
+  std::vector<int> cnt((size_t)n_rows * 3);
+  GCHK(cudaMemcpy(cnt.data(), d_cnt.p, cnt.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  std::memcpy(bound_counts, cnt.data(), n_rows * sizeof(int));
+  std::memcpy(cut_counts, cnt.data() + n_rows, n_rows * sizeof(int));
+  std::memcpy(world_counts, cnt.data() + 2 * (size_t)n_rows, n_rows * sizeof(int));
+  // row offsets of the packed outputs, in row order
+  std::vector<long long> off((size_t)n_rows * 3);
+  long long tot[3] = {0, 0, 0};
+  for (int k = 0; k < 3; k++)
+    for (int r = 0; r < n_rows; r++) {
+      off[(size_t)k * n_rows + r] = tot[k];
+      tot[k] += cnt[(size_t)k * n_rows + r];
+    }
+  if ((bound2d && bound_capacity < tot[0]) || (cut2d && cut_capacity < tot[1]) || (world3d && world_capacity < tot[2]))
+    return refuse("a capacity is smaller than its number of vertices");
+  if (!bound2d && !cut2d && !world3d) return 0;   // size query
+  GCHK(cudaMemcpy(d_off.p, off.data(), off.size() * sizeof(long long), cudaMemcpyHostToDevice));
+  if (bound2d) GCHK(d_ob.alloc((size_t)tot[0] * 2));
+  if (cut2d) GCHK(d_oc.alloc((size_t)tot[1] * 2));
+  if (world3d) GCHK(d_ow.alloc((size_t)tot[2] * 3));
+  pack_kernel<<<(n_rows + 255) / 256, 256>>>(n_rows, d_rf.p, d_ptr.p, d_cnt.p, d_off.p, d_b.p, d_c.p, d_w.p, d_ob.p, d_oc.p, d_ow.p);
+  GCHK(cudaGetLastError());
+  if (bound2d && tot[0] > 0) GCHK(cudaMemcpy(bound2d, d_ob.p, (size_t)tot[0] * 2 * sizeof(float), cudaMemcpyDeviceToHost));
+  if (cut2d && tot[1] > 0) GCHK(cudaMemcpy(cut2d, d_oc.p, (size_t)tot[1] * 2 * sizeof(float), cudaMemcpyDeviceToHost));
+  if (world3d && tot[2] > 0) GCHK(cudaMemcpy(world3d, d_ow.p, (size_t)tot[2] * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+  GCHK(cudaDeviceSynchronize());
+  return 0;
 }
