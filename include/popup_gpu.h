@@ -325,6 +325,35 @@ int pus_popup_polygons(int device, int n_frames, const int* seg_ptr, const float
                        int* bound_counts, int* cut_counts, int* world_counts, float* bound2d, float* cut2d, float* world3d,
                        long long bound_capacity, long long cut_capacity, long long world_capacity);
 
+/* ---- pop-up depth map (float32) ------------------------------------------------------------------ */
+/* popup_plane::get_depth_map_good (PUW/libs/popup_plane.cpp:866-921), the depth init of the popped-up scene, batched over
+ * frames, on the device.  The inputs mean what they mean for pus_popup_clouds: plane_ptr[n_frames+1] the frames' good planes
+ * in order, poly_ptr / polys each plane's closed 2-D bound polygon (pus_popup_polygons' bound2d rows), planes_sensor their
+ * sensor-frame planes (pus_popup_fit_frames' planes_sensor rows), Ts camera-to-world, invK, the image size and downsample.
+ * Per frame the map starts at 0 and its planes are drawn in order, a later plane over an earlier one.  Each polygon's pixels
+ * are those of pus_popup_clouds (OpenCV 4.13's fillConvexPoly + findNonZero, halved and doubled in downsample mode).  Per
+ * pixel, ray = invK (x, y, 1), p_s = -d / (n . ray) ray, p_w = R p_s + t:
+ *   p_w.z < ceiling_threshold   write p_s.z, unless p_s.z < 0 (the pixel keeps its earlier value)
+ *   otherwise                   write the z of ray's hit on the ceiling plane T^T (0, 0, -1, ceiling_threshold), unless it
+ *                               is < 0
+ * The comparisons are the reference's: a NaN height takes the ceiling branch and a NaN depth under a finite height is written.
+ * With downsample the map of a frame with planes is then resized as the reference does: cv::resize 0.5x (INTER_LINEAR, which
+ * OpenCV runs as its area fast path at 0.5), convertTo x4, cv::resize 2x INTER_LINEAR, bit for bit as OpenCV 4.13's own code;
+ * width and height must then be even (the reference's round trip changes the size of an odd image).
+ * depth[n_frames][height][width] receives the maps.  Deterministic, no floating-point atomics: repeated calls and any split
+ * of the batch give the same bytes.  Refusals (malformed CSR offsets, more than PUS_POPUP_MAX_VERTICES vertices, a
+ * coordinate not finite or beyond PUS_POPUP_MAX_COORD, a non-positive size, odd sizes in downsample mode, no depth) fail with
+ * a message and launch nothing; there is no CPU fallback.  Deviations from the reference:
+ *   - pixels outside the image are not written (the reference writes out of bounds);
+ *   - a plane is skipped when the polygon passed in is empty (the reference tests its member all_closed_2d_bound_polygons but
+ *     fills from the argument);
+ *   - the ceiling plane is always formed from Ts and ceiling_threshold (the reference takes it as an argument);
+ *   - the resize follows OpenCV's own code, not the Intel IPP build that the pip wheels enable by default, whose 2x
+ *     INTER_LINEAR differs by up to 3 ulp. */
+int pus_popup_depth(int device, int n_frames, const int* plane_ptr, const int* poly_ptr, const float* polys,
+                    const float* planes_sensor, const float* Ts, const float* invK, int width, int height, int downsample,
+                    float ceiling_threshold, float* depth);
+
 /* ---- device-resident measurement refresh and polygon re-projection (SURVEY.md 8f.1) -------- */
 /* Mapper_mono::update_plane_measurement (pop_planar_slam/src/Mapping.cpp:590-607): after a solve every past
  * frame re-pops its wall planes from its ground segments with the frame's LATEST pose estimate

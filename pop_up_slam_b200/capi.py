@@ -733,3 +733,32 @@ def popup_polygons(lib, seg_ptr, segs, K, invK, Ts, width, height, ceiling_thres
         call(out, cap)
         res.update(bound=out[0][:tot[0]], cut=out[1][:tot[1]], world=out[2][:tot[2]])
     return res
+
+
+def popup_depth(lib, plane_ptr, poly_ptr, polys, planes_sensor, Ts, invK, width, height, downsample=True,
+                ceiling_threshold=2.8, prefix="pus_", device=0):
+    """popup_plane::get_depth_map_good batched over frames (pus_popup_depth, include/popup_gpu.h).
+
+    The inputs are popup_clouds': plane_ptr [n_frames+1] and poly_ptr [n_planes+1] CSR offsets, polys [n_vertices, 2] the
+    planes' closed 2-D bound polygons (popup_polygons' bound_ptr / bound of the good rows), planes_sensor [n_planes, 4],
+    Ts [n_frames, 4, 4] camera-to-world, invK [3, 3].  Returns the depth maps [n_frames, height, width] float32."""
+    plane_ptr = _i32(plane_ptr)
+    nf = len(plane_ptr) - 1
+    poly_ptr = _i32(poly_ptr)
+    polys = np.ascontiguousarray(polys, dtype=np.float32).reshape(-1, 2)
+    planes_sensor = np.ascontiguousarray(planes_sensor, dtype=np.float32).reshape(-1, 4)
+    Ts = np.ascontiguousarray(Ts, dtype=np.float32).reshape(nf, 4, 4)
+    invK = np.ascontiguousarray(invK, dtype=np.float32).reshape(3, 3)
+    out = np.empty((nf, int(height), int(width)), np.float32)
+    fn = getattr(lib, prefix + "popup_depth")
+    fn.restype = C.c_int
+    fn.argtypes = [C.c_int, C.c_int, c_int_p, c_int_p, c_float_p, c_float_p, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int,
+                   C.c_float, c_float_p]
+    err = getattr(lib, prefix + "last_error", None) or getattr(lib, prefix + "popup_last_error")
+    err.restype = C.c_char_p
+    rc = fn(device, nf, _ip(plane_ptr), _ip(poly_ptr), polys.ctypes.data_as(c_float_p), planes_sensor.ctypes.data_as(c_float_p),
+            Ts.ctypes.data_as(c_float_p), invK.ctypes.data_as(c_float_p), int(width), int(height), int(bool(downsample)),
+            float(ceiling_threshold), out.ctypes.data_as(c_float_p))
+    if rc < 0:
+        raise ApiError((err() or b"?").decode())
+    return out

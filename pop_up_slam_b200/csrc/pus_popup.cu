@@ -414,6 +414,18 @@ __device__ __forceinline__ bool member(int x, int2 sp, const int2* runs, int n) 
   return false;
 }
 
+// pixel (fx, fy) on plane pl: ray = invK (x, y, 1), p_s = -d / (n . ray) ray (ray_plane_interact), p_w = R p_s + t
+__device__ __forceinline__ void pixel_on_plane(const float* K, const float* T, const float* pl, float fx, float fy, float* ray,
+                                               float* ps, float* pw) {
+#pragma unroll
+  for (int i = 0; i < 3; i++) ray[i] = K[i * 3 + 0] * fx + K[i * 3 + 1] * fy + K[i * 3 + 2] * 1.0f;
+  const float frac = -pl[3] / (pl[0] * ray[0] + pl[1] * ray[1] + pl[2] * ray[2]);
+#pragma unroll
+  for (int i = 0; i < 3; i++) ps[i] = frac * ray[i];
+#pragma unroll
+  for (int i = 0; i < 3; i++) pw[i] = T[i * 4 + 0] * ps[0] + T[i * 4 + 1] * ps[1] + T[i * 4 + 2] * ps[2] + T[i * 4 + 3];
+}
+
 // COUNT: replay the scanline walk into span[], then count the kept points of every box row.
 // WRITE: write the kept points of every row at row_off[row] in pixel order.
 template <bool WRITE>
@@ -451,16 +463,8 @@ __global__ void __launch_bounds__(kThreads) cloud_kernel(Params P) {
       float pw[3] = {0.f, 0.f, 0.f};
       const int X = (J.bx + x) * P.scale, Y = (J.by + y) * P.scale;
       if (keep) {
-        const float fx = (float)X, fy = (float)Y;
-        float ray[3];
-#pragma unroll
-        for (int i = 0; i < 3; i++) ray[i] = K[i * 3 + 0] * fx + K[i * 3 + 1] * fy + K[i * 3 + 2] * 1.0f;
-        const float frac = -pl[3] / (pl[0] * ray[0] + pl[1] * ray[1] + pl[2] * ray[2]);
-        float ps[3];
-#pragma unroll
-        for (int i = 0; i < 3; i++) ps[i] = frac * ray[i];
-#pragma unroll
-        for (int i = 0; i < 3; i++) pw[i] = T[i * 4 + 0] * ps[0] + T[i * 4 + 1] * ps[1] + T[i * 4 + 2] * ps[2] + T[i * 4 + 3];
+        float ray[3], ps[3];
+        pixel_on_plane(K, T, pl, (float)X, (float)Y, ray, ps, pw);
         // matrixToCloud's filters, popup_plane.cpp:951-977 (-0.2 is a double literal there)
         keep = !(ps[2] < 0.f || ps[2] > P.depth_thre || (double)pw[2] < -0.2) && !(P.border && (X < 4 || Y < 4));
       }
@@ -547,6 +551,123 @@ __global__ void __launch_bounds__(kThreads) cloud_label_kernel(const int* plane_
     }
   }
 }
+
+// ---- pop-up depth map (pus_popup_depth) ----
+// per plane: its outline edges (into edges[v0 ..]) and the scanline walk into span[]
+__global__ void __launch_bounds__(128) depth_span_kernel(const Job* jobs, const int2* vtx, Edge* edges, int2* span) {
+  const Job J = jobs[blockIdx.x];
+  if (J.n <= 0) return;
+  for (int i = threadIdx.x; i < J.n; i += blockDim.x) edges[J.v0 + i] = make_edge(vtx + J.v0, J.n, i, J.bw, J.bh);
+  for (int y = threadIdx.x; y < J.bh; y += blockDim.x) span[J.row0 + y] = make_int2(1, 0);
+  __syncthreads();
+  if (threadIdx.x == 0) scan_spans(vtx + J.v0, J.n, J.bw, J.bh, span + J.row0);
+}
+
+constexpr int kChunk = 32 * 32;   // fill-space columns per pass of a warp: one bit per pixel in a lane's 32-bit mask
+
+// popup_plane.cpp:891-910 on the fill grid (the image, or its even pixels in downsample mode: scale 2), one warp per
+// (frame, fill row).  Last writer wins, so the warp walks the frame's planes from the last to the first and a pixel takes the
+// first value that passes; every pixel of out is written exactly once.
+__global__ void __launch_bounds__(kThreads) depth_kernel(int n_frames, const int* plane_ptr, const Job* jobs, const Edge* edges,
+                                                         const int2* spans, const float* planes, const float* Ts,
+                                                         const float* invK, int fw, int fh, int scale, float ceiling,
+                                                         float* out) {
+  __shared__ int2 runs[kWarps][PUS_POPUP_MAX_VERTICES];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long row = (long long)blockIdx.x * kWarps + warp;
+  if (row >= (long long)n_frames * fh) return;
+  const int f = (int)(row / fh), hy = (int)(row % fh);
+  float T[12], K[9], cs[4];
+#pragma unroll
+  for (int i = 0; i < 12; i++) T[i] = Ts[(size_t)f * 16 + i];
+#pragma unroll
+  for (int i = 0; i < 9; i++) K[i] = invK[i];
+  // ceiling_plane_sensor = T^T (0, 0, -1, c) (popup_plane.cpp:602-603), the four terms as popup_kernel forms the ground
+  const float cw[4] = {0.f, 0.f, -1.f, ceiling};
+#pragma unroll
+  for (int i = 0; i < 4; i++)
+    cs[i] = T[0 * 4 + i] * cw[0] + T[1 * 4 + i] * cw[1] + T[2 * 4 + i] * cw[2] + Ts[(size_t)f * 16 + 12 + i] * cw[3];
+  float* o = out + row * fw;
+  const int p0 = plane_ptr[f], p1 = plane_ptr[f + 1];
+  const float fY = (float)(hy * scale);
+  for (int c0 = 0; c0 < fw; c0 += kChunk) {
+    const int c1 = min(fw, c0 + kChunk);
+    const int nk = c1 - c0 - lane > 0 ? (c1 - c0 - lane + 31) >> 5 : 0;   // this lane's pixels in the chunk
+    const unsigned full = nk >= 32 ? 0xffffffffu : (1u << nk) - 1u;
+    unsigned taken = 0;
+    for (int p = p1 - 1; p >= p0 && !__all_sync(0xffffffffu, taken == full); p--) {
+      const Job J = jobs[p];
+      const int y = hy - J.by;
+      if (J.n <= 0 || y < 0 || y >= J.bh || J.bx >= c1 || J.bx + J.bw <= c0) continue;
+      const int2 sp = spans[J.row0 + y];
+      const int2 range = row_setup(edges + J.v0, J.n, sp, y, runs[warp], lane);
+      if (range.x > range.y) continue;
+      const int lo = max(range.x + J.bx, c0), hi = min(range.y + J.bx, c1 - 1);
+      float pl[4];
+#pragma unroll
+      for (int i = 0; i < 4; i++) pl[i] = planes[(size_t)p * 4 + i];
+      for (int x0 = c0 + ((lo - c0) & ~31); x0 <= hi; x0 += 32) {
+        const int x = x0 + lane;
+        const unsigned bit = 1u << ((x0 - c0) >> 5);
+        if (x < lo || x > hi || (taken & bit) || !member(x - J.bx, sp, runs[warp], J.n)) continue;
+        float ray[3], ps[3], pw[3];
+        pixel_on_plane(K, T, pl, (float)(x * scale), fY, ray, ps, pw);
+        float v;
+        if (pw[2] < ceiling) {
+          if (ps[2] < 0) continue;
+          v = ps[2];
+        } else {   // ray_plane_interact(ray, ceiling_plane_sensor), its z
+          v = -cs[3] / (cs[0] * ray[0] + cs[1] * ray[1] + cs[2] * ray[2]) * ray[2];
+          if (v < 0) continue;
+        }
+        o[x] = v;
+        taken |= bit;
+      }
+      __syncwarp();
+    }
+    for (int k = 0; k < nk; k++)
+      if (!(taken & (1u << k))) o[c0 + lane + 32 * k] = 0.f;
+  }
+}
+
+// downsample mode (popup_plane.cpp:912-916): cv::resize 0.5x (INTER_LINEAR at 0.5 is OpenCV's area fast path), convertTo x4,
+// cv::resize 2x INTER_LINEAR, as OpenCV 4.13's own code computes them (not the IPP build).  half holds the full map's even
+// pixels; its odd pixels are 0, as no written pixel is odd (so the area path's pairwise SIMD sum and its left-to-right scalar
+// tail agree).  One thread per output pixel; each recomputes the horizontal pass of its two source rows, so the result is
+// the separable one.
+__device__ __forceinline__ float depth_quarter(const float* half, int hw, int r, int c) {
+  const float s = ((half[(size_t)r * hw + c] + 0.f) + (0.f + 0.f)) * 0.25f;
+  return s * 4.f + 0.f;
+}
+
+// the horizontal 2x pass at output column dx of half-size row r: left border (1 - 0) x S[0] + 0 x S[1], right border S[w-1]
+// (a one-column source has only the single-term border)
+__device__ __forceinline__ float depth_hpass(const float* half, int hw, int r, int dx) {
+  const int j = dx >> 1;
+  if (dx == 2 * hw - 1 || hw == 1) return depth_quarter(half, hw, r, hw - 1) * 1.f;
+  if (dx == 0) return depth_quarter(half, hw, r, 0) * 1.f + depth_quarter(half, hw, r, 1) * 0.f;
+  const int sx = (dx & 1) ? j : j - 1;
+  const float w0 = (dx & 1) ? 0.75f : 0.25f, w1 = (dx & 1) ? 0.25f : 0.75f;
+  return depth_quarter(half, hw, r, sx) * w0 + depth_quarter(half, hw, r, sx + 1) * w1;
+}
+
+__global__ void depth_resize_kernel(int n_frames, const float* half, int width, int height, float* out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long wh = (long long)width * height;
+  if (i >= (long long)n_frames * wh) return;
+  const int f = (int)(i / wh), Y = (int)(i % wh / width), X = (int)(i % width);
+  const int hw = width / 2, hh = height / 2;
+  const float* H = half + (size_t)f * hw * hh;
+  float v;
+  if (Y == 0 || Y == height - 1) {   // the border rows take one source row
+    v = depth_hpass(H, hw, Y == 0 ? 0 : hh - 1, X) * 1.f;
+  } else {
+    const int sy = (Y & 1) ? Y >> 1 : (Y >> 1) - 1;
+    const float w0 = (Y & 1) ? 0.75f : 0.25f, w1 = (Y & 1) ? 0.25f : 0.75f;
+    v = depth_hpass(H, hw, sy, X) * w0 + depth_hpass(H, hw, sy + 1, X) * w1;
+  }
+  out[i] = v;
+}
 }  // namespace cloud
 }  // namespace pus
 
@@ -557,25 +678,15 @@ struct DevBuf {   // a device allocation freed on every return path
   ~DevBuf() { cudaFree(p); }
   cudaError_t alloc(size_t n) { return cudaMalloc(&p, (n > 0 ? n : 1) * sizeof(T)); }
 };
-}  // namespace
 
-#define CCHK(call)                                                                                        \
-  do {                                                                                                    \
-    cudaError_t e__ = (call);                                                                             \
-    if (e__ != cudaSuccess) { g_err = std::string("pus_popup_clouds: ") + #call + ": " + cudaGetErrorString(e__); return -1; } \
-  } while (0)
-
-extern "C" long long pus_popup_clouds(int device, int n_frames, const int* plane_ptr, const int* poly_ptr, const float* polys,
-                                      const float* planes_sensor, const float* Ts, const float* invK,
-                                      const unsigned char* images, int width, int height, int downsample, float depth_thre,
-                                      float ceiling_threshold, int* counts, long long* offsets, float* xyz, unsigned char* rgb,
-                                      long long capacity, unsigned char* labels) {
-  using namespace pus::cloud;
-  auto refuse = [](const char* why) { g_err = std::string("pus_popup_clouds: ") + why; return -1LL; };
-  if (n_frames < 0) return refuse("n_frames < 0");
-  if (!plane_ptr || plane_ptr[0] != 0) return refuse("plane_ptr must be given and start at 0");
-  if (width <= 0 || height <= 0) return refuse("width and height must be positive");
-  if (labels && downsample && ((width | height) & 1)) return refuse("label images in downsample mode need an even width and height");
+// The planes' polygon arguments of pus_popup_clouds and pus_popup_depth, checked, and per polygon matrix_to_points'
+// truncation, boundingRect and the box-shifted vertices (popup_plane.cpp:85-96).  Returns the number of box rows in all, or
+// -1 with g_err set (prefixed by who).
+long long plane_jobs(const char* who, int n_frames, const int* plane_ptr, const int* poly_ptr, const float* polys,
+                     const float* planes_sensor, const float* Ts, const float* invK, int downsample,
+                     std::vector<pus::cloud::Job>& jobs, std::vector<int2>& vtx) {
+  using pus::cloud::Job;
+  auto refuse = [&](const char* why) { g_err = std::string(who) + why; return -1LL; };
   for (int f = 0; f < n_frames; f++)
     if (plane_ptr[f + 1] < plane_ptr[f]) return refuse("plane_ptr is not ascending");
   const int n_planes = plane_ptr[n_frames];
@@ -591,10 +702,8 @@ extern "C" long long pus_popup_clouds(int device, int n_frames, const int* plane
   if (n_vtx > 0 && !polys) return refuse("polys must be given");
   for (int i = 0; i < 2 * n_vtx; i++)
     if (!(std::fabs(polys[i]) <= PUS_POPUP_MAX_COORD)) return refuse("a polygon coordinate is not finite or exceeds PUS_POPUP_MAX_COORD");
-
-  // per polygon: matrix_to_points' truncation, boundingRect, and the box-shifted vertices (popup_plane.cpp:85-96)
-  std::vector<Job> jobs(n_planes);
-  std::vector<int2> vtx(n_vtx);
+  jobs.assign(n_planes, Job{});
+  vtx.assign(n_vtx, int2{});
   long long rows = 0;
   for (int f = 0; f < n_frames; f++)
     for (int p = plane_ptr[f]; p < plane_ptr[f + 1]; p++) {
@@ -614,6 +723,33 @@ extern "C" long long pus_popup_clouds(int device, int n_frames, const int* plane
       rows += J.bh;
       if (rows > INT_MAX / 2) return refuse("the polygons' bounding boxes have too many rows in all");
     }
+  return rows;
+}
+}  // namespace
+
+#define CCHK(call)                                                                                        \
+  do {                                                                                                    \
+    cudaError_t e__ = (call);                                                                             \
+    if (e__ != cudaSuccess) { g_err = std::string("pus_popup_clouds: ") + #call + ": " + cudaGetErrorString(e__); return -1; } \
+  } while (0)
+
+extern "C" long long pus_popup_clouds(int device, int n_frames, const int* plane_ptr, const int* poly_ptr, const float* polys,
+                                      const float* planes_sensor, const float* Ts, const float* invK,
+                                      const unsigned char* images, int width, int height, int downsample, float depth_thre,
+                                      float ceiling_threshold, int* counts, long long* offsets, float* xyz, unsigned char* rgb,
+                                      long long capacity, unsigned char* labels) {
+  using namespace pus::cloud;
+  auto refuse = [](const char* why) { g_err = std::string("pus_popup_clouds: ") + why; return -1LL; };
+  if (n_frames < 0) return refuse("n_frames < 0");
+  if (!plane_ptr || plane_ptr[0] != 0) return refuse("plane_ptr must be given and start at 0");
+  if (width <= 0 || height <= 0) return refuse("width and height must be positive");
+  if (labels && downsample && ((width | height) & 1)) return refuse("label images in downsample mode need an even width and height");
+  std::vector<Job> jobs;
+  std::vector<int2> vtx;
+  const long long rows = plane_jobs("pus_popup_clouds: ", n_frames, plane_ptr, poly_ptr, polys, planes_sensor, Ts, invK,
+                                    downsample, jobs, vtx);
+  if (rows < 0) return -1;
+  const int n_planes = (int)jobs.size(), n_vtx = (int)vtx.size();
   {
     int ndev = 0;
     cudaError_t de = cudaGetDeviceCount(&ndev);
@@ -683,6 +819,76 @@ extern "C" long long pus_popup_clouds(int device, int n_frames, const int* plane
   }
   CCHK(cudaDeviceSynchronize());
   return total;
+}
+
+#define DCHK(call)                                                                                        \
+  do {                                                                                                    \
+    cudaError_t e__ = (call);                                                                             \
+    if (e__ != cudaSuccess) { g_err = std::string("pus_popup_depth: ") + #call + ": " + cudaGetErrorString(e__); return -1; } \
+  } while (0)
+
+extern "C" int pus_popup_depth(int device, int n_frames, const int* plane_ptr, const int* poly_ptr, const float* polys,
+                               const float* planes_sensor, const float* Ts, const float* invK, int width, int height,
+                               int downsample, float ceiling_threshold, float* depth) {
+  using namespace pus::cloud;
+  auto refuse = [](const char* why) { g_err = std::string("pus_popup_depth: ") + why; return -1; };
+  if (n_frames < 0) return refuse("n_frames < 0");
+  if (!plane_ptr || plane_ptr[0] != 0) return refuse("plane_ptr must be given and start at 0");
+  if (width <= 0 || height <= 0) return refuse("width and height must be positive");
+  if (downsample && ((width | height) & 1)) return refuse("downsample mode needs an even width and height");
+  if (!depth) return refuse("depth must be given");
+  std::vector<Job> jobs;
+  std::vector<int2> vtx;
+  const long long rows = plane_jobs("pus_popup_depth: ", n_frames, plane_ptr, poly_ptr, polys, planes_sensor, Ts, invK,
+                                    downsample, jobs, vtx);
+  if (rows < 0) return -1;
+  const int n_planes = (int)jobs.size(), n_vtx = (int)vtx.size();
+  {
+    int ndev = 0;
+    cudaError_t de = cudaGetDeviceCount(&ndev);
+    if (de != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
+      return refuse("no CUDA device usable; libpopup_gpu has no CPU fallback");
+  }
+  if (n_frames == 0) return 0;
+  DCHK(cudaSetDevice(device));
+  const int scale = downsample ? 2 : 1, fw = width / scale, fh = height / scale;
+  const size_t out_n = (size_t)n_frames * width * height, fill_n = (size_t)n_frames * fw * fh;
+  DevBuf<Job> d_jobs;
+  DevBuf<int2> d_vtx, d_span;
+  DevBuf<Edge> d_edges;
+  DevBuf<float> d_planes, d_T, d_K, d_fill, d_out;
+  DevBuf<int> d_ptr;
+  DCHK(d_jobs.alloc(n_planes));
+  DCHK(d_vtx.alloc(n_vtx));
+  DCHK(d_edges.alloc(n_vtx));
+  DCHK(d_span.alloc(rows));
+  DCHK(d_planes.alloc((size_t)n_planes * 4));
+  DCHK(d_T.alloc((size_t)n_frames * 16));
+  DCHK(d_K.alloc(9));
+  DCHK(d_ptr.alloc(n_frames + 1));
+  DCHK(d_fill.alloc(fill_n));
+  if (downsample) DCHK(d_out.alloc(out_n));
+  if (n_planes > 0) {
+    DCHK(cudaMemcpy(d_jobs.p, jobs.data(), n_planes * sizeof(Job), cudaMemcpyHostToDevice));
+    DCHK(cudaMemcpy(d_planes.p, planes_sensor, (size_t)n_planes * 4 * sizeof(float), cudaMemcpyHostToDevice));
+  }
+  if (n_vtx > 0) DCHK(cudaMemcpy(d_vtx.p, vtx.data(), n_vtx * sizeof(int2), cudaMemcpyHostToDevice));
+  DCHK(cudaMemcpy(d_T.p, Ts, (size_t)n_frames * 16 * sizeof(float), cudaMemcpyHostToDevice));
+  DCHK(cudaMemcpy(d_K.p, invK, 9 * sizeof(float), cudaMemcpyHostToDevice));
+  DCHK(cudaMemcpy(d_ptr.p, plane_ptr, (n_frames + 1) * sizeof(int), cudaMemcpyHostToDevice));
+  if (n_planes > 0) depth_span_kernel<<<n_planes, 128>>>(d_jobs.p, d_vtx.p, d_edges.p, d_span.p);
+  DCHK(cudaGetLastError());
+  const long long fill_rows = (long long)n_frames * fh;
+  depth_kernel<<<(unsigned)((fill_rows + kWarps - 1) / kWarps), kThreads>>>(n_frames, d_ptr.p, d_jobs.p, d_edges.p, d_span.p,
+                                                                             d_planes.p, d_T.p, d_K.p, fw, fh, scale,
+                                                                             ceiling_threshold, d_fill.p);
+  DCHK(cudaGetLastError());
+  if (downsample) {
+    depth_resize_kernel<<<(unsigned)((out_n + 255) / 256), 256>>>(n_frames, d_fill.p, width, height, d_out.p);
+    DCHK(cudaGetLastError());
+  }
+  DCHK(cudaMemcpy(depth, downsample ? d_out.p : d_fill.p, out_n * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
 }
 
 // ---- closed wall and ground polygons (pus_popup_polygons) -------------------------------------------------------------

@@ -163,7 +163,7 @@ def cut_wall(cv2, P, ceiling, wl, cam):
 
 
 def frame(cv2, segs, K, iK, T, w, h, ceiling, wl):
-    """the three polygon lists of one frame, and its branch cases {(kind, A, B, cut)}"""
+    """the three polygon lists of one frame, its branch cases {(kind, A, B, cut)} and its sensor-frame planes (row order)"""
     n = len(segs)
     gw = [f32(0), f32(0), f32(-1), f32(0)]
     gs = [T[0, i] * gw[0] + T[1, i] * gw[1] + T[2, i] * gw[2] + T[3, i] * gw[3] for i in range(4)]
@@ -269,7 +269,7 @@ def frame(cv2, segs, K, iK, T, w, h, ceiling, wl):
         world.append(wd)
         cut.append([to_image(K, to_world(iT, p)) for p in wd])
         cases.add((kind, outer, inner_c, code))
-    return bound, cut, world, cases
+    return bound, cut, world, cases, planes
 
 
 def required(cases):
@@ -306,7 +306,7 @@ def main():
             K, iK, T = b["K"], b["invK"], b["Ts"][0]
             try:
                 with np.errstate(all="ignore"):
-                    bound, cut, world, cs = frame(cv2, fr[0], K, iK, T, w, h, f32(c), f32(wl))
+                    bound, cut, world, cs, _ = frame(cv2, fr[0], K, iK, T, w, h, f32(c), f32(wl))
             except NearCollinear:
                 skipped += 1
                 continue
