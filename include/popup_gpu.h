@@ -231,12 +231,22 @@ int pus_batch_optimize(pus_handle h, int* iterations);
 int pus_update(pus_handle h);
 /* double Slam::chi2()  Slam.cpp:266-268 (ESTIMATE) */
 int pus_chi2(pus_handle h, double* out);
-/* many independent graphs in one launch (BASELINE config 4); one CTA team per graph */
+/* many independent graphs in one launch (BASELINE config 4); one CTA team per graph.
+ * Every *_many call (here, the split calls below and pus_span_emulate_optimize) takes an array of n distinct, non-null
+ * handles: a null array, a null entry or a handle listed twice is refused with a message before any device work (two
+ * teams would otherwise solve one graph's device buffers at once).  n <= 0 does nothing and returns 0.  The handles ride
+ * on the first handle's stream for the duration of the call and get their own streams back when it returns. */
 int pus_batch_optimize_many(pus_handle* hs, int n, int* iterations);
 
 /* split form of pus_batch_optimize for measurement: upload (graph compile + H2D),
  * solve from the uploaded initial estimate with everything resident in HBM (repeatable),
- * download (D2H into the host mirrors). */
+ * download (D2H into the host mirrors).
+ * The resident solve and the download act on the graph as it was uploaded: a structural edit (node or factor added or
+ * removed), a change of linear-solver kind or of direct ordering after pus_upload makes them refuse the handle with
+ * "graph changed since its upload: call pus_upload", and nothing is launched or copied.  Value and measurement changes
+ * (pus_init_*, pus_set_measurement) do not make a handle stale: the resident solve starts again from the uploaded
+ * estimate and measurements, and pus_download overwrites the host values with its result; pus_upload takes them in.
+ * pus_batch_optimize and pus_batch_optimize_many upload first and are not affected. */
 int pus_upload(pus_handle h);
 int pus_solve_resident(pus_handle h, int* iterations);
 int pus_download(pus_handle h);

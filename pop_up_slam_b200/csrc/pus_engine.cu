@@ -3,6 +3,7 @@
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared -Xcompiler -fPIC ...
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -610,6 +611,15 @@ static int launch(Solver** ss, int n, int mode, int restore_init, int debug_stag
   return 0;
 }
 
+// The resident solve and the download act on the layout of the last upload: a structural edit, a change of linear-solver kind or
+// of direct ordering since then (each bumps topo_version) would launch on, or download through, tables of another graph.
+// Host-only, before any device work.
+static int check_uploaded(const Solver* s) {
+  if (!s->uploaded) { g_err = "graph not uploaded"; return -1; }
+  if (s->compiled_topo != s->g.topo_version) { g_err = "graph changed since its upload: call pus_upload"; return -1; }
+  return 0;
+}
+
 static int download(Solver** ss, int n) {
   Solver* s0 = ss[0];
   CUDA_OK(cudaSetDevice(s0->device));
@@ -653,6 +663,23 @@ static void release_stream(Solver* s) {
   if (!s->borrowing || --s->borrow_depth > 0) return;
   s->stream = s->saved_stream; s->own_stream = s->saved_own; s->borrowing = false;
   s->saved_stream = nullptr; s->saved_own = false;
+}
+// The handle array of a *_many call: no null entry, and no handle twice (two teams would solve one graph's device buffers at
+// once).  Host-only, before any device work.
+static int check_batch(const pus_handle* hs, int n, const char* fn) {
+  if (!hs) { g_err = std::string(fn) + ": null handle array"; return -1; }
+  std::vector<std::pair<pus_handle, int>> v(n);
+  for (int i = 0; i < n; i++) {
+    if (!hs[i]) { g_err = std::string(fn) + ": handle " + std::to_string(i) + " is null"; return -1; }
+    v[i] = std::make_pair(hs[i], i);
+  }
+  std::sort(v.begin(), v.end());
+  for (int i = 1; i < n; i++)
+    if (v[i].first == v[i - 1].first) {
+      g_err = std::string(fn) + ": handles " + std::to_string(v[i - 1].second) + " and " + std::to_string(v[i].second) + " are the same handle";
+      return -1;
+    }
+  return 0;
 }
 struct BatchStreams {   // RAII: handles 1..n-1 ride on handle 0's stream until the call returns
   pus_handle* hs; int n;
@@ -911,6 +938,7 @@ int pus_set_solver_options(pus_handle h, const pus_solver_options* in) { NEED(h)
 int pus_upload(pus_handle h) { NEED(h); return upload(SV(h)); }
 int pus_upload_many(pus_handle* hs, int n) {
   if (n <= 0) return 0;
+  if (check_batch(hs, n, "pus_upload_many") < 0) return -1;
   if (ensure_device(SV(hs[0])) < 0) return -1;
   BatchStreams bs(hs, n, SV(hs[0])->stream);
   for (int i = 0; i < n; i++) if (upload(SV(hs[i])) < 0) return -1;
@@ -920,6 +948,7 @@ static int solve_many(pus_handle* hs, int n, int* iters, int mode, int restore) 
   if (n <= 0) return 0;
   std::vector<Solver*> ss(n);
   for (int i = 0; i < n; i++) ss[i] = SV(hs[i]);
+  for (int i = 0; i < n; i++) if (check_uploaded(ss[i]) < 0) return -1;
   if (ensure_device(ss[0]) < 0) return -1;
   BatchStreams bs(hs, n, ss[0]->stream);
   // direct-mode (dense and band) and PCG handles run in their own kernels: a mixed batch is two launches, one per kernel
@@ -932,17 +961,22 @@ static int solve_many(pus_handle* hs, int n, int* iters, int mode, int restore) 
 }
 int pus_solve_resident(pus_handle h, int* iters) { NEED(h); return solve_many(&h, 1, iters, MODE_BATCH, 1); }
 int pus_solve_resident_many(pus_handle* hs, int n, int* iters) {
-  if (n > 1) {  // all graphs ride on the first handle's stream
-    Solver* s0 = SV(hs[0]);
-    if (ensure_device(s0) < 0) return -1;
-  }
+  if (n <= 0) return 0;
+  if (check_batch(hs, n, "pus_solve_resident_many") < 0) return -1;
   return solve_many(hs, n, iters, MODE_BATCH, 1);
 }
-int pus_download(pus_handle h) { NEED(h); Solver* s = SV(h); return download(&s, 1); }
+int pus_download(pus_handle h) {
+  NEED(h);
+  Solver* s = SV(h);
+  if (check_uploaded(s) < 0) return -1;
+  return download(&s, 1);
+}
 int pus_download_many(pus_handle* hs, int n) {
   if (n <= 0) return 0;
+  if (check_batch(hs, n, "pus_download_many") < 0) return -1;
   std::vector<Solver*> ss(n);
   for (int i = 0; i < n; i++) ss[i] = SV(hs[i]);
+  for (int i = 0; i < n; i++) if (check_uploaded(ss[i]) < 0) return -1;
   if (ensure_device(ss[0]) < 0) return -1;
   BatchStreams bs(hs, n, ss[0]->stream);
   return download(ss.data(), n);
@@ -957,6 +991,7 @@ int pus_batch_optimize(pus_handle h, int* iters) {
 }
 int pus_batch_optimize_many(pus_handle* hs, int n, int* iters) {
   if (n <= 0) return 0;
+  if (check_batch(hs, n, "pus_batch_optimize_many") < 0) return -1;
   Solver* s0 = SV(hs[0]);
   if (ensure_device(s0) < 0) return -1;
   BatchStreams bs(hs, n, s0->stream);
@@ -1027,6 +1062,7 @@ int pus_span_optimize(pus_handle h, int* iters) {
 }
 int pus_span_emulate_optimize(pus_handle* hs, int world, int* iters) {
   if (world < 1 || world > 8) { g_err = "pus_span_emulate_optimize: world must be 1..8"; return -1; }
+  if (check_batch(hs, world, "pus_span_emulate_optimize") < 0) return -1;
   for (int i = 0; i < world; i++) if (refuse_direct_span(SV(hs[i]), "pus_span_emulate_optimize") < 0) return -1;
   Solver* s0 = SV(hs[0]);
   if (ensure_device(s0) < 0) return -1;
