@@ -287,7 +287,7 @@ static int upload(Solver* s) {
     AL(ypart, 8, "ypart"); AL(upartb, (size_t)std::max(1, c.ngrp) * 3, "upartb"); AL(hpart, (size_t)std::max(1, c.n_atask) * 9, "hpart");
     AL(ovf, c.n_ovf, "ovf");
     AL(Binv, (size_t)c.nblk * kPackedBlock, "Binv"); AL(Wc, (size_t)c.nce * 18, "Wc"); AL(Yc, (size_t)c.nce * 18, "Yc");
-    AL(Ac, ac_doubles(6 * c.nc_pad), "Ac"); AL(Atri, ac_tri_doubles(6 * c.nc_pad), "Atri"); AL(Apan, ac_panel_doubles(6 * c.nc_pad), "Apan");
+    AL(Ac, ac_elems(6 * c.nc_pad), nullptr); AL(Atri, ac_tri_doubles(6 * c.nc_pad), "Atri"); AL(Apan, ac_panel_doubles(6 * c.nc_pad), "Apan");
     AL(Wc2, (size_t)c.nce2 * 18, "Wc2"); AL(Yc2, (size_t)c.nce2 * 18, "Yc2"); AL(D2inv, (size_t)c.ng2 * kBlockDim * kBlockDim, "D2inv");
     {
       // The vectors the PCG phases exchange live in ONE allocation (the "mirror arena"): when one graph spans several
@@ -2044,11 +2044,11 @@ long long pus_debug_fetch(pus_handle h, const char* name, double* out, long long
     }
     return cnt;
   }
-  if (nm == "Acinv") {  // de-tiled: row-major ldm x ldm
+  if (nm == "Acinv") {  // de-tiled: row-major ldm x ldm, the stored fp32 values widened
     const int ldm = 6 * c.nc_pad;
-    const size_t n = ac_doubles(ldm);
-    std::vector<double> tmp(n);
-    if (cudaMemcpy(tmp.data(), s->hd.Ac, n * 8, cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
+    const size_t n = ac_elems(ldm);
+    std::vector<float> tmp(n);
+    if (cudaMemcpy(tmp.data(), s->hd.Ac, n * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess) { g_err = "memcpy"; return -1; }
     long long cnt = (long long)ldm * ldm;
     if (cnt <= cap)
       for (int r = 0; r < ldm; r++)

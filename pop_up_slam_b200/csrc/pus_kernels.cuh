@@ -126,7 +126,8 @@ struct DevGraph {
   double *Hpp, *gp, *Hll, *gl, *Hinv, *vl, *dl;
   double *upart, *ypart;
   double *Binv, *Wc, *Yc;
-  double *Ac, *Atri, *Apan;     // A_c^-1 for the applies (ac_index); the triangle and panel buffers of its inversion
+  float *Ac;                    // A_c^-1 for the applies (ac_index), rounded to fp32: the preconditioner, not the operator
+  double *Atri, *Apan;          // the triangle and panel buffers of its inversion (fp64)
   double *x, *r, *z, *q, *b, *pv[2], *xprev, *zc;
   double *rcpart[2], *qcpart;
   double *red;
@@ -391,14 +392,15 @@ __device__ __forceinline__ void dmma884(double* cacc, double a, double b) {
                : "d"(a), "d"(b));
 }
 
-// A_c^-1 as the PCG applies read it: full rows, stored as 48-row x 128-column tiles with a padded row stride
+// A_c^-1 as the PCG applies read it: full rows of fp32, stored as 48-row x 128-column tiles with a padded row stride (528
+// bytes: every row of a tile starts 16-byte aligned)
 constexpr int kGjChunk = 128, kGjLdR = kGjChunk + 4;
-constexpr int kGjTile = 48 * kGjLdR;   // doubles per tile
+constexpr int kGjTile = 48 * kGjLdR;   // elements per tile
 __host__ __device__ inline int ac_chunks(int ldm) { return (ldm + kGjChunk - 1) / kGjChunk; }
 __host__ __device__ inline size_t ac_index(int ldm, int row, int col) {
   return ((size_t)(row / 48) * ac_chunks(ldm) + (col / kGjChunk)) * kGjTile + (size_t)(row % 48) * kGjLdR + (col % kGjChunk);
 }
-__host__ __device__ inline size_t ac_doubles(int ldm) { return (size_t)(ldm / 48) * ac_chunks(ldm) * kGjTile; }
+__host__ __device__ inline size_t ac_elems(int ldm) { return (size_t)(ldm / 48) * ac_chunks(ldm) * kGjTile; }
 // A_c while it is assembled and inverted: the lower triangle only, as 48x48 tiles (I, J), I >= J, each stored with a
 // padded row stride (conflict-free DMMA fragment loads; one bulk copy moves a tile).  Tiles are numbered band by band
 // (bands of two tile rows), column by column inside a band: (0,0) (1,0) (1,1) | (2,0) (3,0) (2,1) (3,1) (2,2) (3,2) (3,3) | ...
@@ -477,6 +479,7 @@ static_assert(kSmTmaEnd <= 227 * 1024, "TMA staging buffers");
 // coarse inversion: eight 48x48 tiles (P, two T rows, three snapshot tiles, two staging tiles), the coefficient columns of the pivot
 // inversion and the owned tile range -- the same for every team size
 static_assert(kSmWork + (8 * kAcTile + 48 * 12 + 2) * 8 <= kSmemBytes, "coarse inversion buffers");
+static_assert(kSmWork % 16 == 0 && kSmRc % 16 == 0, "coarse residuals are read with 128-bit shared loads");
 static_assert(kSmemBytes <= 227 * 1024, "dynamic shared memory");
 
 
@@ -801,33 +804,34 @@ __device__ __forceinline__ double packed_row_dot(const double* B, int u, const d
   return acc;
 }
 
-// row of A_c^-1 (arow = its first element in the tiled layout) times the coarse residual src[0 .. ldm), one warp per row:
-// 128-bit loads, a lane owns column pairs (2 lane + 64 t), so a 1 884-wide row is two batches of 16 loads in flight (pairs never
-// straddle a 128-column tile: tile rows are 16-byte aligned, stride 132).  Returns the row sum on every lane.
-__device__ __forceinline__ double coarse_row_dot(const double* arow, const double* src, int ldm, int lane) {
+// row of A_c^-1 (arow = its first element in the fp32 tiled layout) times the coarse residual src[0 .. ldm) (16-byte aligned),
+// one warp per row: a lane owns the four columns 4 lane + 128 t of tile chunk t (one 128-bit load; the residual as two
+// 128-bit shared loads), products and sums in fp64.  kFly chunks are loaded per round.  The block-resident loop takes 16 (up
+// to 2 048 columns; A_c is at most 1 920 wide), so a row is one round of loads.  The general loop (schur_solve) holds many
+// more live values, and loads in flight there cost spills in the whole loop: its two-level apply takes 8, its level-3 apply
+// (a few hundred rows) 4.  Returns the row sum on every lane.
+template <int kFly>
+__device__ __forceinline__ double coarse_row_dot(const float* arow, const double* src, int ldm, int lane) {
   double acc = 0;
-  int j = 2 * lane;
-  for (; j + 64 * 15 < ldm; j += 64 * 16) {
-    double2 av[16];
+  for (int j0 = 4 * lane; j0 < ldm; j0 += kFly * kGjChunk) {
+    float4 av[kFly];
 #pragma unroll
-    for (int t = 0; t < 16; t++) {
-      const int jj = j + 64 * t;
-      av[t] = __ldcg(reinterpret_cast<const double2*>(arow + (size_t)(jj / kGjChunk) * kGjTile + (jj % kGjChunk)));
+    for (int t = 0; t < kFly; t++) {
+      const int jj = j0 + kGjChunk * t;
+      av[t] = (jj < ldm) ? __ldcg(reinterpret_cast<const float4*>(arow + (size_t)(jj / kGjChunk) * kGjTile + (jj % kGjChunk)))
+                         : make_float4(0.f, 0.f, 0.f, 0.f);
     }
 #pragma unroll
-    for (int t = 0; t < 16; t++) acc += av[t].x * src[j + 64 * t] + av[t].y * src[j + 64 * t + 1];
-  }
-  {
-    double2 av[16];
-#pragma unroll
-    for (int t = 0; t < 16; t++) {
-      const int jj = j + 64 * t;
-      av[t] = (jj < ldm) ? __ldcg(reinterpret_cast<const double2*>(arow + (size_t)(jj / kGjChunk) * kGjTile + (jj % kGjChunk))) : make_double2(0.0, 0.0);
-    }
-#pragma unroll
-    for (int t = 0; t < 16; t++) {
-      const int jj = j + 64 * t;
-      if (jj < ldm) acc += av[t].x * src[jj] + av[t].y * src[jj + 1];   // (ldm = 6 nc is even)
+    for (int t = 0; t < kFly; t++) {
+      const int jj = j0 + kGjChunk * t;
+      if (jj < ldm) {   // (ldm = 6 nc is even: the lane's first pair is inside, its second may not be)
+        const double2 s0 = *reinterpret_cast<const double2*>(src + jj);
+        acc += (double)av[t].x * s0.x + (double)av[t].y * s0.y;
+        if (jj + 2 < ldm) {
+          const double2 s1 = *reinterpret_cast<const double2*>(src + jj + 2);
+          acc += (double)av[t].z * s1.x + (double)av[t].w * s1.y;
+        }
+      }
     }
   }
   return warp_sum(acc);
@@ -1753,7 +1757,8 @@ struct Phase {
   // and every owned tile of the column gets  (i,j): A_ij + T_i C_j^T,  (K,j): P C_j^T,  (i,K): -T_i,  (K,K): -P
   // on the FP64 tensor cores.  Look-ahead: the owner of diagonal tile K+1 updates that tile first, inverts it and
   // publishes P_{K+1} before it updates the rest, so no CTA inverts a pivot redundantly (kPivotWeight gives it fewer
-  // tiles).  One team barrier per step.  The last step writes -(its result), mirrored, into the full layout of G.Ac.
+  // tiles).  One team barrier per step.  The last step writes -(its result), mirrored and rounded to fp32, into the full
+  // layout of G.Ac.
   __device__ void coarse_invert() {
     const int ldm = G.ldmc, nb = ldm / 48, nt = ac_ntri(ldm);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3;
@@ -1939,11 +1944,12 @@ struct Phase {
 #pragma unroll
           for (int s = 0; s < 3; s++) {
             if (!frag(s, r, cc)) continue;
-            if (last) {   // -(result) into the apply layout, mirrored; a diagonal tile contributes its lower half only
+            if (last) {   // -(result) into the apply layout in fp32, mirrored (both copies get one rounding: exactly symmetric);
+                          // a diagonal tile contributes its lower half only
               const int R = 48 * i + r, C = 48 * j + cc;
-              const double v0 = -acc[k][s][0], v1 = -acc[k][s][1];
+              const float v0 = (float)-acc[k][s][0], v1 = (float)-acc[k][s][1];
               if (i != j) {
-                *reinterpret_cast<double2*>(G.Ac + ac_index(ldm, R, C)) = make_double2(v0, v1);
+                *reinterpret_cast<float2*>(G.Ac + ac_index(ldm, R, C)) = make_float2(v0, v1);
                 G.Ac[ac_index(ldm, C, R)] = v0;
                 G.Ac[ac_index(ldm, C + 1, R)] = v1;
               } else {
@@ -2422,14 +2428,11 @@ struct Phase {
     }
     __syncthreads();
     lap(13);
-    const double* Ai = G.Ac;
+    const float* Ai = G.Ac;
     double dot = 0.0;
     if (c.l3_local) {
       for (int i = tid >> 5; i < ldm; i += kWarps) {
-        const double* arow = Ai + ac_index(G.ldmc, i, 0);
-        double acc = 0.0;
-        for (int j = lane; j < ldm; j += 32) acc += ldc(arow + (size_t)(j / kGjChunk) * kGjTile + (j % kGjChunk)) * src[j];
-        acc = warp_sum(acc);
+        const double acc = coarse_row_dot<4>(Ai + ac_index(G.ldmc, i, 0), src, ldm, lane);
         if (lane == 0) {
           z3s[i] = acc;
           if (c.rank == 0) dot += src[i] * acc;
@@ -2439,21 +2442,7 @@ struct Phase {
     } else {
       const int nw = nwarp_team();
       for (int i = warp_team(); i < ldm; i += nw) {
-        const double* arow = Ai + ac_index(G.ldmc, i, 0);
-        double acc = 0.0;
-        int j = lane;
-        for (; j + 32 * 7 < ldm; j += 32 * 8) {
-          double av[8];
-#pragma unroll
-          for (int t = 0; t < 8; t++) {
-            const int jj = j + 32 * t;
-            av[t] = ldc(arow + (size_t)(jj / kGjChunk) * kGjTile + (jj % kGjChunk));
-          }
-#pragma unroll
-          for (int t = 0; t < 8; t++) acc += av[t] * src[j + 32 * t];
-        }
-        for (; j < ldm; j += 32) acc += ldc(arow + (size_t)(j / kGjChunk) * kGjTile + (j % kGjChunk)) * src[j];
-        acc = warp_sum(acc);
+        const double acc = coarse_row_dot<4>(Ai + ac_index(G.ldmc, i, 0), src, ldm, lane);
         if (lane == 0) { put(c, &G.zc[i], acc); dot += src[i] * acc; }
       }
     }
@@ -2543,14 +2532,14 @@ struct Phase {
       }
       __syncthreads();
       lap(13);
-      const double* Ai = G.Ac;
+      const float* Ai = G.Ac;
       // coarse part, distributed over the team: one warp per row of A_c^-1.  z is never formed with its coarse
       // part; r.z = r.z_local + rc.zc (rc = P^T r), and the consumers of z add P*zc on the fly.
       {
         const int lane = tid & 31;
         const int nw = nwarp_team();
         for (int i = warp_team(); i < ldm; i += nw) {
-          const double acc = coarse_row_dot(Ai + ac_index(G.ldmc, i, 0), src, ldm, lane);
+          const double acc = coarse_row_dot<8>(Ai + ac_index(G.ldmc, i, 0), src, ldm, lane);
           if (lane == 0) { put(c, &G.zc[i], acc); dot += src[i] * acc; }
         }
       }
@@ -2816,7 +2805,7 @@ struct Phase {
     int wpe = kWarps;   // warps per listed plane (power of two)
     while (wpe > 1 && wpe * nh > kWarps) wpe >>= 1;
     double* hvp = reinterpret_cast<double*>(g_smem + L.hdr + 64 + kResHeavy * 16);   // [kResHeavy][kWarps][3] partial sums
-    const double* Ai = G.Ac;
+    const float* Ai = G.Ac;
     double* pvec = G.pv[0];
     int it = 0;
     double beta = 0.0;
@@ -3002,7 +2991,7 @@ struct Phase {
         const int nw = bal ? ne * kWarps : nwarp_team();
         const int w0 = bal ? (c.rank >= n3 ? warp * ne + (c.rank - n3) : ldm) : warp_team();
         for (int i = w0; i < ldm; i += nw) {
-          const double acc = coarse_row_dot(Ai + ac_index(G.ldmc, i, 0), src, ldm, lane);
+          const double acc = coarse_row_dot<16>(Ai + ac_index(G.ldmc, i, 0), src, ldm, lane);
           if (lane == 0) { G.zc[i] = acc; dot += src[i] * acc; }
         }
       }
