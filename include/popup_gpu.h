@@ -364,6 +364,65 @@ int pus_popup_depth(int device, int n_frames, const int* plane_ptr, const int* p
                     const float* planes_sensor, const float* Ts, const float* invK, int width, int height, int downsample,
                     float ceiling_threshold, float* depth);
 
+/* ---- ground edges (float32) ------------------------------------------------------------------ */
+/* popup_plane::edge_get_polygons (PUW/libs/select_edge.cpp:66-406) with the Python stages it runs through an embedded
+ * interpreter, pop_up_fun.python_get_contours and interval_tree_optimization (pop_up_python/python/pop_up_python/
+ * pop_up_fun.py:85-205), batched over frames, on the device: which of a frame's detected lines form the ground-wall
+ * boundary, given the CNN label map.  The line detector itself stays with the caller.
+ *   labels[n_frames][height][width]   the label maps, ground 255 (any uint8 values are taken)
+ *   line_ptr[n_frames+1], lines[n][4]   CSR offsets and the frames' detected lines x1 y1 x2 y2 (float pixels)
+ *   params   popup_plane's members (popup_plane.h:178-200); NULL is refused
+ * Outputs, as edge_get_polygons' return tuple, packed in frame order like pus_popup_polygons':
+ *   open_counts[n_frames], open_segs[..][4]        ground_seg2d_lines_actual, what main_3d.cpp:428 passes to the fit: the
+ *                                                  counts prefix-summed are pus_popup_fit_frames' seg_ptr, open_segs its segs
+ *   connect_counts[n_frames], connect_segs[..][4]  ground_seg2d_lines_connect: the same segments with the connectors added
+ *   open_in_connect[..]                            final_lines_in_extend_ind: each open segment's row in its frame's
+ *                                                  connected list
+ *   status[n_frames]   0 segments found; 1 no contour (the Python raises; the reference then reads a missing or stale
+ *                      ground_contour), also when the assembly would raise KeyError (a dict pop of a key it never stored,
+ *                      which scikit-image 0.14's lookups by get allow where pixels are shared by several chains);
+ *                      2 nothing survives steps 1-4 (the reference returns empty lists); 3 the interval tree would raise
+ *                      on a null or reversed interval; 4 no segment is longer than post_short_thre (the reference then
+ *                      indexes an empty matrix); 5 the frame's scratch ran out: the contour assembly's node list (4 nodes
+ *                      per marching-squares segment, of which a join through a stale dict entry may copy a contour) --
+ *                      a limit of this library, not an outcome of the reference.  A frame with a non-zero status has
+ *                      no segments.
+ * The counts and status are always written; open_segs = connect_segs = NULL is a size query; the capacities are in rows,
+ * and too small a one fails with a message.  Returns the number of frames with status 0.
+ * Stages, pinned:
+ *   0 labels: with downsample_contour cv::resize 0.5x INTER_NEAREST (source pixel min(2 x, w - 1); the half size rounds
+ *     half to even as cvRound), dilate 8 x 8, erode 8 x 8; otherwise dilate dilation_distance^2 and erode erosion_distance^2.
+ *     A k x k box with OpenCV's anchor k / 2 and its default border (pixels outside take no part), then 255 - v; OpenCV 4.13.
+ *   1 contour: scikit-image 0.14's find_contours(map, 0) (cells row-major, case bits ul > 0 (1), ur (2), ll (4), lr (8),
+ *     saddles 6 and 9 fully_connected='low', degenerate segments skipped, joined through its two point-keyed dicts, stale
+ *     entries and the lower contour number's survival included, sorted by number); at level 0 on uint8 data every point is
+ *     a pixel.  The contour with the largest start-end distance (first maximum), as (x, y), every 20th point but the last,
+ *     doubled with downsample_contour.
+ *   2 steps 1-4 of select_edge.cpp:91-257, each restart loop capped at 100 passes acting on the first triggering pair.
+ *   3 intervaltree 2.x: a set of (begin, end, data) intervals, half-open search, sorted by (begin, end, data),
+ *     split_overlaps at every boundary; overlap sums in float64 of float32 terms and the int() refinement in float64, as
+ *     NumPy 1.x promotes a float32 scalar with a Python number.
+ *   4 post-processing of select_edge.cpp:276-405, direction_hit_boundary as pus_popup_polygons'.
+ * Precision: the thresholds are doubles and compared in double against float values; sample_ind / 10.0 rounds to float;
+ * PI = 3.14159265.  Deviation: angles use float(atan2(double y, double x)) on every side instead of atan2f, whose glibc and
+ * CUDA versions differ (at most 1 ulp).  Refused with a message, nothing launched: malformed line_ptr, non-finite lines,
+ * more than PUS_POPUP_MAX_LINES lines in a frame, width or height below 4, NULL labels or params, kernel sizes below 1.
+ * Deterministic (no floating-point atomics): repeated calls and any split of the batch give the same bytes.  No CPU
+ * fallback. */
+#define PUS_POPUP_MAX_LINES 512
+typedef struct pus_edge_params {
+  int dilation_distance, erosion_distance;   /* 11, 11 (k x k box); with downsample_contour 8 x 8 on the half map */
+  int downsample_contour;                    /* popup_param.yaml: true; popup_tum_far.yaml: false */
+  double pre_vertical_thre, pre_minium_len, pre_boundary_thre, pre_contour_close_thre, pre_merge_angle_thre,
+      pre_merge_dist_thre, pre_proj_angle_thre, pre_proj_cover_thre, pre_proj_cover_large_thre, pre_proj_dist_thre,
+      interval_overlap_thre, post_short_thre, post_bind_dist_thre, post_merge_dist_thre, post_merge_angle_thre,
+      post_extend_thre;
+} pus_edge_params;
+int pus_popup_edges(int device, int n_frames, const unsigned char* labels, int width, int height, const int* line_ptr,
+                    const float* lines, const pus_edge_params* params, int* status, int* open_counts, int* connect_counts,
+                    float* open_segs, float* connect_segs, int* open_in_connect, long long open_capacity,
+                    long long connect_capacity);
+
 /* ---- device-resident measurement refresh and polygon re-projection (SURVEY.md 8f.1) -------- */
 /* Mapper_mono::update_plane_measurement (pop_planar_slam/src/Mapping.cpp:590-607): after a solve every past
  * frame re-pops its wall planes from its ground segments with the frame's LATEST pose estimate

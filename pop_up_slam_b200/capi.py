@@ -762,3 +762,67 @@ def popup_depth(lib, plane_ptr, poly_ptr, polys, planes_sensor, Ts, invK, width,
     if rc < 0:
         raise ApiError((err() or b"?").decode())
     return out
+
+
+class EdgeParams(C.Structure):
+    """pus_edge_params (include/popup_gpu.h)"""
+    _fields_ = [("dilation_distance", C.c_int), ("erosion_distance", C.c_int), ("downsample_contour", C.c_int)] + [
+        (k, C.c_double) for k in (
+            "pre_vertical_thre", "pre_minium_len", "pre_boundary_thre", "pre_contour_close_thre", "pre_merge_angle_thre",
+            "pre_merge_dist_thre", "pre_proj_angle_thre", "pre_proj_cover_thre", "pre_proj_cover_large_thre",
+            "pre_proj_dist_thre", "interval_overlap_thre", "post_short_thre", "post_bind_dist_thre", "post_merge_dist_thre",
+            "post_merge_angle_thre", "post_extend_thre")]
+
+
+# popup_plane's member defaults (popup_plane.h:178-200, popup_plane.cpp:32-33) with popup_param.yaml's downsample_contour.
+# main_3d loads popup_param.yaml over the members, which changes four of them: post_short_thre 20, post_bind_dist_thre 15,
+# post_merge_dist_thre 10, post_extend_thre 50 (popup_tum_far.yaml: downsample_contour off, pre_contour_close_thre 400,
+# post_bind_dist_thre 30, post_merge_dist_thre 50, post_merge_angle_thre 20, post_extend_thre 0).  Pass those as params to
+# follow a launch file.
+EDGE_DEFAULTS = dict(dilation_distance=11, erosion_distance=11, downsample_contour=1, pre_vertical_thre=15.0,
+                     pre_minium_len=15.0, pre_boundary_thre=5.0, pre_contour_close_thre=50.0, pre_merge_angle_thre=10.0,
+                     pre_merge_dist_thre=10.0, pre_proj_angle_thre=20.0, pre_proj_cover_thre=0.6,
+                     pre_proj_cover_large_thre=0.8, pre_proj_dist_thre=100.0, interval_overlap_thre=20.0,
+                     post_short_thre=30.0, post_bind_dist_thre=10.0, post_merge_dist_thre=20.0, post_merge_angle_thre=10.0,
+                     post_extend_thre=15.0)
+
+
+def popup_edges(lib, labels, line_ptr, lines, params=None, segments=True, capacity=None, prefix="pus_", device=0):
+    """popup_plane::edge_get_polygons batched over frames (pus_popup_edges, include/popup_gpu.h).
+
+    labels [n_frames, height, width] uint8 (ground 255), line_ptr [n_frames+1] CSR offsets, lines [n, 4] float pixels,
+    params a dict over EDGE_DEFAULTS (None: the defaults).  Returns a dict: status, open_counts, connect_counts [n_frames]
+    int32, open_ptr / connect_ptr [n_frames+1] and, unless segments=False (a size query), open [.., 4], connect [.., 4]
+    float32 and open_in_connect int32.  open_ptr / open are the seg_ptr / segs of popup_fit_frames and popup_polygons.
+    capacity = (open, connect) in rows fills buffers of that size instead of the queried ones."""
+    labels = np.ascontiguousarray(labels, dtype=np.uint8)
+    nf, h, w = labels.shape
+    line_ptr = _i32(line_ptr)
+    lines = np.ascontiguousarray(lines, dtype=np.float32).reshape(-1, 4)
+    P = EdgeParams(**dict(EDGE_DEFAULTS, **(params or {})))
+    st, oc, cc = (np.zeros(nf, np.int32) for _ in range(3))
+    fn = getattr(lib, prefix + "popup_edges")
+    fn.restype = C.c_int
+    fn.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, c_int_p, c_float_p, C.POINTER(EdgeParams), c_int_p,
+                   c_int_p, c_int_p, c_float_p, c_float_p, c_int_p, C.c_longlong, C.c_longlong]
+    err = getattr(lib, prefix + "last_error", None) or getattr(lib, prefix + "popup_last_error")
+    err.restype = C.c_char_p
+
+    def call(o, c, i, caps):
+        rc = fn(device, nf, labels.ctypes.data, w, h, _ip(line_ptr), lines.ctypes.data_as(c_float_p), C.byref(P), _ip(st),
+                _ip(oc), _ip(cc), *[None if a is None else a.ctypes.data_as(c_float_p) for a in (o, c)],
+                None if i is None else _ip(i), *[int(x) for x in caps])
+        if rc < 0:
+            raise ApiError((err() or b"?").decode())
+
+    call(None, None, None, (0, 0))
+    res = dict(status=st.copy(), open_counts=oc.copy(), connect_counts=cc.copy(),
+               open_ptr=np.concatenate([[0], np.cumsum(oc)]).astype(np.int32),
+               connect_ptr=np.concatenate([[0], np.cumsum(cc)]).astype(np.int32))
+    if segments:
+        tot = (int(res["open_ptr"][-1]), int(res["connect_ptr"][-1]))
+        cap = tot if capacity is None else [int(c) for c in capacity]
+        o, c, i = np.empty((cap[0], 4), np.float32), np.empty((cap[1], 4), np.float32), np.empty(max(cap[0], 0), np.int32)
+        call(o, c, i, cap)
+        res.update(open=o[:tot[0]], connect=c[:tot[1]], open_in_connect=i[:tot[0]])
+    return res

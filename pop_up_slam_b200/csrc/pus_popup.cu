@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "../../include/popup_gpu.h"
+#include "pus_edges.cuh"
 
 namespace pus {
 extern thread_local std::string g_err;
@@ -903,11 +904,9 @@ constexpr int kWallMax = 7;
 constexpr int kHullMax = 34;                          // 6 x 4 edge crossings + 10 corners
 constexpr int kCutSlot = kHullMax + 1;
 
-struct P2 { float x, y; };
 struct P3 { float x, y, z; };
 
-// x86 cvttss2si, which the reference's (int) casts compile to: NaN or out of range gives INT_MIN (cvt.rzi saturates)
-__device__ __forceinline__ int trunc_i(float v) { return (v >= -2147483648.f && v < 2147483648.f) ? __float2int_rz(v) : INT_MIN; }
+// P2, trunc_i and hit_boundary (direction_hit_boundary) are in pus_edges.cuh, shared with pus_popup_edges
 __device__ __forceinline__ int sgnf(float a) { return (a > 0.f) - (a < 0.f); }
 
 __device__ int sklansky(const P2* p, const int* ord, int start, int end, int* stack, int nsign, int sign2) {
@@ -1054,39 +1053,6 @@ __device__ int point_polygon_test(const P2* c, int n, P2 pt) {
     counter += dist > 0;
   }
   return counter % 2 == 0 ? -1 : 1;
-}
-
-// direction_hit_boundary (nobottom = false); its lambdas are double expressions rounded to float
-__device__ P2 hit_boundary(P2 pt, P2 d, int w, int h) {
-  if (d.y < 0) {
-    const float l = (float)((0.0 - (double)pt.y) / (double)d.y);
-    if (l >= 0) {
-      const P2 q{pt.x + l * d.x, pt.y + l * d.y};
-      if (0 <= trunc_i(q.x) && trunc_i(q.x) <= w - 1) return q;
-    }
-  }
-  if (d.y > 0) {
-    const float l = (float)(((double)h - 1.0 - (double)pt.y) / (double)d.y);
-    if (l >= 0) {
-      const P2 q{pt.x + l * d.x, pt.y + l * d.y};
-      if (0 <= trunc_i(q.x) && trunc_i(q.x) <= w - 1) return q;
-    }
-  }
-  if (d.x > 0) {
-    const float l = (float)(((double)w - 1.0 - (double)pt.x) / (double)d.x);
-    if (l >= 0) {
-      const P2 q{pt.x + l * d.x, pt.y + l * d.y};
-      if (0 <= trunc_i(q.y) && trunc_i(q.y) <= h - 1) return q;
-    }
-  }
-  if (d.x < 0) {
-    const float l = (float)((0.0 - (double)pt.x) / (double)d.x);
-    if (l >= 0) {
-      const P2 q{pt.x + l * d.x, pt.y + l * d.y};
-      if (0 <= trunc_i(q.y) && trunc_i(q.y) <= h - 1) return q;
-    }
-  }
-  return P2{-1.f, -1.f};
 }
 
 // A (p, 1) for a row-major 4x4 A, divided by its fourth component (homo_to_real_coord)
@@ -1481,4 +1447,183 @@ extern "C" int pus_popup_polygons(int device, int n_frames, const int* seg_ptr, 
   if (world3d && tot[2] > 0) GCHK(cudaMemcpy(world3d, d_ow.p, (size_t)tot[2] * 3 * sizeof(float), cudaMemcpyDeviceToHost));
   GCHK(cudaDeviceSynchronize());
   return 0;
+}
+
+// ---- ground edges (pus_popup_edges) ----------------------------------------------------------------------------------
+// popup_plane::edge_get_polygons (select_edge.cpp:66-406) with pop_up_fun.python_get_contours and
+// interval_tree_optimization.  The label preprocessing runs as four separable box passes, one thread per pixel; a per-cell
+// kernel counts each frame's marching-squares segments (integer atomics: the count does not depend on their order) so the
+// host can size the assembly scratch; then one thread per frame, each in a block of its own so that the frames' divergent
+// sequential work does not serialise within a warp, replays the order-dependent part -- the dict-driven
+// contour assembly in cell order and the restart loops of the selection -- with the shared code of pus_edges.cuh.
+namespace pus {
+namespace edges {
+struct Frame {   // one frame's scratch and output slots
+  long long node, obj, cpt, line, ivl, tab;
+  int node_cap, obj_cap, cpt_cap, ivl_cap, l0, n;
+};
+
+// one box pass over all frames; pass 0 reads the label maps (with the 0.5x pick), the last one writes 255 - v
+__global__ void edge_box_kernel(int n_frames, const unsigned char* src, int sw, int sh, int ds, int w, int h, int k, int horiz,
+                                int dilate, int invert, unsigned char* dst) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x, per = (long long)w * h;
+  if (i >= per * n_frames) return;
+  const int f = (int)(i / per), p = (int)(i % per);
+  const unsigned char v = box_pass(src + (long long)f * sw * sh, sw, sh, ds, w, h, p % w, p / w, k, horiz, dilate);
+  dst[i] = invert ? (unsigned char)(255 - v) : v;
+}
+
+__global__ void edge_count_kernel(int n_frames, const unsigned char* map, int w, int h, int* counts) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x, per = (long long)(w - 1) * (h - 1);
+  if (i >= per * n_frames) return;
+  const int f = (int)(i / per), p = (int)(i % per);
+  const int c = cell_count(map + (long long)f * w * h, w, p / (w - 1), p % (w - 1));
+  if (c) atomicAdd(counts + f, c);
+}
+
+__global__ void edge_frame_kernel(int n_frames, pus_edge_params P, int width, int height, const unsigned char* map, int w,
+                                  int h, const Frame* fr, int* tab, int* nodes, int* objs, unsigned char* flags, float* cpts,
+                                  const float* lines, Lin* rows, float* bounds, Ivl* ivl, float* open_slot, float* conn_slot,
+                                  int* in_conn_slot, int* out) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= n_frames) return;
+  const Frame F = fr[f];
+  const long long cells = (long long)w * h;
+  Asm A{tab + F.tab, tab + F.tab + cells, nodes + 2 * F.node, nodes + 2 * F.node + F.node_cap, objs + 3 * F.obj,
+        objs + 3 * F.obj + F.obj_cap, objs + 3 * F.obj + 2 * F.obj_cap, flags + 2 * F.obj, flags + 2 * F.obj + F.obj_cap,
+        F.node_cap, F.obj_cap, 0, 0, 0u, false};
+  Sel S{rows + 2 * F.line, 2 * F.n, ivl + 2 * F.ivl, ivl + 2 * F.ivl + F.ivl_cap, bounds + 2 * F.line, F.ivl_cap};
+  int n_open = 0, n_conn = 0;
+  unsigned bits = 0;
+  const int st = frame_edges(P, width, height, map + (long long)f * cells, w, h, A, cpts + 2 * F.cpt, F.cpt_cap,
+                             lines + 4 * (long long)F.l0, F.n, S, open_slot + 8 * (long long)F.l0,
+                             conn_slot + 16 * (long long)F.l0, in_conn_slot + 2 * F.l0, n_open, n_conn, bits);
+  out[4 * f] = st;
+  out[4 * f + 1] = st ? 0 : n_open;
+  out[4 * f + 2] = st ? 0 : n_conn;
+  out[4 * f + 3] = (int)bits;
+}
+}  // namespace edges
+}  // namespace pus
+
+#define ECHK(call)                                                                                          \
+  do {                                                                                                      \
+    cudaError_t e__ = (call);                                                                               \
+    if (e__ != cudaSuccess) { g_err = std::string("pus_popup_edges: ") + #call + ": " + cudaGetErrorString(e__); return -1; } \
+  } while (0)
+
+extern "C" int pus_popup_edges(int device, int n_frames, const unsigned char* labels, int width, int height,
+                               const int* line_ptr, const float* lines, const pus_edge_params* params, int* status,
+                               int* open_counts, int* connect_counts, float* open_segs, float* connect_segs,
+                               int* open_in_connect, long long open_capacity, long long connect_capacity) {
+  using namespace pus::edges;
+  auto refuse = [](const std::string& why) { g_err = "pus_popup_edges: " + why; return -1; };
+  const std::string why = args_error(n_frames, labels, width, height, line_ptr, lines, params, status, open_counts,
+                                      connect_counts);
+  if (!why.empty()) return refuse(why);
+  {
+    int ndev = 0;
+    cudaError_t de = cudaGetDeviceCount(&ndev);
+    if (de != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
+      return refuse("no CUDA device usable; libpopup_gpu has no CPU fallback");
+  }
+  if (n_frames == 0) return 0;
+  ECHK(cudaSetDevice(device));
+  const pus_edge_params P = *params;
+  const int ds = P.downsample_contour ? 1 : 0;
+  const int w = ds ? half_size(width) : width, h = ds ? half_size(height) : height;
+  const int kd = ds ? 8 : P.dilation_distance, ke = ds ? 8 : P.erosion_distance;
+  const long long cells = (long long)w * h, n_lines = line_ptr[n_frames];
+  DevBuf<unsigned char> d_lab, d_a, d_b, d_flags;
+  DevBuf<int> d_cnt, d_tab, d_nodes, d_objs, d_out, d_inc;
+  DevBuf<Frame> d_fr;
+  DevBuf<float> d_cpts, d_lines, d_bounds, d_open, d_conn;
+  DevBuf<Lin> d_rows;
+  DevBuf<Ivl> d_ivl;
+  const size_t lab_n = (size_t)n_frames * width * height, map_n = (size_t)n_frames * cells;
+  ECHK(d_lab.alloc(lab_n));
+  ECHK(d_a.alloc(map_n));
+  ECHK(d_b.alloc(map_n));
+  ECHK(d_cnt.alloc(n_frames));
+  ECHK(cudaMemcpy(d_lab.p, labels, lab_n, cudaMemcpyHostToDevice));
+  ECHK(cudaMemset(d_cnt.p, 0, n_frames * sizeof(int)));
+  const unsigned gb = (unsigned)((map_n + 255) / 256);
+  edge_box_kernel<<<gb, 256>>>(n_frames, d_lab.p, width, height, ds, w, h, kd, 1, 1, 0, d_a.p);
+  edge_box_kernel<<<gb, 256>>>(n_frames, d_a.p, w, h, 0, w, h, kd, 0, 1, 0, d_b.p);
+  edge_box_kernel<<<gb, 256>>>(n_frames, d_b.p, w, h, 0, w, h, ke, 1, 0, 0, d_a.p);
+  edge_box_kernel<<<gb, 256>>>(n_frames, d_a.p, w, h, 0, w, h, ke, 0, 0, 1, d_b.p);
+  ECHK(cudaGetLastError());
+  const long long n_cells = (long long)n_frames * (w - 1) * (h - 1);
+  edge_count_kernel<<<(unsigned)((n_cells + 255) / 256), 256>>>(n_frames, d_b.p, w, h, d_cnt.p);
+  ECHK(cudaGetLastError());
+  std::vector<int> cnt(n_frames);
+  ECHK(cudaMemcpy(cnt.data(), d_cnt.p, n_frames * sizeof(int), cudaMemcpyDeviceToHost));
+  // scratch layout
+  std::vector<Frame> fr(n_frames);
+  long long node = 0, obj = 0, cpt = 0, ivl = 0;
+  for (int f = 0; f < n_frames; f++) {
+    Frame& F = fr[f];
+    F.node_cap = (int)node_cap_of(cnt[f]);
+    F.obj_cap = (int)obj_cap_of(cnt[f]);
+    F.cpt_cap = (int)cpt_cap_of(cnt[f]);
+    F.n = line_ptr[f + 1] - line_ptr[f];
+    F.ivl_cap = (int)ivl_cap_of(F.n);
+    F.l0 = line_ptr[f];
+    F.node = node; F.obj = obj; F.cpt = cpt; F.ivl = ivl; F.line = F.l0; F.tab = 2 * cells * f;
+    node += F.node_cap; obj += F.obj_cap; cpt += F.cpt_cap; ivl += F.ivl_cap;
+  }
+  ECHK(d_fr.alloc(n_frames));
+  ECHK(d_tab.alloc(2 * map_n));
+  ECHK(d_nodes.alloc(2 * node));
+  ECHK(d_objs.alloc(3 * obj));
+  ECHK(d_flags.alloc(2 * obj));
+  ECHK(d_cpts.alloc(2 * cpt));
+  ECHK(d_lines.alloc(4 * n_lines));
+  // per frame of n lines: 2 n work and open rows, 4 n connected rows (Sel in pus_edges.cuh)
+  ECHK(d_rows.alloc(2 * n_lines));
+  ECHK(d_bounds.alloc(2 * n_lines));
+  ECHK(d_ivl.alloc(2 * ivl));
+  ECHK(d_open.alloc(8 * n_lines));
+  ECHK(d_conn.alloc(16 * n_lines));
+  ECHK(d_inc.alloc(2 * n_lines));
+  ECHK(d_out.alloc(4 * (size_t)n_frames));
+  ECHK(cudaMemcpy(d_fr.p, fr.data(), n_frames * sizeof(Frame), cudaMemcpyHostToDevice));
+  if (n_lines > 0) ECHK(cudaMemcpy(d_lines.p, lines, 4 * n_lines * sizeof(float), cudaMemcpyHostToDevice));
+  ECHK(cudaMemset(d_tab.p, 0xff, 2 * map_n * sizeof(int)));
+  edge_frame_kernel<<<n_frames, 1>>>(n_frames, P, width, height, d_b.p, w, h, d_fr.p, d_tab.p, d_nodes.p,
+                                                   d_objs.p, d_flags.p, d_cpts.p, d_lines.p, d_rows.p, d_bounds.p, d_ivl.p,
+                                                   d_open.p, d_conn.p, d_inc.p, d_out.p);
+  ECHK(cudaGetLastError());
+  std::vector<int> out(4 * (size_t)n_frames);
+  ECHK(cudaMemcpy(out.data(), d_out.p, out.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  long long tot_open = 0, tot_conn = 0;
+  int found = 0;
+  for (int f = 0; f < n_frames; f++) {
+    status[f] = out[4 * f];
+    open_counts[f] = out[4 * f + 1];
+    connect_counts[f] = out[4 * f + 2];
+    tot_open += open_counts[f];
+    tot_conn += connect_counts[f];
+    found += status[f] == 0;
+  }
+  if ((open_segs && open_capacity < tot_open) || (connect_segs && connect_capacity < tot_conn))
+    return refuse("a capacity is smaller than its number of segments");
+  if (!open_segs && !connect_segs) return found;   // size query
+  std::vector<float> os(8 * (size_t)n_lines), cs(16 * (size_t)n_lines);
+  std::vector<int> inc(2 * (size_t)n_lines);
+  if (n_lines > 0) {
+    ECHK(cudaMemcpy(os.data(), d_open.p, os.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    ECHK(cudaMemcpy(cs.data(), d_conn.p, cs.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    ECHK(cudaMemcpy(inc.data(), d_inc.p, inc.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  }
+  long long po = 0, pc = 0;
+  for (int f = 0; f < n_frames; f++) {
+    const long long l0 = line_ptr[f];
+    if (open_segs) std::memcpy(open_segs + 4 * po, os.data() + 8 * l0, 4 * (size_t)open_counts[f] * sizeof(float));
+    if (open_in_connect) std::memcpy(open_in_connect + po, inc.data() + 2 * l0, (size_t)open_counts[f] * sizeof(int));
+    if (connect_segs) std::memcpy(connect_segs + 4 * pc, cs.data() + 16 * l0, 4 * (size_t)connect_counts[f] * sizeof(float));
+    po += open_counts[f];
+    pc += connect_counts[f];
+  }
+  return found;
 }
