@@ -368,7 +368,8 @@ int pus_popup_depth(int device, int n_frames, const int* plane_ptr, const int* p
 /* popup_plane::edge_get_polygons (PUW/libs/select_edge.cpp:66-406) with the Python stages it runs through an embedded
  * interpreter, pop_up_fun.python_get_contours and interval_tree_optimization (pop_up_python/python/pop_up_python/
  * pop_up_fun.py:85-205), batched over frames, on the device: which of a frame's detected lines form the ground-wall
- * boundary, given the CNN label map.  The line detector itself stays with the caller.
+ * boundary, given the CNN label map.  The lines come from pus_popup_lines (below) or the caller's own detector.
+ * PUS_POPUP_MAX_LINES stays this call's limit even though pus_popup_lines may give a frame more lines.
  *   labels[n_frames][height][width]   the label maps, ground 255 (any uint8 values are taken)
  *   line_ptr[n_frames+1], lines[n][4]   CSR offsets and the frames' detected lines x1 y1 x2 y2 (float pixels)
  *   params   popup_plane's members (popup_plane.h:178-200); NULL is refused
@@ -422,6 +423,61 @@ int pus_popup_edges(int device, int n_frames, const unsigned char* labels, int w
                     const float* lines, const pus_edge_params* params, int* status, int* open_counts, int* connect_counts,
                     float* open_segs, float* connect_segs, int* open_in_connect, long long open_capacity,
                     long long connect_capacity);
+
+/* ---- line detection (float32) ------------------------------------------------------------------ */
+/* The detector half of popup_plane::get_ground_edges (popup_plane.cpp:753-770): grey, contrast and
+ * line_lbd_detect::detect_raw_lines with use_LSD = false (main_3d.cpp:417-424), i.e. line_lbd's EDLines
+ * (binary_descriptor.cpp: detectImpl, OctaveKeyLines, EDLineDetector::EdgeDrawing / EDline) in the configuration the SLAM
+ * pipeline runs: one octave, the EDLineDetector() defaults (gradient threshold 80, anchor threshold 8, scan interval 2,
+ * minimum line length 15, fit error threshold 1.6, TryTime 6, SkipEdgePoint 2), an all-ones mask.  Batched over frames.
+ *   images[n_frames][height][width][channels]   channels 3 (BGR, as pus_popup_clouds takes them) or 1 (grey, used as is)
+ *   downsample   popup_plane's use_fast_edges_detection: detect on the 0.5x image, lines scaled by 2
+ * Outputs: counts[n_frames] and status[n_frames] (always written); lines[total][4] x1 y1 x2 y2, packed in frame order,
+ * so that the prefix sum of counts is pus_popup_edges' line_ptr and lines its lines as is.  lines = NULL is a size query;
+ * capacity is in rows and too small a one fails with a message.  Returns the total number of lines.
+ *   status 0 lines found (possibly none); 1 EdgeDrawing's arrays would overflow -- more anchors than N / 5, more edge
+ *          pixels than N / 5 in either half, or more chains than N / 100 (N the detection image's pixels).  The reference
+ *          writes past its arrays before it checks these limits, then prints an error, and detectImpl ignores the -1:
+ *          the frame gets no lines.  Here likewise: status 1, no lines.
+ * Stages, pinned (OpenCV 4.13 on 8-bit data):
+ *   1 grey: cvtColor BGR2GRAY, (3735 B + 19235 G + 9798 R + 2^14) >> 15.
+ *   2 contrast: if the integer pixel sum times 1.0 / N (double) is below 90, equalizeHist: LUT from the first non-empty
+ *     bin i (0 there), saturate_cast<uchar>(float(cumulative count) * (255.f / (N - hist[i]))), round half to even; an
+ *     image of one value maps every pixel to itself.
+ *   3 downsample: resize 0.5 x INTER_LINEAR, which OpenCV runs on 8U as its area path: (a + b + c + d + 2) >> 2.  Odd
+ *     sizes are refused in this mode.
+ *   4 blur: GaussianBlur 5 x 5, sigma 1, the bit-exact fixed-point filter (14 62 104 62 14) / 256 per pass, rows kept
+ *     with 8 fractional bits, columns rounded from 16; BORDER_REFLECT_101.
+ *   5 Sobel 3 x 3 to CV_16S (BORDER_REFLECT_101), |dx| + |dy|, THRESH_TOZERO at 81, / 4 as saturate_cast<short>(v * 0.25f)
+ *     (round half to even: 82 -> 20, 86 -> 22); direction Horizontal where |dx| < |dy|.
+ *   6 anchors scanned column-major (x outer, y inner), both from 1 in steps of 2.
+ *   7 edge drawing in anchor order: neighbour comparisons on the gradient's low byte ((unsigned char) of the short), the
+ *     loop condition on the full short; the last position carried from walk to walk; the anchor unmarked between the two
+ *     half-walks and its second copy skipped in the chain; chains under 16 pixels dropped with their pixels left marked.
+ *   8 per chain: LeastSquaresLineFit_ (both forms: Mat_<float> matrices, products accumulated in double and rounded to
+ *     float once as OpenCV's gemm, ATA + tmp a float add, the solve in double; a singular fit gives NaN, which fails every
+ *     comparison), the extension with up to 3 popped-back outliers and TryTime, LineValidation_ and nfa in double,
+ *     endpoints computed in double and stored as float.
+ *   9 OctaveKeyLines' endpoint swap: the float direction against double multiples of M_PI (a direction that rounds to
+ *     float pi lies beyond M_PI and takes no range); then keylines_to_mat's float rows (times 2 with downsample).
+ * Deviations, where the reference is undefined:
+ *   - the overflow cases above (status 1);
+ *   - the mask test reads the all-ones mask at projected endpoints that can lie just outside the image: here no line is
+ *     ever removed;
+ *   - an initial fit that ends NaN at the end of a chain makes the reference read past the chain to form a line that its
+ *     validation always rejects: here the chain simply ends;
+ *   - EDline sizes its line index array 5 x chains and writes past it when a frame has more lines: here every line is
+ *     kept.
+ * The transcendentals of the validation (atan2 and nfa's log, exp, sinh, pow, log10) are CUDA's on the device and
+ * glibc's on the host, which may differ by an ulp; only the decisions they feed (nfa > 0, |angle difference| <
+ * 0.392699, the direction ranges) reach the output.  There is no per-frame line cap: a frame may give more than
+ * PUS_POPUP_MAX_LINES lines, which pus_popup_edges refuses as before.  Refused with a message, nothing launched: NULL
+ * images, status or counts, channels other than 1 or 3, odd sizes with downsample, a detection image below 3 x 3, more
+ * than PUS_POPUP_LINES_MAX_PIXELS pixels in a frame (pixel indices are 32-bit).  Deterministic (no floating-point
+ * atomics): repeated calls and any split of the batch give the same bytes.  No CPU fallback. */
+#define PUS_POPUP_LINES_MAX_PIXELS (1LL << 28)
+long long pus_popup_lines(int device, int n_frames, const unsigned char* images, int width, int height, int channels,
+                          int downsample, int* status, int* counts, float* lines, long long capacity);
 
 /* ---- device-resident measurement refresh and polygon re-projection (SURVEY.md 8f.1) -------- */
 /* Mapper_mono::update_plane_measurement (pop_planar_slam/src/Mapping.cpp:590-607): after a solve every past

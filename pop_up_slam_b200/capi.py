@@ -826,3 +826,40 @@ def popup_edges(lib, labels, line_ptr, lines, params=None, segments=True, capaci
         call(o, c, i, cap)
         res.update(open=o[:tot[0]], connect=c[:tot[1]], open_in_connect=i[:tot[0]])
     return res
+
+
+def popup_lines(lib, images, downsample=False, lines=True, capacity=None, prefix="pus_", device=0):
+    """popup_plane::get_ground_edges' line detection (grey, contrast, EDLines) batched over frames (pus_popup_lines,
+    include/popup_gpu.h).
+
+    images [n_frames, height, width, 3] uint8 BGR or [n_frames, height, width] grey.  Returns a dict: status, counts
+    [n_frames] int32, line_ptr [n_frames+1] and, unless lines=False (a size query), lines [total, 4] float32 -- line_ptr
+    and lines are popup_edges' arguments as they are.  capacity (rows) fills a buffer of that size instead."""
+    images = np.ascontiguousarray(images, dtype=np.uint8)
+    if images.ndim not in (3, 4):
+        raise ValueError("images must be [n, h, w] or [n, h, w, c]")
+    nf, h, w = images.shape[:3]
+    ch = 1 if images.ndim == 3 else images.shape[3]
+    st, cnt = np.zeros(nf, np.int32), np.zeros(nf, np.int32)
+    fn = getattr(lib, prefix + "popup_lines")
+    fn.restype = C.c_longlong
+    fn.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, c_int_p, c_int_p, c_float_p,
+                   C.c_longlong]
+    err = getattr(lib, prefix + "last_error", None) or getattr(lib, prefix + "popup_last_error")
+    err.restype = C.c_char_p
+
+    def call(out, cap):
+        rc = fn(device, nf, images.ctypes.data if images.size else None, w, h, ch, int(bool(downsample)), _ip(st),
+                _ip(cnt), None if out is None else out.ctypes.data_as(c_float_p), int(cap))
+        if rc < 0:
+            raise ApiError((err() or b"?").decode())
+        return rc
+
+    total = call(None, 0)
+    res = dict(status=st.copy(), counts=cnt.copy(), line_ptr=np.concatenate([[0], np.cumsum(cnt)]).astype(np.int32))
+    if lines:
+        cap = total if capacity is None else int(capacity)
+        out = np.empty((max(cap, 0), 4), np.float32)
+        call(out, cap)
+        res["lines"] = out[:total]
+    return res

@@ -1,0 +1,370 @@
+// pus_lines.cu -- popup_plane::get_ground_edges' line detection (popup_plane.cpp:753-770 and line_lbd's EDLines,
+// binary_descriptor.cpp:483-585, 792-1144, 1579-2870) batched over frames on the device, behind pus_popup_lines.
+// Per-pixel kernels make the grey image, the per-frame histogram and LUT, the optional 0.5x image, the 5 x 5 blur,
+// the Sobel maps and one packed record per pixel; one block per frame compacts the anchors in the reference's
+// column-major scan order; one thread per frame replays the order-dependent walk (pus_lines.cuh); one thread per chain
+// extracts its lines; a per-frame prefix sum over the chains and a scatter pack them in frame and chain order.
+// Compiled with --fmad=false so the double arithmetic of the fits rounds like the reference's scalar code.
+#include <cuda_runtime.h>
+
+#include <climits>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "../../include/popup_gpu.h"
+#include "pus_lines.cuh"
+
+namespace pus {
+extern thread_local std::string g_err;
+
+namespace lines {
+template <class T>
+struct Buf {   // a device allocation freed on every return path
+  T* p = nullptr;
+  ~Buf() { if (p) cudaFree(p); }
+  cudaError_t alloc(size_t n) { return cudaMalloc(&p, (n > 0 ? n : 1) * sizeof(T)); }
+};
+
+struct Dims {
+  int W, H, C, ds, w, h;          // input size and channels, halving, detection size
+  long long N, n;                 // input and detection pixels per frame
+  int plim, clim, hcap, nslot;    // pix_limit, chain_limit, half_cap, line_slots of n
+};
+
+__device__ __forceinline__ int refl(int p, int n) { return p < 0 ? -p : (p >= n ? 2 * n - 2 - p : p); }
+
+// cvtColor BGR2GRAY on 8U (OpenCV's fixed point, 15 fractional bits) or a copy; the frame's histogram in shared memory
+__global__ void grey_hist_kernel(Dims D, const unsigned char* __restrict__ img, unsigned char* __restrict__ grey,
+                                 int* __restrict__ hist) {
+  __shared__ int sh[256];
+  const int f = blockIdx.y;
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) sh[i] = 0;
+  __syncthreads();
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < D.N) {
+    const long long q = (long long)f * D.N + p;
+    int v;
+    if (D.C == 3) {
+      const unsigned char* s = img + 3 * q;
+      v = (s[0] * 3735 + s[1] * 19235 + s[2] * 9798 + (1 << 14)) >> 15;
+    } else {
+      v = img[q];
+    }
+    grey[q] = (unsigned char)v;
+    atomicAdd(&sh[v], 1);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < 256; i += blockDim.x)
+    if (sh[i]) atomicAdd(&hist[256 * f + i], sh[i]);
+}
+
+// cv::mean < 90 (the integer sum times 1.0 / N in double) decides equalizeHist; its LUT, or the identity
+__global__ void lut_kernel(int n_frames, Dims D, const int* __restrict__ hist, unsigned char* __restrict__ lut,
+                           unsigned* __restrict__ bits) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= n_frames) return;
+  const int* hf = hist + 256 * f;
+  unsigned char* L = lut + 256 * f;
+  long long sum = 0;
+  for (int v = 0; v < 256; v++) sum += (long long)v * hf[v];
+  unsigned b = D.ds ? B_HALVED : 0;
+  for (int v = 0; v < 256; v++) L[v] = (unsigned char)v;
+  if ((double)sum * (1.0 / (double)D.N) < 90) {
+    b |= B_EQUALIZED;
+    int i = 0;
+    while (!hf[i]) ++i;
+    const int total = (int)D.N;
+    if (hf[i] == total) {
+      b |= B_ONE_BIN;
+    } else {
+      const float scale = (256 - 1.f) / (total - hf[i]);
+      int s = 0;
+      for (L[i++] = 0; i < 256; ++i) {
+        s += hf[i];
+        L[i] = (unsigned char)__float2int_rn((float)s * scale);   // <= 255: s <= total - hf[first]
+      }
+    }
+  }
+  bits[f] = b;
+}
+
+// the LUT, then with downsample OpenCV's 0.5x INTER_LINEAR on 8U (its area fast path: (a + b + c + d + 2) >> 2)
+__global__ void prep_kernel(int n_frames, Dims D, const unsigned char* __restrict__ grey,
+                            const unsigned char* __restrict__ lut, unsigned char* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= D.n * n_frames) return;
+  const int f = (int)(i / D.n), p = (int)(i % D.n);
+  const unsigned char* L = lut + 256 * f;
+  const unsigned char* g = grey + (long long)f * D.N;
+  if (D.ds) {
+    const int x = p % D.w, y = p / D.w;
+    const unsigned char* r0 = g + (long long)(2 * y) * D.W + 2 * x;
+    out[i] = (unsigned char)((L[r0[0]] + L[r0[1]] + L[r0[D.W]] + L[r0[D.W + 1]] + 2) >> 2);
+  } else {
+    out[i] = L[g[p]];
+  }
+}
+
+// GaussianBlur 5 x 5, sigma 1 on 8U: OpenCV 4.13's bit-exact separable filter (kernel 14 62 104 62 14 / 256, the row
+// pass kept with 8 fractional bits, the column pass rounded from 16), BORDER_REFLECT_101
+__constant__ int c_gk[5] = {14, 62, 104, 62, 14};
+__global__ void blur_row_kernel(int n_frames, Dims D, const unsigned char* __restrict__ in, unsigned short* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= D.n * n_frames) return;
+  const int p = (int)(i % D.n), x = p % D.w;
+  const unsigned char* row = in + (i - x);
+  int s = 0;
+  for (int j = 0; j < 5; j++) s += c_gk[j] * row[refl(x + j - 2, D.w)];
+  out[i] = (unsigned short)s;
+}
+__global__ void blur_col_kernel(int n_frames, Dims D, const unsigned short* __restrict__ in, unsigned char* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= D.n * n_frames) return;
+  const long long f0 = i - i % D.n;
+  const int p = (int)(i % D.n), x = p % D.w, y = p / D.w;
+  unsigned s = 0;
+  for (int j = 0; j < 5; j++) s += (unsigned)c_gk[j] * in[f0 + (long long)refl(y + j - 2, D.h) * D.w + x];
+  out[i] = (unsigned char)((s + (1u << 15)) >> 16);
+}
+
+// Sobel 3 x 3 to 16S (BORDER_REFLECT_101), |dx| + |dy|, THRESH_TOZERO at 81, / 4 (saturate_cast<short> of v * 0.25f:
+// round half to even), the direction |dx| < |dy|, and the packed record
+__global__ void grad_kernel(int n_frames, Dims D, const unsigned char* __restrict__ b, short* __restrict__ dx,
+                            short* __restrict__ dy, short* __restrict__ g, unsigned short* __restrict__ rec) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= D.n * n_frames) return;
+  const long long f0 = i - i % D.n;
+  const int p = (int)(i % D.n), x = p % D.w, y = p / D.w;
+  const int xm = refl(x - 1, D.w), xp = refl(x + 1, D.w);
+  const unsigned char* rm = b + f0 + (long long)refl(y - 1, D.h) * D.w;
+  const unsigned char* r0 = b + f0 + (long long)y * D.w;
+  const unsigned char* rp = b + f0 + (long long)refl(y + 1, D.h) * D.w;
+  const int gx = (rm[xp] + 2 * r0[xp] + rp[xp]) - (rm[xm] + 2 * r0[xm] + rp[xm]);
+  const int gy = (rp[xm] + 2 * rp[x] + rp[xp]) - (rm[xm] + 2 * rm[x] + rm[xp]);
+  const int ax = gx < 0 ? -gx : gx, ay = gy < 0 ? -gy : gy;
+  const int t = ax + ay > kGradThr + 1 ? ax + ay : 0;
+  const int q = t >> 2, r = t & 3;
+  const int gv = r < 2 ? q : (r > 2 ? q + 1 : q + (q & 1));
+  dx[i] = (short)gx;
+  dy[i] = (short)gy;
+  g[i] = (short)gv;
+  rec[i] = pack(gv, ax < ay);
+}
+
+// The anchors of one frame (binary_descriptor.cpp:1640-1666: w outer, h inner, both from 1 in steps of 2) compacted in
+// that order by a block-wide prefix sum; one block per frame.  n_anchor receives the full count, anchors the first plim.
+__global__ void __launch_bounds__(1024) anchor_kernel(Dims D, const short* __restrict__ g, const unsigned short* __restrict__ rec,
+                                                      int* __restrict__ anchors, int* __restrict__ n_anchor) {
+  __shared__ int warp_sum[32];
+  __shared__ int carry_s;
+  const int f = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  const short* gf = g + (long long)f * D.n;
+  const unsigned short* rf = rec + (long long)f * D.n;
+  int* af = anchors + (long long)f * D.plim;
+  const int nh = (D.h - 1) / 2, nw = (D.w - 1) / 2, npos = nw * nh;
+  if (t == 0) carry_s = 0;
+  __syncthreads();
+  for (int base = 0; base < npos; base += 1024) {
+    const int k = base + t;
+    int flag = 0, idx = 0;
+    if (k < npos) {
+      const int x = 1 + 2 * (k / nh), y = 1 + 2 * (k % nh);
+      idx = y * D.w + x;
+      const int v = gf[idx];
+      if (rf[idx] & kHoriz) flag = v >= gf[idx - D.w] + kAnchorThr && v >= gf[idx + D.w] + kAnchorThr;
+      else flag = v >= gf[idx - 1] + kAnchorThr && v >= gf[idx + 1] + kAnchorThr;
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, flag);
+    if (lane == 0) warp_sum[wid] = __popc(m);
+    __syncthreads();
+    if (wid == 0) {
+      int v = warp_sum[lane], s = v;
+      for (int o = 1; o < 32; o <<= 1) {
+        const int u = __shfl_up_sync(0xffffffffu, s, o);
+        if (lane >= o) s += u;
+      }
+      warp_sum[lane] = s - v;   // exclusive
+    }
+    __syncthreads();
+    const int carry = carry_s;
+    if (flag) {
+      const int pos = carry + warp_sum[wid] + __popc(m & ((1u << lane) - 1));
+      if (pos < D.plim) af[pos] = idx;
+    }
+    __syncthreads();
+    if (t == 1023) carry_s = carry + warp_sum[31] + __popc(m);
+    __syncthreads();
+  }
+  if (t == 0) n_anchor[f] = carry_s;
+}
+
+// The walk of each frame, one thread in a block of its own (the frames' walks diverge; a warp would serialise them)
+__global__ void walk_kernel(int n_frames, Dims D, unsigned short* rec, const int* __restrict__ anchors,
+                            const int* __restrict__ n_anchor, int* p1, int* p2, int* s1, int* s2, int* chain_px, int* sid,
+                            int* __restrict__ status, int* __restrict__ n_chains) {
+  const int f = blockIdx.x;
+  if (f >= n_frames || threadIdx.x) return;
+  unsigned bits = 0;
+  n_chains[f] = 0;
+  if (n_anchor[f] > D.plim) { status[f] = 1; return; }
+  const long long hc = D.hcap, sc = D.clim + 2;
+  Walk W{rec + (long long)f * D.n, D.w, D.h, p1 + f * hc, p2 + f * hc, s1 + f * sc, s2 + f * sc};
+  int nc = 0;
+  status[f] = draw_edges(W, anchors + (long long)f * D.plim, n_anchor[f], chain_px + 2 * hc * f, sid + sc * f, nc, bits);
+  n_chains[f] = status[f] ? 0 : nc;
+}
+
+// one thread per (frame, chain): the chain's lines into its slots
+__global__ void chain_kernel(int n_frames, Dims D, const unsigned short* __restrict__ rec, const short* __restrict__ dx,
+                             const short* __restrict__ dy, const int* __restrict__ chain_px, const int* __restrict__ sid,
+                             const int* __restrict__ n_chains, float* __restrict__ slots, int* __restrict__ chain_count) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long per = D.clim + 1;
+  if (i >= per * n_frames) return;
+  const int f = (int)(i / per), c = (int)(i % per);
+  if (c >= n_chains[f]) return;
+  const long long sc = D.clim + 2, off = (long long)f * D.n;
+  const int* sf = sid + sc * f;
+  const int s = sf[c], e = sf[c + 1];
+  unsigned bits = 0;
+  chain_count[i] = chain_lines(chain_px + 2 * D.hcap * f + s, e - s, rec + off, dx + off, dy + off, D.w, D.h,
+                               D.ds ? 2.0f : 1.0f, slots + 4 * ((long long)D.nslot * f + line_slot(s, c)), bits);
+}
+
+// per frame: the chains' first rows (prefix sum in chain order) and the frame's count
+__global__ void count_kernel(int n_frames, Dims D, const int* __restrict__ n_chains, int* __restrict__ chain_count,
+                             int* __restrict__ frame_count) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= n_frames) return;
+  int* cc = chain_count + (long long)(D.clim + 1) * f;
+  int s = 0;
+  for (int c = 0; c < n_chains[f]; c++) {
+    const int v = cc[c];
+    cc[c] = s;
+    s += v;
+  }
+  cc[n_chains[f]] = s;
+  frame_count[f] = s;
+}
+
+// one thread per (frame, chain): its rows to the packed output
+__global__ void scatter_kernel(int n_frames, Dims D, const int* __restrict__ sid, const int* __restrict__ n_chains,
+                               const int* __restrict__ chain_first, const long long* __restrict__ frame_first,
+                               const float* __restrict__ slots, float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long per = D.clim + 1;
+  if (i >= per * n_frames) return;
+  const int f = (int)(i / per), c = (int)(i % per);
+  if (c >= n_chains[f]) return;
+  const int r0 = chain_first[i], r1 = chain_first[i + 1];
+  const float4* src = (const float4*)(slots + 4 * ((long long)D.nslot * f + line_slot(sid[(D.clim + 2) * f + c], c)));
+  float4* dst = (float4*)(out + 4 * (frame_first[f] + r0));
+  for (int r = 0; r < r1 - r0; r++) dst[r] = src[r];
+}
+}  // namespace lines
+}  // namespace pus
+
+#define LCHK(call)                                                                                          \
+  do {                                                                                                      \
+    cudaError_t e__ = (call);                                                                               \
+    if (e__ != cudaSuccess) { g_err = std::string("pus_popup_lines: ") + #call + ": " + cudaGetErrorString(e__); return -1; } \
+  } while (0)
+
+extern "C" long long pus_popup_lines(int device, int n_frames, const unsigned char* images, int width, int height,
+                                     int channels, int downsample, int* status, int* counts, float* lines,
+                                     long long capacity) {
+  using namespace pus;
+  using namespace pus::lines;
+  auto refuse = [](const char* why) { g_err = std::string("pus_popup_lines: ") + why; return -1LL; };
+  if (n_frames < 0) return refuse("n_frames < 0");
+  if (!images && n_frames > 0) return refuse("images is NULL");
+  if (!status || !counts) return refuse("status and counts are required");
+  if (channels != 1 && channels != 3) return refuse("channels must be 1 (grey) or 3 (BGR)");
+  if (downsample && ((width & 1) || (height & 1))) return refuse("downsample needs even width and height");
+  const int w = downsample ? width / 2 : width, h = downsample ? height / 2 : height;
+  if (w < 3 || h < 3) return refuse("the detection image (after the optional halving) must be at least 3 x 3");
+  if ((long long)width * height > PUS_POPUP_LINES_MAX_PIXELS) return refuse("a frame has more than 2^28 pixels");
+  {
+    int ndev = 0;
+    cudaError_t de = cudaGetDeviceCount(&ndev);
+    if (de != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
+      return refuse("no CUDA device usable; libpopup_gpu has no CPU fallback");
+  }
+  if (n_frames == 0) return 0;
+  LCHK(cudaSetDevice(device));
+  Dims D;
+  D.W = width; D.H = height; D.C = channels; D.ds = downsample ? 1 : 0; D.w = w; D.h = h;
+  D.N = (long long)width * height; D.n = (long long)w * h;
+  D.plim = (int)pix_limit(D.n); D.clim = (int)chain_limit(D.n); D.hcap = (int)half_cap(D.n); D.nslot = (int)line_slots(D.n);
+  const long long F = n_frames, nn = F * D.n, per = D.clim + 1;
+  Buf<unsigned char> d_img, d_grey, d_lut, d_i8, d_b8;
+  Buf<unsigned short> d_h16, d_rec;
+  Buf<short> d_dx, d_dy, d_g;
+  Buf<int> d_hist, d_anc, d_nanc, d_p1, d_p2, d_s1, d_s2, d_cpx, d_sid, d_st, d_nc, d_cc, d_fc;
+  Buf<unsigned> d_bits;
+  Buf<float> d_slots, d_out;
+  Buf<long long> d_ff;
+  LCHK(d_img.alloc(F * D.N * channels));
+  LCHK(d_grey.alloc(F * D.N));
+  LCHK(d_hist.alloc(256 * F));
+  LCHK(d_lut.alloc(256 * F));
+  LCHK(d_bits.alloc(F));
+  LCHK(d_i8.alloc(nn));
+  LCHK(d_h16.alloc(nn));
+  LCHK(d_b8.alloc(nn));
+  LCHK(d_dx.alloc(nn));
+  LCHK(d_dy.alloc(nn));
+  LCHK(d_g.alloc(nn));
+  LCHK(d_rec.alloc(nn));
+  LCHK(d_anc.alloc(F * D.plim));
+  LCHK(d_nanc.alloc(F));
+  LCHK(d_p1.alloc(F * D.hcap));
+  LCHK(d_p2.alloc(F * D.hcap));
+  LCHK(d_s1.alloc(F * (D.clim + 2)));
+  LCHK(d_s2.alloc(F * (D.clim + 2)));
+  LCHK(d_cpx.alloc(2 * F * D.hcap));
+  LCHK(d_sid.alloc(F * (D.clim + 2)));
+  LCHK(d_st.alloc(F));
+  LCHK(d_nc.alloc(F));
+  LCHK(d_cc.alloc(F * per));
+  LCHK(d_fc.alloc(F));
+  LCHK(d_slots.alloc(4 * F * D.nslot));
+  LCHK(cudaMemcpy(d_img.p, images, (size_t)(F * D.N * channels), cudaMemcpyHostToDevice));
+  LCHK(cudaMemset(d_hist.p, 0, 256 * F * sizeof(int)));
+  grey_hist_kernel<<<dim3((unsigned)((D.N + 255) / 256), (unsigned)F), 256>>>(D, d_img.p, d_grey.p, d_hist.p);
+  lut_kernel<<<(unsigned)((F + 63) / 64), 64>>>(n_frames, D, d_hist.p, d_lut.p, d_bits.p);
+  const unsigned gb = (unsigned)((nn + 255) / 256);
+  prep_kernel<<<gb, 256>>>(n_frames, D, d_grey.p, d_lut.p, d_i8.p);
+  blur_row_kernel<<<gb, 256>>>(n_frames, D, d_i8.p, d_h16.p);
+  blur_col_kernel<<<gb, 256>>>(n_frames, D, d_h16.p, d_b8.p);
+  grad_kernel<<<gb, 256>>>(n_frames, D, d_b8.p, d_dx.p, d_dy.p, d_g.p, d_rec.p);
+  anchor_kernel<<<(unsigned)F, 1024>>>(D, d_g.p, d_rec.p, d_anc.p, d_nanc.p);
+  walk_kernel<<<(unsigned)F, 1>>>(n_frames, D, d_rec.p, d_anc.p, d_nanc.p, d_p1.p, d_p2.p, d_s1.p, d_s2.p, d_cpx.p,
+                                  d_sid.p, d_st.p, d_nc.p);
+  const unsigned gc = (unsigned)((F * per + 127) / 128);
+  chain_kernel<<<gc, 128>>>(n_frames, D, d_rec.p, d_dx.p, d_dy.p, d_cpx.p, d_sid.p, d_nc.p, d_slots.p, d_cc.p);
+  count_kernel<<<(unsigned)((F + 63) / 64), 64>>>(n_frames, D, d_nc.p, d_cc.p, d_fc.p);
+  LCHK(cudaGetLastError());
+  std::vector<int> st(F), fc(F);
+  LCHK(cudaMemcpy(st.data(), d_st.p, F * sizeof(int), cudaMemcpyDeviceToHost));
+  LCHK(cudaMemcpy(fc.data(), d_fc.p, F * sizeof(int), cudaMemcpyDeviceToHost));
+  std::vector<long long> ff(F);
+  long long total = 0;
+  for (int f = 0; f < n_frames; f++) {
+    status[f] = st[f];
+    counts[f] = st[f] ? 0 : fc[f];
+    ff[f] = total;
+    total += counts[f];
+  }
+  if (!lines) return total;   // size query
+  if (capacity < total) return refuse("capacity is smaller than the number of lines");
+  if (total == 0) return 0;
+  LCHK(d_ff.alloc(F));
+  LCHK(d_out.alloc(4 * total));
+  LCHK(cudaMemcpy(d_ff.p, ff.data(), F * sizeof(long long), cudaMemcpyHostToDevice));
+  scatter_kernel<<<gc, 128>>>(n_frames, D, d_sid.p, d_nc.p, d_cc.p, d_ff.p, d_slots.p, d_out.p);
+  LCHK(cudaGetLastError());
+  LCHK(cudaMemcpy(lines, d_out.p, 4 * total * sizeof(float), cudaMemcpyDeviceToHost));
+  return total;
+}
