@@ -479,6 +479,94 @@ int pus_popup_edges(int device, int n_frames, const unsigned char* labels, int w
 long long pus_popup_lines(int device, int n_frames, const unsigned char* images, int width, int height, int channels,
                           int downsample, int* status, int* counts, float* lines, long long capacity);
 
+/* ---- pop-up session: whole frames, device-resident ------------------------------------------------------------------ */
+/* main_3d's per-frame pop-up (main_3d.cpp:417-454 on popup_plane) over a batch of frames in one call, with intermediates kept
+ * on the device, scratch reused across runs and no host loop between the stages.  Per frame, in main_3d's order:
+ *   1 lines (pus_popup_lines, downsample = fast_edges);  2 edges (pus_popup_edges);  3 the fit, mode 0, on the OPEN segments
+ *   (pus_popup_fit_frames);  4 get_plane_equation's actual-index filter on its good flags (popup_plane.cpp:629-635 with
+ *   get_ground_edges' actual_plane_indices_inall = {0} u {open_in_connect + 1}, :792-794): open wall s stays good only when
+ *   s is one of the frame's open_in_connect values;  5 polygons on the OPEN segments (pus_popup_polygons; the reference's
+ *   get_plane_equation calls find_2d_3d_closed_polygon on the list it fits, :551, 607), so their rows are the fit's;
+ *   6 clouds of the good rows (pus_popup_clouds) from their cut polygons when walllength_threshold > 0 and their bound ones
+ *   otherwise (:821-823), given the images when they are BGR (and with them the 960-wide border rule; a grey session gives
+ *   the clouds no images, so colour 0 and no border rule, as the stage call without images);  7 with want_depth the depth map of the good rows'
+ *   bound polygons (pus_popup_depth).  Each output equals, bit for bit, what those stage calls give for the same frames
+ *   with this glue between them.  A frame without open segments has no good planes and no clouds, not even the ground
+ *   (the reference's ground_seg2d_lines.rows() > 0 branch, :553, 645-650).  cloud_projected_plane is not built (it is
+ *   always zero on this path, :44, 834).
+ * Inputs (each a host or a device pointer, told apart by cudaPointerGetAttributes; host data goes through the session's
+ * pinned staging, device data is read in place, ordered on the session's stream): images [n][height][width][channels]
+ * (BGR or grey), labels [n][height][width] (ground 255), Ts [n][16] row-major camera-to-world.
+ * Per-frame outcomes instead of whole-batch refusals (other frames are unaffected):
+ *   status[f]        0 planes popped up (possibly none); 1 the frame's lines are ones pus_popup_edges refuses (more than
+ *                    PUS_POPUP_MAX_LINES, or a coordinate not finite): the edge stage is not run for it; 2 more than
+ *                    PUS_POPUP_MAX_SEGMENTS open segments.  A frame with a non-zero status has no segments, no good planes
+ *                    and no clouds; its fit rows are the one empty ground row of a frame without segments.
+ *   line_status[f]   pus_popup_lines' status (0 / 1), line_counts[f] its counts
+ *   edge_status[f]   pus_popup_edges' status (0-5), -1 where status is 1
+ *   plane_status[p]  per good plane, bit 0: its cloud polygon has more than PUS_POPUP_MAX_VERTICES vertices or a coordinate
+ *                    beyond PUS_POPUP_MAX_COORD (checked before the truncation): the plane gets no points and no label
+ *                    pixels; bit 1: the same for its bound polygon, which the depth map then does not draw.
+ * Outputs, packed in frame order as the stage calls pack them (pus_popup_frames; rows r of frame f run from
+ * open_ptr[f] + f to open_ptr[f + 1] + f, row 0 of a frame its ground): the open and connected segments with
+ * open_in_connect; per row planes_world, planes_sensor, dist and good after the filter; per row the bound, cut and world
+ * polygons (CSR offsets bound_ptr / cut_ptr / world_ptr); good_ptr [n + 1] / good_rows [n_good], the frames'
+ * good_plane_indices (row indices within the frame); per good plane its cloud's count and offset into xyz / rgb; labels
+ * [n][height][width] and depth [n][height][width] when asked for.
+ * Sizing: buffers only grow (by at least half their size), host and device inputs take the same buffers.  A run
+ * synchronises with the host four times to read back totals (the line total with the edge scratch, the open / connected
+ * segment totals, the good planes with the polygon and box totals, the point total).  The buffers sized by the batch shape
+ * never grow again; those sized by these totals grow only when a total exceeds what the buffers hold.  So a run of the
+ * same frames as an earlier one performs no cudaMalloc / cudaFree, and neither does one of other frames of the same shape
+ * whose totals fit (pus_popup_session_memory counts the allocations).  Deterministic, no floating-point atomics: repeated runs, any split of
+ * the batch and reuse across batch sizes give the same bytes.
+ * Refused with a message, nothing launched, the session still usable: a NULL session or input, n_frames < 0, and at create
+ * a config that the stage calls would refuse (channels, sizes below 4 x 4, odd sizes with fast_edges, or with
+ * downsample_poly and labels or depth, kernel sizes below 1, non-finite K / invK) or want_rgb with grey images.
+ * A single-threaded object; no CPU fallback. */
+typedef void* pus_popup_session;
+typedef struct pus_popup_config {
+  float K[9], invK[9];                 /* row-major */
+  int width, height, channels;         /* fixed for the session; channels 1 (grey) or 3 (BGR) */
+  int fast_edges;                      /* popup_plane::use_fast_edges_detection: pus_popup_lines' downsample */
+  pus_edge_params edges;               /* as pus_popup_edges */
+  float plane_cam_dist_thre;           /* get_plane_equation */
+  float ceiling_threshold, walllength_threshold;   /* main_3d: 5.0, 3.0 */
+  int downsample_poly;                 /* generate_cloud's and get_depth_map_good's downsample; main_3d: 1 */
+  float depth_thre;                    /* generate_cloud's; main_3d: 10.0 */
+  int want_rgb, want_labels, want_depth;           /* optional outputs */
+} pus_popup_config;
+typedef struct pus_popup_frames {
+  int n_frames, n_rows, n_good;
+  long long n_open, n_connect, n_bound, n_cut, n_world, n_points;
+  int *status, *line_status, *line_counts, *edge_status;         /* [n_frames] */
+  int *open_ptr, *connect_ptr;                                   /* [n_frames + 1] */
+  float *open_segs, *connect_segs;                               /* [n_open][4], [n_connect][4] */
+  int* open_in_connect;                                          /* [n_open] */
+  float *planes_world, *planes_sensor, *dist;                    /* [n_rows][4], [n_rows][4], [n_rows] */
+  int* good;                                                     /* [n_rows] */
+  int *bound_ptr, *cut_ptr, *world_ptr;                          /* [n_rows + 1] */
+  float *bound2d, *cut2d, *world3d;                              /* [n_bound][2], [n_cut][2], [n_world][3] */
+  int *good_ptr, *good_rows, *plane_status, *cloud_counts;       /* [n_frames + 1], [n_good] x 3 */
+  long long* cloud_offsets;                                      /* [n_good] */
+  float* xyz;                                                    /* [n_points][3] */
+  unsigned char *rgb, *labels;                                   /* [n_points][3] (r, g, b); [n_frames][height][width] */
+  float* depth;                                                  /* [n_frames][height][width] */
+} pus_popup_frames;
+int pus_popup_session_create(int device, const pus_popup_config* config, pus_popup_session* out);
+int pus_popup_session_destroy(pus_popup_session s);
+/* run on this CUDA stream (cudaStream_t as void*); NULL: the session's own stream */
+int pus_popup_session_set_stream(pus_popup_session s, void* cuda_stream);
+int pus_popup_session_run(pus_popup_session s, int n_frames, const unsigned char* images, const unsigned char* labels,
+                          const float* Ts);
+/* the last successful run's counts and device pointers (valid until the next run or destroy) */
+int pus_popup_session_result(pus_popup_session s, pus_popup_frames* out);
+/* copies every output whose pointer in dst is non-NULL (host or device memory, sized from the result's counts) on the
+ * session's stream, then synchronises once */
+int pus_popup_session_download(pus_popup_session s, pus_popup_frames* dst);
+/* device and pinned allocations made so far, and the bytes they hold */
+int pus_popup_session_memory(pus_popup_session s, long long* allocations, long long* reserved_bytes);
+
 /* ---- device-resident measurement refresh and polygon re-projection (SURVEY.md 8f.1) -------- */
 /* Mapper_mono::update_plane_measurement (pop_planar_slam/src/Mapping.cpp:590-607): after a solve every past
  * frame re-pops its wall planes from its ground segments with the frame's LATEST pose estimate

@@ -863,3 +863,156 @@ def popup_lines(lib, images, downsample=False, lines=True, capacity=None, prefix
         call(out, cap)
         res["lines"] = out[:total]
     return res
+
+
+class PopupConfig(C.Structure):
+    """pus_popup_config (include/popup_gpu.h)"""
+    _fields_ = [("K", C.c_float * 9), ("invK", C.c_float * 9), ("width", C.c_int), ("height", C.c_int),
+                ("channels", C.c_int), ("fast_edges", C.c_int), ("edges", EdgeParams), ("plane_cam_dist_thre", C.c_float),
+                ("ceiling_threshold", C.c_float), ("walllength_threshold", C.c_float), ("downsample_poly", C.c_int),
+                ("depth_thre", C.c_float), ("want_rgb", C.c_int), ("want_labels", C.c_int), ("want_depth", C.c_int)]
+
+
+# (field, dtype, per-element shape, length as a function of the result's counts)
+_FRAME_OUTPUTS = [
+    ("status", np.int32, (), "n"), ("line_status", np.int32, (), "n"), ("line_counts", np.int32, (), "n"),
+    ("edge_status", np.int32, (), "n"), ("open_ptr", np.int32, (), "n1"), ("connect_ptr", np.int32, (), "n1"),
+    ("open_segs", np.float32, (4,), "n_open"), ("connect_segs", np.float32, (4,), "n_connect"),
+    ("open_in_connect", np.int32, (), "n_open"), ("planes_world", np.float32, (4,), "n_rows"),
+    ("planes_sensor", np.float32, (4,), "n_rows"), ("dist", np.float32, (), "n_rows"), ("good", np.int32, (), "n_rows"),
+    ("bound_ptr", np.int32, (), "rows1"), ("cut_ptr", np.int32, (), "rows1"), ("world_ptr", np.int32, (), "rows1"),
+    ("bound2d", np.float32, (2,), "n_bound"), ("cut2d", np.float32, (2,), "n_cut"), ("world3d", np.float32, (3,), "n_world"),
+    ("good_ptr", np.int32, (), "n1"), ("good_rows", np.int32, (), "n_good"), ("plane_status", np.int32, (), "n_good"),
+    ("cloud_counts", np.int32, (), "n_good"), ("cloud_offsets", np.int64, (), "n_good"),
+    ("xyz", np.float32, (3,), "n_points"), ("rgb", np.uint8, (3,), "n_points"), ("labels", np.uint8, ("h", "w"), "n"),
+    ("depth", np.float32, ("h", "w"), "n")]
+_CT = {np.int32: C.c_int, np.float32: C.c_float, np.int64: C.c_longlong, np.uint8: C.c_ubyte}
+
+
+class PopupFrameResult(C.Structure):
+    """pus_popup_frames (include/popup_gpu.h)"""
+    _fields_ = [("n_frames", C.c_int), ("n_rows", C.c_int), ("n_good", C.c_int)] + [
+        (k, C.c_longlong) for k in ("n_open", "n_connect", "n_bound", "n_cut", "n_world", "n_points")] + [
+        (k, C.POINTER(_CT[t])) for k, t, _, _ in _FRAME_OUTPUTS]
+
+
+def popup_config(config):
+    """a PopupConfig from a dict (see PopupFrames)"""
+    c = dict(fast_edges=0, edges=None, plane_cam_dist_thre=10.0, ceiling_threshold=5.0, walllength_threshold=3.0,
+             downsample_poly=1, depth_thre=10.0, want_rgb=None, want_labels=0, want_depth=0)
+    c.update(config)
+    if c["want_rgb"] is None:
+        c["want_rgb"] = int(c["channels"] == 3)
+    cfg = PopupConfig()
+    cfg.K[:] = [float(v) for v in np.asarray(c["K"], np.float32).ravel()]
+    cfg.invK[:] = [float(v) for v in np.asarray(c["invK"], np.float32).ravel()]
+    for k in ("width", "height", "channels", "fast_edges", "downsample_poly", "want_rgb", "want_labels", "want_depth"):
+        setattr(cfg, k, int(c[k]))
+    for k in ("plane_cam_dist_thre", "ceiling_threshold", "walllength_threshold", "depth_thre"):
+        setattr(cfg, k, float(c[k]))
+    cfg.edges = EdgeParams(**dict(EDGE_DEFAULTS, **(c["edges"] or {})))
+    return cfg
+
+
+class PopupFrames:
+    """A pop-up session (pus_popup_session_*, include/popup_gpu.h): main_3d's per-frame pop-up over batches of frames.
+
+    config: K, invK [3, 3], width, height, channels (3 BGR, 1 grey) and optionally fast_edges, edges (a dict over
+    EDGE_DEFAULTS), plane_cam_dist_thre (10), ceiling_threshold (5), walllength_threshold (3), downsample_poly (True),
+    depth_thre (10), want_rgb (True with BGR), want_labels, want_depth (False).  run(images, labels, Ts) takes numpy arrays
+    and returns a dict of numpy arrays, or torch CUDA tensors and returns torch CUDA tensors, ordered on torch's current
+    stream."""
+
+    def __init__(self, lib, config, device=0):
+        self.lib = lib
+        cfg = popup_config(config)
+        self.config = cfg
+        vp = C.c_void_p
+        lib.pus_popup_session_create.argtypes = [C.c_int, C.POINTER(PopupConfig), C.POINTER(vp)]
+        lib.pus_popup_session_destroy.argtypes = [vp]
+        lib.pus_popup_session_set_stream.argtypes = [vp, vp]
+        lib.pus_popup_session_run.argtypes = [vp, C.c_int, vp, vp, vp]
+        lib.pus_popup_session_result.argtypes = [vp, C.POINTER(PopupFrameResult)]
+        lib.pus_popup_session_download.argtypes = [vp, C.POINTER(PopupFrameResult)]
+        lib.pus_popup_session_memory.argtypes = [vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]
+        lib.pus_last_error.restype = C.c_char_p
+        self.h = vp()
+        self._check(lib.pus_popup_session_create(int(device), C.byref(cfg), C.byref(self.h)))
+
+    def _check(self, rc):
+        if rc < 0:
+            raise ApiError((self.lib.pus_last_error() or b"?").decode())
+        return rc
+
+    def close(self):
+        if self.h:
+            self.lib.pus_popup_session_destroy(self.h)
+            self.h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def memory(self):
+        """(allocations made so far, bytes reserved) of the session's device and pinned buffers"""
+        a, b = C.c_longlong(), C.c_longlong()
+        self._check(self.lib.pus_popup_session_memory(self.h, C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+    def _check_shapes(self, img, lab, T):
+        """the library reads n frames of the configured size from each input: refuse arrays of another shape"""
+        c, n = self.config, img[0] if len(img) else -1
+        want = (n, c.height, c.width) + ((c.channels,) if c.channels == 3 else ())
+        if tuple(img) != want and not (c.channels == 1 and tuple(img) == want + (1,)):
+            raise ValueError(f"images must be {want}, not {tuple(img)}")
+        if tuple(lab) != (n, c.height, c.width):
+            raise ValueError(f"labels must be {(n, c.height, c.width)}, not {tuple(lab)}")
+        if tuple(T) not in ((n, 4, 4), (n, 16)):
+            raise ValueError(f"Ts must be ({n}, 4, 4), not {tuple(T)}")
+
+    def run(self, images, labels, Ts):
+        torch_in = type(images).__module__.startswith("torch")
+        if torch_in:
+            import torch
+            for t in (images, labels, Ts):
+                if not (t.is_cuda and t.is_contiguous()):
+                    raise ValueError("torch inputs must be contiguous CUDA tensors")
+            if images.dtype != torch.uint8 or labels.dtype != torch.uint8 or Ts.dtype != torch.float32:
+                raise ValueError("images and labels must be uint8, Ts float32")
+            n = images.shape[0]
+            self._check_shapes(tuple(images.shape), tuple(labels.shape), tuple(Ts.shape))
+            self._check(self.lib.pus_popup_session_set_stream(self.h, C.c_void_p(torch.cuda.current_stream().cuda_stream)))
+            ptrs = [t.data_ptr() or None for t in (images, labels, Ts)]
+        else:
+            images = np.ascontiguousarray(images, np.uint8)
+            labels = np.ascontiguousarray(labels, np.uint8)
+            Ts = np.ascontiguousarray(Ts, np.float32)
+            n = images.shape[0]
+            self._check_shapes(images.shape, labels.shape, Ts.shape)
+            self._check(self.lib.pus_popup_session_set_stream(self.h, None))
+            ptrs = [a.ctypes.data if a.size else None for a in (images, labels, Ts)]
+        self._check(self.lib.pus_popup_session_run(self.h, int(n), *ptrs))
+        res = PopupFrameResult()
+        self._check(self.lib.pus_popup_session_result(self.h, C.byref(res)))
+        cfg = self.config
+        size = dict(n=res.n_frames, n1=res.n_frames + 1, rows1=res.n_rows + 1, n_rows=res.n_rows, n_good=res.n_good,
+                    n_open=res.n_open, n_connect=res.n_connect, n_bound=res.n_bound, n_cut=res.n_cut, n_world=res.n_world,
+                    n_points=res.n_points, h=cfg.height, w=cfg.width)
+        dst, out = PopupFrameResult(), {}
+        for k, t, shape, count in _FRAME_OUTPUTS:
+            if not getattr(res, k):
+                continue
+            shp = (int(size[count]),) + tuple(int(size[s]) if isinstance(s, str) else s for s in shape)
+            if torch_in:
+                a = torch.empty(shp, dtype=getattr(torch, np.dtype(t).name), device=images.device)
+                p = a.data_ptr()
+            else:
+                a = np.empty(shp, t)
+                p = a.ctypes.data
+            if a.numel() if torch_in else a.size:
+                setattr(dst, k, C.cast(C.c_void_p(p), C.POINTER(_CT[t])))
+            out[k] = a
+        self._check(self.lib.pus_popup_session_download(self.h, C.byref(dst)))
+        return out

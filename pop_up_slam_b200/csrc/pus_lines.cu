@@ -14,23 +14,12 @@
 
 #include "../../include/popup_gpu.h"
 #include "pus_lines.cuh"
+#include "pus_stages.cuh"
 
 namespace pus {
 extern thread_local std::string g_err;
 
 namespace lines {
-template <class T>
-struct Buf {   // a device allocation freed on every return path
-  T* p = nullptr;
-  ~Buf() { if (p) cudaFree(p); }
-  cudaError_t alloc(size_t n) { return cudaMalloc(&p, (n > 0 ? n : 1) * sizeof(T)); }
-};
-
-struct Dims {
-  int W, H, C, ds, w, h;          // input size and channels, halving, detection size
-  long long N, n;                 // input and detection pixels per frame
-  int plim, clim, hcap, nslot;    // pix_limit, chain_limit, half_cap, line_slots of n
-};
 
 __device__ __forceinline__ int refl(int p, int n) { return p < 0 ? -p : (p >= n ? 2 * n - 2 - p : p); }
 
@@ -262,6 +251,72 @@ __global__ void scatter_kernel(int n_frames, Dims D, const int* __restrict__ sid
   float4* dst = (float4*)(out + 4 * (frame_first[f] + r0));
   for (int r = 0; r < r1 - r0; r++) dst[r] = src[r];
 }
+
+Dims make_dims(int width, int height, int channels, int downsample) {
+  Dims D;
+  D.W = width; D.H = height; D.C = channels; D.ds = downsample ? 1 : 0;
+  D.w = downsample ? width / 2 : width; D.h = downsample ? height / 2 : height;
+  D.N = (long long)width * height; D.n = (long long)D.w * D.h;
+  D.plim = (int)pix_limit(D.n); D.clim = (int)chain_limit(D.n); D.hcap = (int)half_cap(D.n); D.nslot = (int)line_slots(D.n);
+  return D;
+}
+
+#define WCHK(call)                        \
+  do {                                    \
+    const cudaError_t e__ = (call);       \
+    if (e__ != cudaSuccess) return e__;   \
+  } while (0)
+
+cudaError_t detect(cudaStream_t st, Alloc& A, int n_frames, const Dims& D, const unsigned char* d_img, Work& W) {
+  const long long F = n_frames, nn = F * D.n, per = D.clim + 1;
+  WCHK(A.get(W.grey, F * D.N));
+  WCHK(A.get(W.hist, 256 * F));
+  WCHK(A.get(W.lut, 256 * F));
+  WCHK(A.get(W.bits, F));
+  WCHK(A.get(W.i8, nn));
+  WCHK(A.get(W.h16, nn));
+  WCHK(A.get(W.b8, nn));
+  WCHK(A.get(W.dx, nn));
+  WCHK(A.get(W.dy, nn));
+  WCHK(A.get(W.g, nn));
+  WCHK(A.get(W.rec, nn));
+  WCHK(A.get(W.anc, F * D.plim));
+  WCHK(A.get(W.nanc, F));
+  WCHK(A.get(W.p1, F * D.hcap));
+  WCHK(A.get(W.p2, F * D.hcap));
+  WCHK(A.get(W.s1, F * (D.clim + 2)));
+  WCHK(A.get(W.s2, F * (D.clim + 2)));
+  WCHK(A.get(W.cpx, 2 * F * D.hcap));
+  WCHK(A.get(W.sid, F * (D.clim + 2)));
+  WCHK(A.get(W.st, F));
+  WCHK(A.get(W.nc, F));
+  WCHK(A.get(W.cc, F * per));
+  WCHK(A.get(W.fc, F));
+  WCHK(A.get(W.slots, 4 * F * D.nslot));
+  if (n_frames == 0) return cudaSuccess;
+  WCHK(cudaMemsetAsync(W.hist, 0, 256 * F * sizeof(int), st));
+  grey_hist_kernel<<<dim3((unsigned)((D.N + 255) / 256), (unsigned)F), 256, 0, st>>>(D, d_img, W.grey, W.hist);
+  lut_kernel<<<(unsigned)((F + 63) / 64), 64, 0, st>>>(n_frames, D, W.hist, W.lut, W.bits);
+  const unsigned gb = (unsigned)((nn + 255) / 256);
+  prep_kernel<<<gb, 256, 0, st>>>(n_frames, D, W.grey, W.lut, W.i8);
+  blur_row_kernel<<<gb, 256, 0, st>>>(n_frames, D, W.i8, W.h16);
+  blur_col_kernel<<<gb, 256, 0, st>>>(n_frames, D, W.h16, W.b8);
+  grad_kernel<<<gb, 256, 0, st>>>(n_frames, D, W.b8, W.dx, W.dy, W.g, W.rec);
+  anchor_kernel<<<(unsigned)F, 1024, 0, st>>>(D, W.g, W.rec, W.anc, W.nanc);
+  walk_kernel<<<(unsigned)F, 1, 0, st>>>(n_frames, D, W.rec, W.anc, W.nanc, W.p1, W.p2, W.s1, W.s2, W.cpx, W.sid, W.st, W.nc);
+  const unsigned gc = (unsigned)((F * per + 127) / 128);
+  chain_kernel<<<gc, 128, 0, st>>>(n_frames, D, W.rec, W.dx, W.dy, W.cpx, W.sid, W.nc, W.slots, W.cc);
+  count_kernel<<<(unsigned)((F + 63) / 64), 64, 0, st>>>(n_frames, D, W.nc, W.cc, W.fc);
+  return cudaGetLastError();
+}
+
+cudaError_t scatter(cudaStream_t st, int n_frames, const Dims& D, const Work& W, const long long* d_first, float* d_out) {
+  if (n_frames == 0) return cudaSuccess;
+  const unsigned gc = (unsigned)(((long long)n_frames * (D.clim + 1) + 127) / 128);
+  scatter_kernel<<<gc, 128, 0, st>>>(n_frames, D, W.sid, W.nc, W.cc, d_first, W.slots, d_out);
+  return cudaGetLastError();
+}
+#undef WCHK
 }  // namespace lines
 }  // namespace pus
 
@@ -293,62 +348,17 @@ extern "C" long long pus_popup_lines(int device, int n_frames, const unsigned ch
   }
   if (n_frames == 0) return 0;
   LCHK(cudaSetDevice(device));
-  Dims D;
-  D.W = width; D.H = height; D.C = channels; D.ds = downsample ? 1 : 0; D.w = w; D.h = h;
-  D.N = (long long)width * height; D.n = (long long)w * h;
-  D.plim = (int)pix_limit(D.n); D.clim = (int)chain_limit(D.n); D.hcap = (int)half_cap(D.n); D.nslot = (int)line_slots(D.n);
-  const long long F = n_frames, nn = F * D.n, per = D.clim + 1;
-  Buf<unsigned char> d_img, d_grey, d_lut, d_i8, d_b8;
-  Buf<unsigned short> d_h16, d_rec;
-  Buf<short> d_dx, d_dy, d_g;
-  Buf<int> d_hist, d_anc, d_nanc, d_p1, d_p2, d_s1, d_s2, d_cpx, d_sid, d_st, d_nc, d_cc, d_fc;
-  Buf<unsigned> d_bits;
-  Buf<float> d_slots, d_out;
-  Buf<long long> d_ff;
-  LCHK(d_img.alloc(F * D.N * channels));
-  LCHK(d_grey.alloc(F * D.N));
-  LCHK(d_hist.alloc(256 * F));
-  LCHK(d_lut.alloc(256 * F));
-  LCHK(d_bits.alloc(F));
-  LCHK(d_i8.alloc(nn));
-  LCHK(d_h16.alloc(nn));
-  LCHK(d_b8.alloc(nn));
-  LCHK(d_dx.alloc(nn));
-  LCHK(d_dy.alloc(nn));
-  LCHK(d_g.alloc(nn));
-  LCHK(d_rec.alloc(nn));
-  LCHK(d_anc.alloc(F * D.plim));
-  LCHK(d_nanc.alloc(F));
-  LCHK(d_p1.alloc(F * D.hcap));
-  LCHK(d_p2.alloc(F * D.hcap));
-  LCHK(d_s1.alloc(F * (D.clim + 2)));
-  LCHK(d_s2.alloc(F * (D.clim + 2)));
-  LCHK(d_cpx.alloc(2 * F * D.hcap));
-  LCHK(d_sid.alloc(F * (D.clim + 2)));
-  LCHK(d_st.alloc(F));
-  LCHK(d_nc.alloc(F));
-  LCHK(d_cc.alloc(F * per));
-  LCHK(d_fc.alloc(F));
-  LCHK(d_slots.alloc(4 * F * D.nslot));
-  LCHK(cudaMemcpy(d_img.p, images, (size_t)(F * D.N * channels), cudaMemcpyHostToDevice));
-  LCHK(cudaMemset(d_hist.p, 0, 256 * F * sizeof(int)));
-  grey_hist_kernel<<<dim3((unsigned)((D.N + 255) / 256), (unsigned)F), 256>>>(D, d_img.p, d_grey.p, d_hist.p);
-  lut_kernel<<<(unsigned)((F + 63) / 64), 64>>>(n_frames, D, d_hist.p, d_lut.p, d_bits.p);
-  const unsigned gb = (unsigned)((nn + 255) / 256);
-  prep_kernel<<<gb, 256>>>(n_frames, D, d_grey.p, d_lut.p, d_i8.p);
-  blur_row_kernel<<<gb, 256>>>(n_frames, D, d_i8.p, d_h16.p);
-  blur_col_kernel<<<gb, 256>>>(n_frames, D, d_h16.p, d_b8.p);
-  grad_kernel<<<gb, 256>>>(n_frames, D, d_b8.p, d_dx.p, d_dy.p, d_g.p, d_rec.p);
-  anchor_kernel<<<(unsigned)F, 1024>>>(D, d_g.p, d_rec.p, d_anc.p, d_nanc.p);
-  walk_kernel<<<(unsigned)F, 1>>>(n_frames, D, d_rec.p, d_anc.p, d_nanc.p, d_p1.p, d_p2.p, d_s1.p, d_s2.p, d_cpx.p,
-                                  d_sid.p, d_st.p, d_nc.p);
-  const unsigned gc = (unsigned)((F * per + 127) / 128);
-  chain_kernel<<<gc, 128>>>(n_frames, D, d_rec.p, d_dx.p, d_dy.p, d_cpx.p, d_sid.p, d_nc.p, d_slots.p, d_cc.p);
-  count_kernel<<<(unsigned)((F + 63) / 64), 64>>>(n_frames, D, d_nc.p, d_cc.p, d_fc.p);
-  LCHK(cudaGetLastError());
+  const Dims D = make_dims(width, height, channels, downsample);
+  const long long F = n_frames;
+  TempAlloc A;
+  Work W;
+  unsigned char* d_img = nullptr;
+  LCHK(A.get(d_img, F * D.N * channels));
+  LCHK(cudaMemcpy(d_img, images, (size_t)(F * D.N * channels), cudaMemcpyHostToDevice));
+  LCHK(detect(0, A, n_frames, D, d_img, W));
   std::vector<int> st(F), fc(F);
-  LCHK(cudaMemcpy(st.data(), d_st.p, F * sizeof(int), cudaMemcpyDeviceToHost));
-  LCHK(cudaMemcpy(fc.data(), d_fc.p, F * sizeof(int), cudaMemcpyDeviceToHost));
+  LCHK(cudaMemcpy(st.data(), W.st, F * sizeof(int), cudaMemcpyDeviceToHost));
+  LCHK(cudaMemcpy(fc.data(), W.fc, F * sizeof(int), cudaMemcpyDeviceToHost));
   std::vector<long long> ff(F);
   long long total = 0;
   for (int f = 0; f < n_frames; f++) {
@@ -360,11 +370,12 @@ extern "C" long long pus_popup_lines(int device, int n_frames, const unsigned ch
   if (!lines) return total;   // size query
   if (capacity < total) return refuse("capacity is smaller than the number of lines");
   if (total == 0) return 0;
-  LCHK(d_ff.alloc(F));
-  LCHK(d_out.alloc(4 * total));
-  LCHK(cudaMemcpy(d_ff.p, ff.data(), F * sizeof(long long), cudaMemcpyHostToDevice));
-  scatter_kernel<<<gc, 128>>>(n_frames, D, d_sid.p, d_nc.p, d_cc.p, d_ff.p, d_slots.p, d_out.p);
-  LCHK(cudaGetLastError());
-  LCHK(cudaMemcpy(lines, d_out.p, 4 * total * sizeof(float), cudaMemcpyDeviceToHost));
+  long long* d_ff = nullptr;
+  float* d_out = nullptr;
+  LCHK(A.get(d_ff, F));
+  LCHK(A.get(d_out, 4 * total));
+  LCHK(cudaMemcpy(d_ff, ff.data(), F * sizeof(long long), cudaMemcpyHostToDevice));
+  LCHK(scatter(0, n_frames, D, W, d_ff, d_out));
+  LCHK(cudaMemcpy(lines, d_out, 4 * total * sizeof(float), cudaMemcpyDeviceToHost));
   return total;
 }

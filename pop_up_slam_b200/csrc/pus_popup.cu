@@ -19,6 +19,8 @@
 
 #include "../../include/popup_gpu.h"
 #include "pus_edges.cuh"
+#include "pus_frames.cuh"
+#include "pus_stages.cuh"
 
 namespace pus {
 extern thread_local std::string g_err;
@@ -172,6 +174,14 @@ cudaError_t launch_refresh(cudaStream_t st, int n_frames, const int* d_frame_pos
   if (n_map > 0) store_meas_kernel<<<(n_map + 255) / 256, 256, 0, st>>>(n_map, d_map_row, d_map_slot, d_planes_sensor, d_pp_meas, d_out);
   return cudaGetLastError();
 }
+cudaError_t launch_fit(cudaStream_t st, int n_frames, const int* d_seg_ptr, const int* d_row_frame, int n_rows,
+                       const float* d_segs, const float* d_invK, const float* d_Ts, float dist_thre, int mode, float* d_pw,
+                       float* d_ps, float* d_dist, int* d_good, float* d_ends) {
+  if (n_rows > 0)
+    popup_kernel<<<(n_rows + 255) / 256, 256, 0, st>>>(n_frames, d_seg_ptr, d_row_frame, n_rows, d_segs, d_invK, d_Ts, dist_thre,
+                                                        mode, d_pw, d_ps, d_dist, d_good, d_ends);
+  return cudaGetLastError();
+}
 cudaError_t launch_project(cudaStream_t st, int n, const int* d_plane_idx, const double* d_plane4, const float* d_in, float* d_out) {
   project_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, d_plane_idx, d_plane4, d_in, d_out);
   return cudaGetLastError();
@@ -226,8 +236,7 @@ extern "C" int pus_popup_fit_frames(int device, int n_frames, const int* seg_ptr
   PCHK(cudaMemset(d_ps, 0, (size_t)n_rows * 4 * sizeof(float)));
   PCHK(cudaMemset(d_dist, 0, (size_t)n_rows * sizeof(float)));
   PCHK(cudaMemset(d_good, 0, (size_t)n_rows * sizeof(int)));
-  popup_kernel<<<(n_rows + 255) / 256, 256>>>(n_frames, d_ptr, d_rf, n_rows, d_segs, d_K, d_T, dist_thre, mode, d_pw, d_ps, d_dist, d_good);
-  PCHK(cudaGetLastError());
+  PCHK(launch_fit(0, n_frames, d_ptr, d_rf, n_rows, d_segs, d_K, d_T, dist_thre, mode, d_pw, d_ps, d_dist, d_good, nullptr));
   PCHK(cudaDeviceSynchronize());
   if (planes_world) PCHK(cudaMemcpy(planes_world, d_pw, (size_t)n_rows * 4 * sizeof(float), cudaMemcpyDeviceToHost));
   if (planes_sensor) PCHK(cudaMemcpy(planes_sensor, d_ps, (size_t)n_rows * 4 * sizeof(float), cudaMemcpyDeviceToHost));
@@ -250,8 +259,6 @@ namespace cloud {
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 
-struct Job { int frame, v0, n, bx, by, bw, bh, row0; };   // per plane: polygon in vtx[v0 .. v0+n), box, first span row
-struct Edge { int x1, y1, major, minor, sy, vert, valid; };
 
 // cv::LineIterator's clip against [0, w) x [0, h): Cohen-Sutherland with truncating divisions in double
 __device__ bool clip_line(long long w, long long h, long long& x1, long long& y1, long long& x2, long long& y2) {
@@ -375,22 +382,6 @@ __device__ void scan_spans(const int2* v, int n, int w, int h, int2* span) {
     ex[1] += edx[1];
   } while (++y <= ymax);
 }
-
-struct Params {
-  const Job* jobs;
-  const int2* vtx;
-  const float* planes;   // [n_planes][4] sensor frame
-  const float* Ts;       // [n_frames][16]
-  const float* invK;
-  const unsigned char* images;   // uploaded only when colours are written
-  int width, height, scale, border;   // border: images were given and are 960 wide (matrixToCloud's x < 4 || y < 4 rule)
-  float depth_thre, ceiling;
-  int2* span;            // [rows]
-  int* row_count;        // [rows]
-  const long long* row_off;
-  float* xyz;
-  unsigned char* rgb;
-};
 
 // the warp's pixel range of box row y, and its edge runs in runs[] (lanes over edges)
 __device__ __forceinline__ int2 row_setup(const Edge* E, int n, int2 sp, int y, int2* runs, int lane) {
@@ -669,6 +660,39 @@ __global__ void depth_resize_kernel(int n_frames, const float* half, int width, 
   }
   out[i] = v;
 }
+
+cudaError_t launch_count(cudaStream_t st, int n_planes, long long rows, const Params& P, long long* d_row_off, int* d_counts,
+                         long long* d_offsets) {
+  if (n_planes > 0) cloud_kernel<false><<<n_planes, kThreads, 0, st>>>(P);
+  cloud_scan_kernel<<<1, 1024, 0, st>>>((int)rows, P.row_count, d_row_off, n_planes, P.jobs, d_counts, d_offsets);
+  return cudaGetLastError();
+}
+cudaError_t launch_write(cudaStream_t st, int n_planes, const Params& P) {
+  if (n_planes > 0) cloud_kernel<true><<<n_planes, kThreads, 0, st>>>(P);
+  return cudaGetLastError();
+}
+cudaError_t launch_labels(cudaStream_t st, int n_frames, const int* d_plane_ptr, const Params& P, unsigned char* d_labels) {
+  if (n_frames > 0)
+    cloud_label_kernel<<<n_frames, kThreads, 0, st>>>(d_plane_ptr, P.jobs, P.vtx, P.span, P.width, P.height, P.scale, d_labels);
+  return cudaGetLastError();
+}
+cudaError_t launch_depth(cudaStream_t st, int n_frames, int n_planes, const int* d_plane_ptr, const Job* d_jobs,
+                         const int2* d_vtx, Edge* d_edges, int2* d_span, const float* d_planes, const float* d_Ts,
+                         const float* d_invK, int width, int height, int downsample, float ceiling, float* d_fill,
+                         float* d_out) {
+  if (n_frames == 0) return cudaSuccess;
+  const int scale = downsample ? 2 : 1, fw = width / scale, fh = height / scale;
+  if (n_planes > 0) depth_span_kernel<<<n_planes, 128, 0, st>>>(d_jobs, d_vtx, d_edges, d_span);
+  const long long fill_rows = (long long)n_frames * fh;
+  depth_kernel<<<(unsigned)((fill_rows + kWarps - 1) / kWarps), kThreads, 0, st>>>(n_frames, d_plane_ptr, d_jobs, d_edges, d_span,
+                                                                                   d_planes, d_Ts, d_invK, fw, fh, scale,
+                                                                                   ceiling, d_fill);
+  if (downsample) {
+    const size_t out_n = (size_t)n_frames * width * height;
+    depth_resize_kernel<<<(unsigned)((out_n + 255) / 256), 256, 0, st>>>(n_frames, d_fill, width, height, d_out);
+  }
+  return cudaGetLastError();
+}
 }  // namespace cloud
 }  // namespace pus
 
@@ -711,16 +735,7 @@ long long plane_jobs(const char* who, int n_frames, const int* plane_ptr, const 
       Job& J = jobs[p];
       J = Job{f, poly_ptr[p], poly_ptr[p + 1] - poly_ptr[p], 0, 0, 0, 0, (int)rows};
       if (J.n == 0) continue;
-      const float* q = polys + 2 * (size_t)J.v0;
-      auto at = [&](int i) { return downsample ? q[i] / 2.f : q[i]; };
-      int xmin = INT_MAX, xmax = INT_MIN, ymin = INT_MAX, ymax = INT_MIN;
-      for (int i = 0; i < J.n; i++) {
-        const int x = (int)at(2 * i), y = (int)at(2 * i + 1);
-        xmin = std::min(xmin, x); xmax = std::max(xmax, x); ymin = std::min(ymin, y); ymax = std::max(ymax, y);
-      }
-      J.bx = xmin; J.by = ymin; J.bw = xmax - xmin + 1; J.bh = ymax - ymin + 1;
-      for (int i = 0; i < J.n; i++)
-        vtx[J.v0 + i] = make_int2((int)(at(2 * i) - (float)J.bx), (int)(at(2 * i + 1) - (float)J.by));
+      pus::glue::polygon_box(polys + 2 * (size_t)J.v0, J.n, downsample, J, vtx.data() + J.v0);
       rows += J.bh;
       if (rows > INT_MAX / 2) return refuse("the polygons' bounding boxes have too many rows in all");
     }
@@ -790,10 +805,7 @@ extern "C" long long pus_popup_clouds(int device, int n_frames, const int* plane
   }
   Params P{d_jobs.p, d_vtx.p, d_planes.p, d_T.p, d_K.p, d_img.p, width, height, downsample ? 2 : 1, images && width == 960, depth_thre,
            ceiling_threshold, d_span.p, d_rowcnt.p, d_rowoff.p, nullptr, nullptr};
-  if (n_planes > 0) cloud_kernel<false><<<n_planes, kThreads>>>(P);
-  CCHK(cudaGetLastError());
-  cloud_scan_kernel<<<1, 1024>>>((int)rows, d_rowcnt.p, d_rowoff.p, n_planes, d_jobs.p, d_cnt.p, d_off.p);
-  CCHK(cudaGetLastError());
+  CCHK(launch_count(0, n_planes, rows, P, d_rowoff.p, d_cnt.p, d_off.p));
   long long total = 0;
   CCHK(cudaMemcpy(&total, d_rowoff.p + rows, sizeof(long long), cudaMemcpyDeviceToHost));
   if (counts && n_planes > 0) CCHK(cudaMemcpy(counts, d_cnt.p, n_planes * sizeof(int), cudaMemcpyDeviceToHost));
@@ -804,8 +816,7 @@ extern "C" long long pus_popup_clouds(int device, int n_frames, const int* plane
     if (rgb) CCHK(d_rgb.alloc((size_t)total * 3));
     P.xyz = d_xyz.p;
     P.rgb = d_rgb.p;
-    cloud_kernel<true><<<n_planes, kThreads>>>(P);
-    CCHK(cudaGetLastError());
+    CCHK(launch_write(0, n_planes, P));
     if (xyz) CCHK(cudaMemcpy(xyz, d_xyz.p, (size_t)total * 3 * sizeof(float), cudaMemcpyDeviceToHost));
     if (rgb) CCHK(cudaMemcpy(rgb, d_rgb.p, (size_t)total * 3, cudaMemcpyDeviceToHost));
   }
@@ -814,8 +825,7 @@ extern "C" long long pus_popup_clouds(int device, int n_frames, const int* plane
     CCHK(d_ptr.alloc(n_frames + 1));
     CCHK(cudaMemcpy(d_ptr.p, plane_ptr, (n_frames + 1) * sizeof(int), cudaMemcpyHostToDevice));
     CCHK(cudaMemset(d_lab.p, 127, (size_t)n_frames * width * height));
-    cloud_label_kernel<<<n_frames, kThreads>>>(d_ptr.p, d_jobs.p, d_vtx.p, d_span.p, width, height, downsample ? 2 : 1, d_lab.p);
-    CCHK(cudaGetLastError());
+    CCHK(launch_labels(0, n_frames, d_ptr.p, P, d_lab.p));
     CCHK(cudaMemcpy(labels, d_lab.p, (size_t)n_frames * width * height, cudaMemcpyDeviceToHost));
   }
   CCHK(cudaDeviceSynchronize());
@@ -877,17 +887,8 @@ extern "C" int pus_popup_depth(int device, int n_frames, const int* plane_ptr, c
   DCHK(cudaMemcpy(d_T.p, Ts, (size_t)n_frames * 16 * sizeof(float), cudaMemcpyHostToDevice));
   DCHK(cudaMemcpy(d_K.p, invK, 9 * sizeof(float), cudaMemcpyHostToDevice));
   DCHK(cudaMemcpy(d_ptr.p, plane_ptr, (n_frames + 1) * sizeof(int), cudaMemcpyHostToDevice));
-  if (n_planes > 0) depth_span_kernel<<<n_planes, 128>>>(d_jobs.p, d_vtx.p, d_edges.p, d_span.p);
-  DCHK(cudaGetLastError());
-  const long long fill_rows = (long long)n_frames * fh;
-  depth_kernel<<<(unsigned)((fill_rows + kWarps - 1) / kWarps), kThreads>>>(n_frames, d_ptr.p, d_jobs.p, d_edges.p, d_span.p,
-                                                                             d_planes.p, d_T.p, d_K.p, fw, fh, scale,
-                                                                             ceiling_threshold, d_fill.p);
-  DCHK(cudaGetLastError());
-  if (downsample) {
-    depth_resize_kernel<<<(unsigned)((out_n + 255) / 256), 256>>>(n_frames, d_fill.p, width, height, d_out.p);
-    DCHK(cudaGetLastError());
-  }
+  DCHK(launch_depth(0, n_frames, n_planes, d_ptr.p, d_jobs.p, d_vtx.p, d_edges.p, d_span.p, d_planes.p, d_T.p, d_K.p, width,
+                    height, downsample, ceiling_threshold, d_fill.p, d_out.p));
   DCHK(cudaMemcpy(depth, downsample ? d_out.p : d_fill.p, out_n * sizeof(float), cudaMemcpyDeviceToHost));
   return 0;
 }
@@ -899,11 +900,6 @@ extern "C" int pus_popup_depth(int device, int n_frames, const int* plane_ptr, c
 // pass packs the slots in row order at offsets scanned from the counts.
 namespace pus {
 namespace poly {
-constexpr int kBoundSlot = PUS_POPUP_MAX_VERTICES;   // the ground polygon has n + 6 vertices at most, a wall's 7
-constexpr int kWallMax = 7;
-constexpr int kHullMax = 34;                          // 6 x 4 edge crossings + 10 corners
-constexpr int kCutSlot = kHullMax + 1;
-
 struct P3 { float x, y, z; };
 
 // P2, trunc_i and hit_boundary (direction_hit_boundary) are in pus_edges.cuh, shared with pus_popup_edges
@@ -1166,24 +1162,6 @@ __device__ int cut_wall(const P3* P, int m, float ceiling, float walllength, P3 
   return ns;
 }
 
-struct Params {
-  const int* seg_ptr;
-  const int* row_frame;
-  int n_rows;
-  const float* segs;
-  const float* K;
-  const float* invK;
-  const float* Ts;
-  const float* planes;   // [n_rows][4] sensor frame, from popup_kernel
-  const float* ends;     // [n_rows][6] world ground endpoints of the wall rows, from popup_kernel
-  int width, height;
-  float ceiling, walllength;
-  float* bound;          // [n_rows][kBoundSlot][2]
-  float* cut;            // [n_rows][kCutSlot][2]
-  float* world;          // [n_rows][kCutSlot][3]
-  int* counts;           // [3][n_rows]: bound, cut, world
-};
-
 // the up image direction of a world vertical at ground endpoint k of the frame's segment s (popup_plane.cpp:127-143)
 __device__ P2 up_direction(const Params& P, const float* K, const float* iT, int row_of_seg, int k) {
   const float* e = P.ends + (size_t)row_of_seg * 6 + 3 * k;
@@ -1342,6 +1320,17 @@ __global__ void pack_kernel(int n_rows, const int* row_frame, const int* seg_ptr
   if (ow)
     for (int i = 0; i < 3 * counts[2 * n_rows + row]; i++) ow[3 * off[2 * n_rows + row] + i] = world[(size_t)row * kCutSlot * 3 + i];
 }
+
+cudaError_t launch_rows(cudaStream_t st, const Params& P) {
+  if (P.n_rows > 0) polygon_kernel<<<(P.n_rows + 127) / 128, 128, 0, st>>>(P);
+  return cudaGetLastError();
+}
+cudaError_t launch_pack(cudaStream_t st, const Params& P, const long long* d_off, float* ob, float* oc, float* ow) {
+  if (P.n_rows > 0)
+    pack_kernel<<<(P.n_rows + 255) / 256, 256, 0, st>>>(P.n_rows, P.row_frame, P.seg_ptr, P.counts, d_off, P.bound, P.cut,
+                                                        P.world, ob, oc, ow);
+  return cudaGetLastError();
+}
 }  // namespace poly
 }  // namespace pus
 
@@ -1413,13 +1402,11 @@ extern "C" int pus_popup_polygons(int device, int n_frames, const int* seg_ptr, 
   GCHK(cudaMemcpy(d_iK.p, invK, 9 * sizeof(float), cudaMemcpyHostToDevice));
   GCHK(cudaMemcpy(d_T.p, Ts, (size_t)n_frames * 16 * sizeof(float), cudaMemcpyHostToDevice));
   // the planes and the world ground endpoints: get_plane_equation, as pus_popup_fit_frames runs it (mode 0)
-  popup_kernel<<<(n_rows + 255) / 256, 256>>>(n_frames, d_ptr.p, d_rf.p, n_rows, d_segs.p, d_iK.p, d_T.p, 0.f, 0, nullptr,
-                                               d_pl.p, nullptr, nullptr, d_ends.p);
-  GCHK(cudaGetLastError());
+  GCHK(launch_fit(0, n_frames, d_ptr.p, d_rf.p, n_rows, d_segs.p, d_iK.p, d_T.p, 0.f, 0, nullptr, d_pl.p, nullptr, nullptr,
+                  d_ends.p));
   Params P{d_ptr.p, d_rf.p, n_rows, d_segs.p, d_K.p, d_iK.p, d_T.p, d_pl.p, d_ends.p, width, height, ceiling_threshold,
            walllength_threshold, d_b.p, d_c.p, d_w.p, d_cnt.p};
-  polygon_kernel<<<(n_rows + 127) / 128, 128>>>(P);
-  GCHK(cudaGetLastError());
+  GCHK(launch_rows(0, P));
   std::vector<int> cnt((size_t)n_rows * 3);
   GCHK(cudaMemcpy(cnt.data(), d_cnt.p, cnt.size() * sizeof(int), cudaMemcpyDeviceToHost));
   std::memcpy(bound_counts, cnt.data(), n_rows * sizeof(int));
@@ -1440,8 +1427,7 @@ extern "C" int pus_popup_polygons(int device, int n_frames, const int* seg_ptr, 
   if (bound2d) GCHK(d_ob.alloc((size_t)tot[0] * 2));
   if (cut2d) GCHK(d_oc.alloc((size_t)tot[1] * 2));
   if (world3d) GCHK(d_ow.alloc((size_t)tot[2] * 3));
-  pack_kernel<<<(n_rows + 255) / 256, 256>>>(n_rows, d_rf.p, d_ptr.p, d_cnt.p, d_off.p, d_b.p, d_c.p, d_w.p, d_ob.p, d_oc.p, d_ow.p);
-  GCHK(cudaGetLastError());
+  GCHK(launch_pack(0, P, d_off.p, d_ob.p, d_oc.p, d_ow.p));
   if (bound2d && tot[0] > 0) GCHK(cudaMemcpy(bound2d, d_ob.p, (size_t)tot[0] * 2 * sizeof(float), cudaMemcpyDeviceToHost));
   if (cut2d && tot[1] > 0) GCHK(cudaMemcpy(cut2d, d_oc.p, (size_t)tot[1] * 2 * sizeof(float), cudaMemcpyDeviceToHost));
   if (world3d && tot[2] > 0) GCHK(cudaMemcpy(world3d, d_ow.p, (size_t)tot[2] * 3 * sizeof(float), cudaMemcpyDeviceToHost));
@@ -1458,11 +1444,6 @@ extern "C" int pus_popup_polygons(int device, int n_frames, const int* seg_ptr, 
 // contour assembly in cell order and the restart loops of the selection -- with the shared code of pus_edges.cuh.
 namespace pus {
 namespace edges {
-struct Frame {   // one frame's scratch and output slots
-  long long node, obj, cpt, line, ivl, tab;
-  int node_cap, obj_cap, cpt_cap, ivl_cap, l0, n;
-};
-
 // one box pass over all frames; pass 0 reads the label maps (with the 0.5x pick), the last one writes 255 - v
 __global__ void edge_box_kernel(int n_frames, const unsigned char* src, int sw, int sh, int ds, int w, int h, int k, int horiz,
                                 int dilate, int invert, unsigned char* dst) {
@@ -1503,6 +1484,53 @@ __global__ void edge_frame_kernel(int n_frames, pus_edge_params P, int width, in
   out[4 * f + 2] = st ? 0 : n_conn;
   out[4 * f + 3] = (int)bits;
 }
+
+cudaError_t prep(cudaStream_t st, Alloc& A, int n_frames, const unsigned char* d_labels, int width, int height,
+                 const pus_edge_params& P, Maps& M) {
+  const int ds = P.downsample_contour ? 1 : 0;
+  M.w = ds ? half_size(width) : width;
+  M.h = ds ? half_size(height) : height;
+  const int w = M.w, h = M.h, kd = ds ? 8 : P.dilation_distance, ke = ds ? 8 : P.erosion_distance;
+  const size_t map_n = (size_t)n_frames * w * h;
+  unsigned char* d_a = nullptr;
+  cudaError_t e;
+  if ((e = A.get(d_a, map_n)) != cudaSuccess || (e = A.get(M.map, map_n)) != cudaSuccess ||
+      (e = A.get(M.seg_count, n_frames)) != cudaSuccess)
+    return e;
+  if (n_frames == 0) return cudaSuccess;
+  if ((e = cudaMemsetAsync(M.seg_count, 0, n_frames * sizeof(int), st)) != cudaSuccess) return e;
+  const unsigned gb = (unsigned)((map_n + 255) / 256);
+  edge_box_kernel<<<gb, 256, 0, st>>>(n_frames, d_labels, width, height, ds, w, h, kd, 1, 1, 0, d_a);
+  edge_box_kernel<<<gb, 256, 0, st>>>(n_frames, d_a, w, h, 0, w, h, kd, 0, 1, 0, M.map);
+  edge_box_kernel<<<gb, 256, 0, st>>>(n_frames, M.map, w, h, 0, w, h, ke, 1, 0, 0, d_a);
+  edge_box_kernel<<<gb, 256, 0, st>>>(n_frames, d_a, w, h, 0, w, h, ke, 0, 0, 1, M.map);
+  const long long n_cells = (long long)n_frames * (w - 1) * (h - 1);
+  edge_count_kernel<<<(unsigned)((n_cells + 255) / 256), 256, 0, st>>>(n_frames, M.map, w, h, M.seg_count);
+  return cudaGetLastError();
+}
+
+cudaError_t select(cudaStream_t st, Alloc& A, int n_frames, const pus_edge_params& P, int width, int height, const Maps& M,
+                   const Frame* d_fr, const long long tot[4], long long n_lines, const float* d_lines, float* d_open,
+                   float* d_conn, int* d_inc, int* d_out) {
+  const size_t map_n = (size_t)n_frames * M.w * M.h;
+  int *d_tab = nullptr, *d_nodes = nullptr, *d_objs = nullptr;
+  unsigned char* d_flags = nullptr;
+  float *d_cpts = nullptr, *d_bounds = nullptr;
+  Lin* d_rows = nullptr;
+  Ivl* d_ivl = nullptr;
+  cudaError_t e;
+  // per frame of n lines: 2 n work and open rows, 4 n connected rows (Sel in pus_edges.cuh)
+  if ((e = A.get(d_tab, 2 * map_n)) != cudaSuccess || (e = A.get(d_nodes, 2 * tot[0])) != cudaSuccess ||
+      (e = A.get(d_objs, 3 * tot[1])) != cudaSuccess || (e = A.get(d_flags, 2 * tot[1])) != cudaSuccess ||
+      (e = A.get(d_cpts, 2 * tot[2])) != cudaSuccess || (e = A.get(d_rows, 2 * n_lines)) != cudaSuccess ||
+      (e = A.get(d_bounds, 2 * n_lines)) != cudaSuccess || (e = A.get(d_ivl, 2 * tot[3])) != cudaSuccess)
+    return e;
+  if (n_frames == 0) return cudaSuccess;
+  if ((e = cudaMemsetAsync(d_tab, 0xff, 2 * map_n * sizeof(int), st)) != cudaSuccess) return e;
+  edge_frame_kernel<<<n_frames, 1, 0, st>>>(n_frames, P, width, height, M.map, M.w, M.h, d_fr, d_tab, d_nodes, d_objs, d_flags,
+                                            d_cpts, d_lines, d_rows, d_bounds, d_ivl, d_open, d_conn, d_inc, d_out);
+  return cudaGetLastError();
+}
 }  // namespace edges
 }  // namespace pus
 
@@ -1530,72 +1558,35 @@ extern "C" int pus_popup_edges(int device, int n_frames, const unsigned char* la
   if (n_frames == 0) return 0;
   ECHK(cudaSetDevice(device));
   const pus_edge_params P = *params;
-  const int ds = P.downsample_contour ? 1 : 0;
-  const int w = ds ? half_size(width) : width, h = ds ? half_size(height) : height;
-  const int kd = ds ? 8 : P.dilation_distance, ke = ds ? 8 : P.erosion_distance;
-  const long long cells = (long long)w * h, n_lines = line_ptr[n_frames];
-  DevBuf<unsigned char> d_lab, d_a, d_b, d_flags;
-  DevBuf<int> d_cnt, d_tab, d_nodes, d_objs, d_out, d_inc;
-  DevBuf<Frame> d_fr;
-  DevBuf<float> d_cpts, d_lines, d_bounds, d_open, d_conn;
-  DevBuf<Lin> d_rows;
-  DevBuf<Ivl> d_ivl;
-  const size_t lab_n = (size_t)n_frames * width * height, map_n = (size_t)n_frames * cells;
-  ECHK(d_lab.alloc(lab_n));
-  ECHK(d_a.alloc(map_n));
-  ECHK(d_b.alloc(map_n));
-  ECHK(d_cnt.alloc(n_frames));
-  ECHK(cudaMemcpy(d_lab.p, labels, lab_n, cudaMemcpyHostToDevice));
-  ECHK(cudaMemset(d_cnt.p, 0, n_frames * sizeof(int)));
-  const unsigned gb = (unsigned)((map_n + 255) / 256);
-  edge_box_kernel<<<gb, 256>>>(n_frames, d_lab.p, width, height, ds, w, h, kd, 1, 1, 0, d_a.p);
-  edge_box_kernel<<<gb, 256>>>(n_frames, d_a.p, w, h, 0, w, h, kd, 0, 1, 0, d_b.p);
-  edge_box_kernel<<<gb, 256>>>(n_frames, d_b.p, w, h, 0, w, h, ke, 1, 0, 0, d_a.p);
-  edge_box_kernel<<<gb, 256>>>(n_frames, d_a.p, w, h, 0, w, h, ke, 0, 0, 1, d_b.p);
-  ECHK(cudaGetLastError());
-  const long long n_cells = (long long)n_frames * (w - 1) * (h - 1);
-  edge_count_kernel<<<(unsigned)((n_cells + 255) / 256), 256>>>(n_frames, d_b.p, w, h, d_cnt.p);
-  ECHK(cudaGetLastError());
+  const long long n_lines = line_ptr[n_frames];
+  const size_t lab_n = (size_t)n_frames * width * height;
+  TempAlloc A;
+  unsigned char* d_lab = nullptr;
+  ECHK(A.get(d_lab, lab_n));
+  ECHK(cudaMemcpy(d_lab, labels, lab_n, cudaMemcpyHostToDevice));
+  Maps M;
+  ECHK(prep(0, A, n_frames, d_lab, width, height, P, M));
   std::vector<int> cnt(n_frames);
-  ECHK(cudaMemcpy(cnt.data(), d_cnt.p, n_frames * sizeof(int), cudaMemcpyDeviceToHost));
+  ECHK(cudaMemcpy(cnt.data(), M.seg_count, n_frames * sizeof(int), cudaMemcpyDeviceToHost));
   // scratch layout
   std::vector<Frame> fr(n_frames);
-  long long node = 0, obj = 0, cpt = 0, ivl = 0;
-  for (int f = 0; f < n_frames; f++) {
-    Frame& F = fr[f];
-    F.node_cap = (int)node_cap_of(cnt[f]);
-    F.obj_cap = (int)obj_cap_of(cnt[f]);
-    F.cpt_cap = (int)cpt_cap_of(cnt[f]);
-    F.n = line_ptr[f + 1] - line_ptr[f];
-    F.ivl_cap = (int)ivl_cap_of(F.n);
-    F.l0 = line_ptr[f];
-    F.node = node; F.obj = obj; F.cpt = cpt; F.ivl = ivl; F.line = F.l0; F.tab = 2 * cells * f;
-    node += F.node_cap; obj += F.obj_cap; cpt += F.cpt_cap; ivl += F.ivl_cap;
-  }
-  ECHK(d_fr.alloc(n_frames));
-  ECHK(d_tab.alloc(2 * map_n));
-  ECHK(d_nodes.alloc(2 * node));
-  ECHK(d_objs.alloc(3 * obj));
-  ECHK(d_flags.alloc(2 * obj));
-  ECHK(d_cpts.alloc(2 * cpt));
-  ECHK(d_lines.alloc(4 * n_lines));
-  // per frame of n lines: 2 n work and open rows, 4 n connected rows (Sel in pus_edges.cuh)
-  ECHK(d_rows.alloc(2 * n_lines));
-  ECHK(d_bounds.alloc(2 * n_lines));
-  ECHK(d_ivl.alloc(2 * ivl));
-  ECHK(d_open.alloc(8 * n_lines));
-  ECHK(d_conn.alloc(16 * n_lines));
-  ECHK(d_inc.alloc(2 * n_lines));
-  ECHK(d_out.alloc(4 * (size_t)n_frames));
-  ECHK(cudaMemcpy(d_fr.p, fr.data(), n_frames * sizeof(Frame), cudaMemcpyHostToDevice));
-  if (n_lines > 0) ECHK(cudaMemcpy(d_lines.p, lines, 4 * n_lines * sizeof(float), cudaMemcpyHostToDevice));
-  ECHK(cudaMemset(d_tab.p, 0xff, 2 * map_n * sizeof(int)));
-  edge_frame_kernel<<<n_frames, 1>>>(n_frames, P, width, height, d_b.p, w, h, d_fr.p, d_tab.p, d_nodes.p,
-                                                   d_objs.p, d_flags.p, d_cpts.p, d_lines.p, d_rows.p, d_bounds.p, d_ivl.p,
-                                                   d_open.p, d_conn.p, d_inc.p, d_out.p);
-  ECHK(cudaGetLastError());
+  long long tot[4] = {0, 0, 0, 0};
+  for (int f = 0; f < n_frames; f++)
+    pus::glue::edge_frame(f, cnt[f], line_ptr[f], line_ptr[f + 1] - line_ptr[f], (long long)M.w * M.h, tot, fr[f]);
+  Frame* d_fr = nullptr;
+  float *d_lines = nullptr, *d_open = nullptr, *d_conn = nullptr;
+  int *d_inc = nullptr, *d_out = nullptr;
+  ECHK(A.get(d_fr, n_frames));
+  ECHK(A.get(d_lines, 4 * n_lines));
+  ECHK(A.get(d_open, 8 * n_lines));
+  ECHK(A.get(d_conn, 16 * n_lines));
+  ECHK(A.get(d_inc, 2 * n_lines));
+  ECHK(A.get(d_out, 4 * (size_t)n_frames));
+  ECHK(cudaMemcpy(d_fr, fr.data(), n_frames * sizeof(Frame), cudaMemcpyHostToDevice));
+  if (n_lines > 0) ECHK(cudaMemcpy(d_lines, lines, 4 * n_lines * sizeof(float), cudaMemcpyHostToDevice));
+  ECHK(select(0, A, n_frames, P, width, height, M, d_fr, tot, n_lines, d_lines, d_open, d_conn, d_inc, d_out));
   std::vector<int> out(4 * (size_t)n_frames);
-  ECHK(cudaMemcpy(out.data(), d_out.p, out.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  ECHK(cudaMemcpy(out.data(), d_out, out.size() * sizeof(int), cudaMemcpyDeviceToHost));
   long long tot_open = 0, tot_conn = 0;
   int found = 0;
   for (int f = 0; f < n_frames; f++) {
@@ -1612,9 +1603,9 @@ extern "C" int pus_popup_edges(int device, int n_frames, const unsigned char* la
   std::vector<float> os(8 * (size_t)n_lines), cs(16 * (size_t)n_lines);
   std::vector<int> inc(2 * (size_t)n_lines);
   if (n_lines > 0) {
-    ECHK(cudaMemcpy(os.data(), d_open.p, os.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    ECHK(cudaMemcpy(cs.data(), d_conn.p, cs.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    ECHK(cudaMemcpy(inc.data(), d_inc.p, inc.size() * sizeof(int), cudaMemcpyDeviceToHost));
+    ECHK(cudaMemcpy(os.data(), d_open, os.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    ECHK(cudaMemcpy(cs.data(), d_conn, cs.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    ECHK(cudaMemcpy(inc.data(), d_inc, inc.size() * sizeof(int), cudaMemcpyDeviceToHost));
   }
   long long po = 0, pc = 0;
   for (int f = 0; f < n_frames; f++) {
