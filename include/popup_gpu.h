@@ -268,6 +268,7 @@ int pus_get_trace(pus_handle h, int capacity, double* lambda, double* chi2_new, 
  *   invK[9] row-major, Ts[n_frames*16] row-major camera-to-world
  *   outputs have one row per (frame, plane) with plane 0 = ground, i.e. n_seg(f)+1 rows
  *   per frame at row offset seg_ptr[f]+f:  planes_world/sensor 4 floats, dist 1, good 1 (0/1).
+ * A seg_ptr that is NULL, does not start at 0 or decreases is refused before any device work.
  * Any output may be NULL. */
 int pus_popup_fit_frames(int device, int n_frames, const int* seg_ptr, const float* segs, const float* invK,
                          const float* Ts, float dist_thre, int mode, float* planes_world, float* planes_sensor,
@@ -577,7 +578,7 @@ int pus_popup_session_memory(pus_popup_session s, long long* allocations, long l
  * graph is not resident), the fit and the factor store run on the device, and only the new measurements come
  * back to refresh the host mirrors (pus_get_measurement):
  *   frame_pose[n_frames]   pose node id of every frame
- *   seg_ptr[n_frames+1], segs, invK   as pus_popup_fit_frames
+ *   seg_ptr[n_frames+1], segs, invK   as pus_popup_fit_frames (a malformed seg_ptr is refused before any device work)
  *   map_fid / map_frame / map_row [n_map]   factor id, frame index, plane row inside the frame
  *                                           (0 = ground, 1 + i = segment i: good_plane_indices)
  *   new_meas[n_map*4]      optional copy of the stored measurements */
@@ -590,7 +591,8 @@ int pus_refresh_plane_measurements(pus_handle h, int n_frames, const int* frame_
  * into the device factor store.  new_meas = NULL: nothing returns to the host -- the host mirrors (pus_get_measurement,
  * FactorT::measurement()) are refreshed lazily on their next read or at the next layout rebuild; new_meas != NULL: [n_map][4]
  * out, mirrors refreshed at once.  A structural edit between bind and run is fine as long as the bound frames / factors still
- * exist (the layout-dependent tables are rebuilt by the run). */
+ * exist (the layout-dependent tables are rebuilt by the run).  pus_refresh_bind refuses a malformed seg_ptr as
+ * pus_refresh_plane_measurements does. */
 int pus_refresh_bind(pus_handle h, int n_frames, const int* frame_pose, const int* seg_ptr, const float* segs, const float* invK,
                      int n_map, const int* map_fid, const int* map_frame, const int* map_row);
 int pus_refresh_run(pus_handle h, double* new_meas);

@@ -735,6 +735,14 @@ PUS_EHD inline long long obj_cap_of(long long ns) { return ns + 1; }
 PUS_EHD inline long long cpt_cap_of(long long ns) { return node_cap_of(ns) / 20 + 2; }
 PUS_EHD inline long long ivl_cap_of(long long n) { return 2 * n * n + 2; }
 
+// the frame size and pus_edge_params rules of pus_popup_edges, shared with the pop-up session's config check; "" when they pass
+inline std::string shape_error(int width, int height, const pus_edge_params* params) {
+  if (width < 4 || height < 4) return "width and height must be at least 4";
+  if (!params) return "params must be given";
+  if (!params->downsample_contour && (params->dilation_distance < 1 || params->erosion_distance < 1))
+    return "dilation_distance and erosion_distance must be at least 1";
+  return "";
+}
 // the checks of pus_popup_edges' arguments, shared with the test oracle's restatement of the call; "" when they pass
 inline std::string args_error(int n_frames, const unsigned char* labels, int width, int height, const int* line_ptr,
                             const float* lines, const pus_edge_params* params, const int* status, const int* open_counts,
@@ -746,10 +754,8 @@ inline std::string args_error(int n_frames, const unsigned char* labels, int wid
     if (n < 0) return "line_ptr is not ascending";
     if (n > PUS_POPUP_MAX_LINES) return "a frame has more than PUS_POPUP_MAX_LINES lines";
   }
-  if (width < 4 || height < 4) return "width and height must be at least 4";
-  if (!params) return "params must be given";
-  if (!params->downsample_contour && (params->dilation_distance < 1 || params->erosion_distance < 1))
-    return "dilation_distance and erosion_distance must be at least 1";
+  const std::string why = shape_error(width, height, params);
+  if (!why.empty()) return why;
   if (n_frames > 0 && !labels) return "labels must be given";
   const int n = line_ptr[n_frames];
   if (n > 0 && !lines) return "lines must be given";

@@ -14,6 +14,7 @@
 #include "../../include/popup_gpu.h"
 #include "pus_export.cuh"
 #include "pus_graph.hpp"
+#include "pus_stages.cuh"
 
 namespace pus {
 // the device code is instantiated twice: kplain (here) = the single-GPU kernel, spanning hooks compiled out; kspan
@@ -1131,6 +1132,8 @@ int pus_refresh_plane_measurements(pus_handle h, int n_frames, const int* frame_
   NEED(h);
   Solver* s = SV(h);
   if (n_frames <= 0) return 0;
+  std::vector<int> row_frame;
+  if (const char* why = row_frames(n_frames, seg_ptr, row_frame)) { g_err = why; return -1; }
   // (re-upload when the topology OR the host values changed: update_plane_measurement uses pose_vertex->value())
   if (!s->uploaded || s->compiled_topo != s->g.topo_version || s->values_dirty) {
     if (upload(s) < 0) return -1;
@@ -1139,12 +1142,10 @@ int pus_refresh_plane_measurements(pus_handle h, int n_frames, const int* frame_
   }
   const Compiled& c = s->c;
   const int n_seg = seg_ptr[n_frames], n_rows = n_seg + n_frames;
-  std::vector<int> fpose(n_frames), row_frame(n_rows), mrow(n_map), mslot(n_map);
+  std::vector<int> fpose(n_frames), mrow(n_map), mslot(n_map);
   for (int f = 0; f < n_frames; f++) {
     if (!s->g.ok_node(frame_pose[f], NODE_POSE)) { g_err = "frame " + std::to_string(f) + ": not a pose node"; return -1; }
-    if (seg_ptr[f + 1] < seg_ptr[f]) { g_err = "seg_ptr must be non-decreasing"; return -1; }
     fpose[f] = c.node_idx[frame_pose[f]];
-    for (int r = seg_ptr[f] + f; r < seg_ptr[f + 1] + f + 1; r++) row_frame[r] = f;
   }
   if ((int)s->fid2slot.size() != (int)s->g.factors.size() || s->fid2slot_topo != s->compiled_topo) {
     s->fid2slot.assign(s->g.factors.size(), -1);
@@ -1231,17 +1232,15 @@ int pus_refresh_bind(pus_handle h, int n_frames, const int* frame_pose, const in
   Solver::RefreshTables& t = s->rt;
   t.bound = false;
   if (n_frames <= 0 || n_map < 0) { g_err = "pus_refresh_bind: nothing to bind"; return -1; }
+  std::vector<int> row_frame;
+  if (const char* why = row_frames(n_frames, seg_ptr, row_frame)) { g_err = why; return -1; }
   if (ensure_device(s) < 0) return -1;
   const int n_seg = seg_ptr[n_frames], n_rows = n_seg + n_frames;
-  std::vector<int> row_frame(n_rows);
   t.frame_node.assign(frame_pose, frame_pose + n_frames);
   t.map_fid.assign(map_fid, map_fid + n_map);
   t.mrow.resize(n_map);
-  for (int f = 0; f < n_frames; f++) {
+  for (int f = 0; f < n_frames; f++)
     if (!s->g.ok_node(frame_pose[f], NODE_POSE)) { g_err = "frame " + std::to_string(f) + ": not a pose node"; return -1; }
-    if (seg_ptr[f + 1] < seg_ptr[f]) { g_err = "seg_ptr must be non-decreasing"; return -1; }
-    for (int r = seg_ptr[f] + f; r < seg_ptr[f + 1] + f + 1; r++) row_frame[r] = f;
-  }
   for (int m = 0; m < n_map; m++) {
     const int f = map_frame[m];
     if (f < 0 || f >= n_frames) { g_err = "map_frame out of range"; return -1; }

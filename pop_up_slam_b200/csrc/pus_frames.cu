@@ -17,8 +17,6 @@
 #include "pus_stages.cuh"
 
 namespace pus {
-extern thread_local std::string g_err;
-
 namespace frames {
 constexpr int kScan = 1024;
 
@@ -277,15 +275,12 @@ bool finite9(const float* a) {
   return true;
 }
 
-// "" when the config is one the stage calls accept as main_3d runs them
+// "" when the config is one the stage calls accept as main_3d runs them: the edges' and the lines' own rules (the edges'
+// frame size first), then the session's
 std::string config_error(const pus_popup_config& c) {
-  if (c.channels != 1 && c.channels != 3) return "channels must be 1 (grey) or 3 (BGR)";
-  if (c.width < 4 || c.height < 4) return "width and height must be at least 4";
-  if ((long long)c.width * c.height > PUS_POPUP_LINES_MAX_PIXELS) return "a frame has more than 2^28 pixels";
-  if (c.fast_edges && ((c.width | c.height) & 1)) return "fast_edges needs an even width and height";
-  if (c.fast_edges && (c.width / 2 < 3 || c.height / 2 < 3)) return "the detection image must be at least 3 x 3";
-  if (!c.edges.downsample_contour && (c.edges.dilation_distance < 1 || c.edges.erosion_distance < 1))
-    return "edges.dilation_distance and edges.erosion_distance must be at least 1";
+  const std::string why = edges::shape_error(c.width, c.height, &c.edges);
+  if (!why.empty()) return why;
+  if (const char* w = lines::shape_error(c.width, c.height, c.channels, c.fast_edges)) return w;
   if (!finite9(c.K) || !finite9(c.invK)) return "K and invK must be finite";
   if (c.downsample_poly && (c.want_labels || c.want_depth) && ((c.width | c.height) & 1))
     return "label images and depth maps in downsample_poly mode need an even width and height";
@@ -293,33 +288,17 @@ std::string config_error(const pus_popup_config& c) {
   return "";
 }
 
-int refuse(const std::string& why) {
-  pus::g_err = "pus_popup_session: " + why;
-  return -1;
-}
+const Call kSession{"pus_popup_session"};
 }  // namespace
 }  // namespace pus
 
 using namespace pus;
 
-#define SCHK(call)                                                                                            \
-  do {                                                                                                        \
-    const cudaError_t e__ = (call);                                                                           \
-    if (e__ != cudaSuccess) {                                                                                 \
-      g_err = std::string("pus_popup_session_run: ") + #call + ": " + cudaGetErrorString(e__);                 \
-      S.res = pus_popup_frames{};                                                                             \
-      return -1;                                                                                              \
-    }                                                                                                         \
-  } while (0)
-
 extern "C" int pus_popup_session_create(int device, const pus_popup_config* cfg, pus_popup_session* out) {
-  if (!cfg || !out) return refuse("config and out must be given");
+  if (!cfg || !out) return kSession.refuse("config and out must be given");
   const std::string why = config_error(*cfg);
-  if (!why.empty()) return refuse(why);
-  int ndev = 0;
-  const cudaError_t de = cudaGetDeviceCount(&ndev);
-  if (de != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
-    return refuse("no CUDA device usable; libpopup_gpu has no CPU fallback");
+  if (!why.empty()) return kSession.refuse(why);
+  if (kSession.check_device(device) < 0) return -1;
   Session* S = new Session;
   S->device = device;
   S->cfg = *cfg;
@@ -327,7 +306,7 @@ extern "C" int pus_popup_session_create(int device, const pus_popup_config* cfg,
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&S->own, cudaStreamNonBlocking);
   if (e != cudaSuccess) {
     delete S;
-    return refuse(std::string("stream: ") + cudaGetErrorString(e));
+    return kSession.refuse(std::string("stream: ") + cudaGetErrorString(e));
   }
   S->st = S->own;
   *out = S;
@@ -335,7 +314,7 @@ extern "C" int pus_popup_session_create(int device, const pus_popup_config* cfg,
 }
 
 extern "C" int pus_popup_session_destroy(pus_popup_session s) {
-  if (!s) return refuse("session is NULL");
+  if (!s) return kSession.refuse("session is NULL");
   Session* S = (Session*)s;
   cudaSetDevice(S->device);
   delete S;
@@ -343,14 +322,14 @@ extern "C" int pus_popup_session_destroy(pus_popup_session s) {
 }
 
 extern "C" int pus_popup_session_set_stream(pus_popup_session s, void* cuda_stream) {
-  if (!s) return refuse("session is NULL");
+  if (!s) return kSession.refuse("session is NULL");
   Session* S = (Session*)s;
   S->st = cuda_stream ? (cudaStream_t)cuda_stream : S->own;
   return 0;
 }
 
 extern "C" int pus_popup_session_memory(pus_popup_session s, long long* allocations, long long* reserved_bytes) {
-  if (!s) return refuse("session is NULL");
+  if (!s) return kSession.refuse("session is NULL");
   Session* S = (Session*)s;
   if (allocations) *allocations = S->n_allocs;
   if (reserved_bytes) *reserved_bytes = S->reserved;
@@ -360,13 +339,14 @@ extern "C" int pus_popup_session_memory(pus_popup_session s, long long* allocati
 extern "C" int pus_popup_session_run(pus_popup_session s, int n_frames, const unsigned char* images, const unsigned char* labels,
                                      const float* Ts) {
   using namespace pus::frames;
-  if (!s) return refuse("session is NULL");
-  if (n_frames < 0) return refuse("n_frames < 0");
-  if (n_frames > 0 && (!images || !labels || !Ts)) return refuse("images, labels and Ts must be given");
+  if (!s) return kSession.refuse("session is NULL");
+  if (n_frames < 0) return kSession.refuse("n_frames < 0");
+  if (n_frames > 0 && (!images || !labels || !Ts)) return kSession.refuse("images, labels and Ts must be given");
   Session& S = *(Session*)s;
   const pus_popup_config& c = S.cfg;
-  S.res = pus_popup_frames{};
-  SCHK(cudaSetDevice(S.device));
+  S.res = pus_popup_frames{};   // and so it stays until the run has succeeded
+  const Call C{"pus_popup_session_run"};
+  PUS_CALL_OK(C, cudaSetDevice(S.device));
   S.cursor = S.hcursor = 0;
   Arena A(S);
   cudaStream_t st = S.st;
@@ -403,14 +383,14 @@ extern "C" int pus_popup_session_run(pus_popup_session s, int n_frames, const un
   float* d_K = nullptr;
   long long* sizes = nullptr;
   long long* h_sizes = nullptr;
-  SCHK(input(images, (size_t)(n * px * c.channels), d_img));
-  SCHK(input(labels, (size_t)(n * px), d_lab));
-  SCHK(input(Ts, (size_t)n * 16, d_T));
-  SCHK(dev(d_K, 18));
-  SCHK(dev(sizes, S_N));
-  SCHK(pinned(h_sizes, S_N));
-  SCHK(cudaMemcpyAsync(d_K, c.K, 9 * sizeof(float), cudaMemcpyHostToDevice, st));
-  SCHK(cudaMemcpyAsync(d_K + 9, c.invK, 9 * sizeof(float), cudaMemcpyHostToDevice, st));
+  PUS_CALL_OK(C, input(images, (size_t)(n * px * c.channels), d_img));
+  PUS_CALL_OK(C, input(labels, (size_t)(n * px), d_lab));
+  PUS_CALL_OK(C, input(Ts, (size_t)n * 16, d_T));
+  PUS_CALL_OK(C, dev(d_K, 18));
+  PUS_CALL_OK(C, dev(sizes, S_N));
+  PUS_CALL_OK(C, pinned(h_sizes, S_N));
+  PUS_CALL_OK(C, cudaMemcpyAsync(d_K, c.K, 9 * sizeof(float), cudaMemcpyHostToDevice, st));
+  PUS_CALL_OK(C, cudaMemcpyAsync(d_K + 9, c.invK, 9 * sizeof(float), cudaMemcpyHostToDevice, st));
   const float *d_Kf = d_K, *d_iK = d_K + 9;
   auto readback = [&]() {   // one host synchronisation
     cudaError_t e = cudaMemcpyAsync(h_sizes, sizes, S_N * sizeof(long long), cudaMemcpyDeviceToHost, st);
@@ -424,25 +404,25 @@ extern "C" int pus_popup_session_run(pus_popup_session s, int n_frames, const un
   int *line_status = nullptr, *line_counts = nullptr, *status = nullptr, *edge_lines = nullptr;
   long long* first = nullptr;
   float* d_lines = nullptr;
-  SCHK(lines::detect(st, A, n, D, d_img, LW));
-  SCHK(dev(line_status, n));
-  SCHK(dev(line_counts, n));
-  SCHK(dev(status, n));
-  SCHK(dev(edge_lines, n));
-  SCHK(dev(first, n));
-  SCHK(dev(d_lines, 4 * (size_t)n * D.nslot));   // a frame has at most line_slots lines
+  PUS_CALL_OK(C, lines::detect(st, A, n, D, d_img, LW));
+  PUS_CALL_OK(C, dev(line_status, n));
+  PUS_CALL_OK(C, dev(line_counts, n));
+  PUS_CALL_OK(C, dev(status, n));
+  PUS_CALL_OK(C, dev(edge_lines, n));
+  PUS_CALL_OK(C, dev(first, n));
+  PUS_CALL_OK(C, dev(d_lines, 4 * (size_t)n * D.nslot));   // a frame has at most line_slots lines
   // 2. edges: label maps first, then the table from their segment counts and the lines
   edges::Maps M;
   edges::Frame* d_fr = nullptr;
-  SCHK(edges::prep(st, A, n, d_lab, W, H, c.edges, M));
-  SCHK(dev(d_fr, n));
+  PUS_CALL_OK(C, edges::prep(st, A, n, d_lab, W, H, c.edges, M));
+  PUS_CALL_OK(C, dev(d_fr, n));
   if (n > 0) {
     line_scan_kernel<<<1, kScan, 0, st>>>(n, LW.st, LW.fc, line_status, line_counts, first, sizes);
-    SCHK(lines::scatter(st, n, D, LW, first, d_lines));
+    PUS_CALL_OK(C, lines::scatter(st, n, D, LW, first, d_lines));
     line_check_kernel<<<fb, 128, 0, st>>>(n, line_counts, first, d_lines, status, edge_lines);
     edge_table_kernel<<<1, 1, 0, st>>>(n, M.seg_count, first, edge_lines, (long long)M.w * M.h, d_fr, sizes);
-    SCHK(cudaGetLastError());
-    SCHK(readback());   // sync 1: the line total and the edge scratch
+    PUS_CALL_OK(C, cudaGetLastError());
+    PUS_CALL_OK(C, readback());   // sync 1: the line total and the edge scratch
   } else {
     std::memset(h_sizes, 0, S_N * sizeof(long long));
   }
@@ -450,64 +430,65 @@ extern "C" int pus_popup_session_run(pus_popup_session s, int n_frames, const un
   const long long tot[4] = {h_sizes[S_NODE], h_sizes[S_OBJ], h_sizes[S_CPT], h_sizes[S_IVL]};
   float *open_slot = nullptr, *conn_slot = nullptr;
   int *inc_slot = nullptr, *eout = nullptr, *edge_status = nullptr, *open_ptr = nullptr, *conn_ptr = nullptr;
-  SCHK(dev(open_slot, 8 * n_lines));
-  SCHK(dev(conn_slot, 16 * n_lines));
-  SCHK(dev(inc_slot, 2 * n_lines));
-  SCHK(dev(eout, 4 * (size_t)n));
-  SCHK(dev(edge_status, n));
-  SCHK(dev(open_ptr, n + 1));
-  SCHK(dev(conn_ptr, n + 1));
-  SCHK(edges::select(st, A, n, c.edges, W, H, M, d_fr, tot, n_lines, d_lines, open_slot, conn_slot, inc_slot, eout));
+  PUS_CALL_OK(C, dev(open_slot, 8 * n_lines));
+  PUS_CALL_OK(C, dev(conn_slot, 16 * n_lines));
+  PUS_CALL_OK(C, dev(inc_slot, 2 * n_lines));
+  PUS_CALL_OK(C, dev(eout, 4 * (size_t)n));
+  PUS_CALL_OK(C, dev(edge_status, n));
+  PUS_CALL_OK(C, dev(open_ptr, n + 1));
+  PUS_CALL_OK(C, dev(conn_ptr, n + 1));
+  PUS_CALL_OK(C, edges::select(st, A, n, c.edges, W, H, M, d_fr, tot, n_lines, d_lines, open_slot, conn_slot, inc_slot, eout));
   if (n > 0) {
     edge_scan_kernel<<<1, kScan, 0, st>>>(n, eout, status, edge_status, open_ptr, conn_ptr, sizes);
-    SCHK(cudaGetLastError());
-    SCHK(readback());   // sync 2: the open and connected totals
+    PUS_CALL_OK(C, cudaGetLastError());
+    PUS_CALL_OK(C, readback());   // sync 2: the open and connected totals
   }
   const long long n_open = h_sizes[S_OPEN], n_conn = h_sizes[S_CONN];
   const int n_rows = (int)(n_open + n);
   // 3. fit on the open segments; the same launch gives the polygons their planes and world ground endpoints
   float *open = nullptr, *conn = nullptr, *pw = nullptr, *ps = nullptr, *dist = nullptr, *ends = nullptr;
   int *inc = nullptr, *row_frame = nullptr, *good = nullptr;
-  SCHK(dev(open, 4 * n_open));
-  SCHK(dev(conn, 4 * n_conn));
-  SCHK(dev(inc, n_open));
-  SCHK(dev(row_frame, n_rows));
-  SCHK(dev(pw, 4 * (size_t)n_rows));
-  SCHK(dev(ps, 4 * (size_t)n_rows));
-  SCHK(dev(dist, n_rows));
-  SCHK(dev(good, n_rows));
-  SCHK(dev(ends, 6 * (size_t)n_rows));
+  PUS_CALL_OK(C, dev(open, 4 * n_open));
+  PUS_CALL_OK(C, dev(conn, 4 * n_conn));
+  PUS_CALL_OK(C, dev(inc, n_open));
+  PUS_CALL_OK(C, dev(row_frame, n_rows));
+  PUS_CALL_OK(C, dev(pw, 4 * (size_t)n_rows));
+  PUS_CALL_OK(C, dev(ps, 4 * (size_t)n_rows));
+  PUS_CALL_OK(C, dev(dist, n_rows));
+  PUS_CALL_OK(C, dev(good, n_rows));
+  PUS_CALL_OK(C, dev(ends, 6 * (size_t)n_rows));
   // 5. polygons on the open segments (their rows are the fit's)
   float *bslot = nullptr, *cslot = nullptr, *wslot = nullptr, *bound = nullptr, *cut = nullptr, *world = nullptr;
   int *pcnt = nullptr, *ptr3 = nullptr, *n_good = nullptr, *good_ptr = nullptr;
   long long* poff = nullptr;
-  SCHK(dev(bslot, (size_t)n_rows * poly::kBoundSlot * 2));
-  SCHK(dev(cslot, (size_t)n_rows * poly::kCutSlot * 2));
-  SCHK(dev(wslot, (size_t)n_rows * poly::kCutSlot * 3));
-  SCHK(dev(bound, (size_t)n_rows * poly::kBoundSlot * 2));
-  SCHK(dev(cut, (size_t)n_rows * poly::kBoundSlot * 2));
-  SCHK(dev(world, (size_t)n_rows * poly::kCutSlot * 3));
-  SCHK(dev(pcnt, 3 * (size_t)n_rows));
-  SCHK(dev(poff, 3 * (size_t)n_rows));
-  SCHK(dev(ptr3, 3 * ((size_t)n_rows + 1)));
-  SCHK(dev(n_good, n));
-  SCHK(dev(good_ptr, n + 1));
+  PUS_CALL_OK(C, dev(bslot, (size_t)n_rows * poly::kBoundSlot * 2));
+  PUS_CALL_OK(C, dev(cslot, (size_t)n_rows * poly::kCutSlot * 2));
+  PUS_CALL_OK(C, dev(wslot, (size_t)n_rows * poly::kCutSlot * 3));
+  PUS_CALL_OK(C, dev(bound, (size_t)n_rows * poly::kBoundSlot * 2));
+  PUS_CALL_OK(C, dev(cut, (size_t)n_rows * poly::kBoundSlot * 2));
+  PUS_CALL_OK(C, dev(world, (size_t)n_rows * poly::kCutSlot * 3));
+  PUS_CALL_OK(C, dev(pcnt, 3 * (size_t)n_rows));
+  PUS_CALL_OK(C, dev(poff, 3 * (size_t)n_rows));
+  PUS_CALL_OK(C, dev(ptr3, 3 * ((size_t)n_rows + 1)));
+  PUS_CALL_OK(C, dev(n_good, n));
+  PUS_CALL_OK(C, dev(good_ptr, n + 1));
   const poly::Params PP{open_ptr, row_frame, n_rows, open, d_Kf, d_iK, d_T, ps, ends, W, H, c.ceiling_threshold,
                         c.walllength_threshold, bslot, cslot, wslot, pcnt};
   if (n > 0) {
     edge_pack_kernel<<<fb, 128, 0, st>>>(n, first, open_ptr, conn_ptr, open_slot, conn_slot, inc_slot, open, conn, inc,
                                          row_frame);
-    SCHK(cudaMemsetAsync(pw, 0, 4 * (size_t)n_rows * sizeof(float), st));
-    SCHK(cudaMemsetAsync(ps, 0, 4 * (size_t)n_rows * sizeof(float), st));
-    SCHK(cudaMemsetAsync(dist, 0, (size_t)n_rows * sizeof(float), st));
-    SCHK(cudaMemsetAsync(good, 0, (size_t)n_rows * sizeof(int), st));
-    SCHK(launch_fit(st, n, open_ptr, row_frame, n_rows, open, d_iK, d_T, c.plane_cam_dist_thre, 0, pw, ps, dist, good, ends));
-    SCHK(poly::launch_rows(st, PP));
+    PUS_CALL_OK(C, cudaMemsetAsync(pw, 0, 4 * (size_t)n_rows * sizeof(float), st));
+    PUS_CALL_OK(C, cudaMemsetAsync(ps, 0, 4 * (size_t)n_rows * sizeof(float), st));
+    PUS_CALL_OK(C, cudaMemsetAsync(dist, 0, (size_t)n_rows * sizeof(float), st));
+    PUS_CALL_OK(C, cudaMemsetAsync(good, 0, (size_t)n_rows * sizeof(int), st));
+    PUS_CALL_OK(C, launch_fit(st, n, open_ptr, row_frame, n_rows, open, d_iK, d_T, c.plane_cam_dist_thre, 0, pw, ps, dist, good,
+                              ends));
+    PUS_CALL_OK(C, poly::launch_rows(st, PP));
     // 4. the actual-index filter, then the offsets
     filter_kernel<<<fb, 128, 0, st>>>(n, open_ptr, inc, good, n_good);
     row_scan_kernel<<<4, kScan, 0, st>>>(n, n_rows, n_good, pcnt, good_ptr, poff, ptr3, sizes);
-    SCHK(poly::launch_pack(st, PP, poff, bound, cut, world));
-    SCHK(cudaGetLastError());
+    PUS_CALL_OK(C, poly::launch_pack(st, PP, poff, bound, cut, world));
+    PUS_CALL_OK(C, cudaGetLastError());
   }
   // 6. / 7. the good rows' jobs for the clouds and the depth map
   const int vcap = n_rows * poly::kBoundSlot;
@@ -515,21 +496,21 @@ extern "C" int pus_popup_session_run(pus_popup_session s, int n_frames, const un
   float* planes = nullptr;
   cloud::Job *cjobs = nullptr, *djobs = nullptr;
   int2 *cvtx = nullptr, *dvtx = nullptr;
-  SCHK(dev(good_rows, n_rows));
-  SCHK(dev(plane_status, n_rows));
-  SCHK(dev(planes, 4 * (size_t)n_rows));
-  SCHK(dev(cjobs, n_rows));
-  SCHK(dev(djobs, n_rows));
-  SCHK(dev(cvtx, vcap));
-  SCHK(dev(dvtx, vcap));
+  PUS_CALL_OK(C, dev(good_rows, n_rows));
+  PUS_CALL_OK(C, dev(plane_status, n_rows));
+  PUS_CALL_OK(C, dev(planes, 4 * (size_t)n_rows));
+  PUS_CALL_OK(C, dev(cjobs, n_rows));
+  PUS_CALL_OK(C, dev(djobs, n_rows));
+  PUS_CALL_OK(C, dev(cvtx, vcap));
+  PUS_CALL_OK(C, dev(dvtx, vcap));
   const int cloud_from_cut = c.walllength_threshold > 0;
   if (n > 0) {
     frames::JobArgs JA{n, c.downsample_poly ? 1 : 0, cloud_from_cut, open_ptr, good, good_ptr, ps, bound, cut,
                        ptr3, ptr3 + (n_rows + 1), good_rows, plane_status, planes, cjobs, djobs, cvtx, dvtx};
     job_kernel<<<fb, 128, 0, st>>>(JA);
     job_scan_kernel<<<1, kScan, 0, st>>>(n, good_ptr, cjobs, djobs, sizes);
-    SCHK(cudaGetLastError());
-    SCHK(readback());   // sync 3: good planes, vertex totals, box rows
+    PUS_CALL_OK(C, cudaGetLastError());
+    PUS_CALL_OK(C, readback());   // sync 3: good planes, vertex totals, box rows
   }
   const int n_planes = (int)h_sizes[S_GOOD];
   const long long crows = h_sizes[S_CROWS], drows = h_sizes[S_DROWS];
@@ -537,45 +518,45 @@ extern "C" int pus_popup_session_run(pus_popup_session s, int n_frames, const un
   int2* cspan = nullptr;
   int *rowcnt = nullptr, *ccount = nullptr;
   long long *rowoff = nullptr, *coff = nullptr;
-  SCHK(dev(cspan, crows));
-  SCHK(dev(rowcnt, crows));
-  SCHK(dev(rowoff, crows + 1));
-  SCHK(dev(ccount, n_planes));
-  SCHK(dev(coff, n_planes));
+  PUS_CALL_OK(C, dev(cspan, crows));
+  PUS_CALL_OK(C, dev(rowcnt, crows));
+  PUS_CALL_OK(C, dev(rowoff, crows + 1));
+  PUS_CALL_OK(C, dev(ccount, n_planes));
+  PUS_CALL_OK(C, dev(coff, n_planes));
   cloud::Params CP{cjobs, cvtx, planes, d_T, d_iK, c.want_rgb ? d_img : nullptr, W, H, c.downsample_poly ? 2 : 1, c.channels == 3 && W == 960,
                    c.depth_thre, c.ceiling_threshold, cspan, rowcnt, rowoff, nullptr, nullptr};
   long long n_points = 0;
   if (n > 0) {
-    SCHK(cloud::launch_count(st, n_planes, crows, CP, rowoff, ccount, coff));
-    SCHK(cudaMemcpyAsync(sizes, rowoff + crows, sizeof(long long), cudaMemcpyDeviceToDevice, st));
-    SCHK(readback());   // sync 4: the point total
+    PUS_CALL_OK(C, cloud::launch_count(st, n_planes, crows, CP, rowoff, ccount, coff));
+    PUS_CALL_OK(C, cudaMemcpyAsync(sizes, rowoff + crows, sizeof(long long), cudaMemcpyDeviceToDevice, st));
+    PUS_CALL_OK(C, readback());   // sync 4: the point total
     n_points = h_sizes[0];
   }
   float* xyz = nullptr;
   unsigned char *rgb = nullptr, *lab = nullptr;
   float *depth = nullptr, *fill = nullptr;
-  SCHK(dev(xyz, 3 * n_points));
-  SCHK(dev(rgb, c.want_rgb ? 3 * n_points : 0));
-  SCHK(dev(lab, c.want_labels ? (size_t)(n * px) : 0));
+  PUS_CALL_OK(C, dev(xyz, 3 * n_points));
+  PUS_CALL_OK(C, dev(rgb, c.want_rgb ? 3 * n_points : 0));
+  PUS_CALL_OK(C, dev(lab, c.want_labels ? (size_t)(n * px) : 0));
   const int scale = c.downsample_poly ? 2 : 1;
-  SCHK(dev(depth, c.want_depth ? (size_t)(n * px) : 0));
-  SCHK(dev(fill, c.want_depth && scale == 2 ? (size_t)n * (W / 2) * (H / 2) : 0));
+  PUS_CALL_OK(C, dev(depth, c.want_depth ? (size_t)(n * px) : 0));
+  PUS_CALL_OK(C, dev(fill, c.want_depth && scale == 2 ? (size_t)n * (W / 2) * (H / 2) : 0));
   cloud::Edge* dedges = nullptr;
   int2* dspan = nullptr;
-  SCHK(dev(dedges, c.want_depth ? vcap : 0));
-  SCHK(dev(dspan, c.want_depth ? drows : 0));
+  PUS_CALL_OK(C, dev(dedges, c.want_depth ? vcap : 0));
+  PUS_CALL_OK(C, dev(dspan, c.want_depth ? drows : 0));
   if (n > 0) {
     CP.xyz = xyz;
     CP.rgb = c.want_rgb ? rgb : nullptr;
-    if (n_points > 0) SCHK(cloud::launch_write(st, n_planes, CP));
+    if (n_points > 0) PUS_CALL_OK(C, cloud::launch_write(st, n_planes, CP));
     if (c.want_labels) {
-      SCHK(cudaMemsetAsync(lab, 127, (size_t)(n * px), st));
-      SCHK(cloud::launch_labels(st, n, good_ptr, CP, lab));
+      PUS_CALL_OK(C, cudaMemsetAsync(lab, 127, (size_t)(n * px), st));
+      PUS_CALL_OK(C, cloud::launch_labels(st, n, good_ptr, CP, lab));
     }
     if (c.want_depth)
-      SCHK(cloud::launch_depth(st, n, n_planes, good_ptr, djobs, dvtx, dedges, dspan, planes, d_T, d_iK, W, H, c.downsample_poly,
-                               c.ceiling_threshold, scale == 2 ? fill : depth, depth));
-    SCHK(cudaGetLastError());
+      PUS_CALL_OK(C, cloud::launch_depth(st, n, n_planes, good_ptr, djobs, dvtx, dedges, dspan, planes, d_T, d_iK, W, H,
+                                         c.downsample_poly, c.ceiling_threshold, scale == 2 ? fill : depth, depth));
+    PUS_CALL_OK(C, cudaGetLastError());
   }
   pus_popup_frames& R = S.res;
   R.n_frames = n;
@@ -599,13 +580,13 @@ extern "C" int pus_popup_session_run(pus_popup_session s, int n_frames, const un
 }
 
 extern "C" int pus_popup_session_result(pus_popup_session s, pus_popup_frames* out) {
-  if (!s || !out) return refuse("session and out must be given");
+  if (!s || !out) return kSession.refuse("session and out must be given");
   *out = ((Session*)s)->res;
   return 0;
 }
 
 extern "C" int pus_popup_session_download(pus_popup_session s, pus_popup_frames* dst) {
-  if (!s || !dst) return refuse("session and dst must be given");
+  if (!s || !dst) return kSession.refuse("session and dst must be given");
   Session& S = *(Session*)s;
   const pus_popup_frames& R = S.res;
   const long long n = R.n_frames, rows = R.n_rows, g = R.n_good, px = (long long)S.cfg.width * S.cfg.height;
@@ -623,13 +604,13 @@ extern "C" int pus_popup_session_download(pus_popup_session s, pus_popup_frames*
       {dst->plane_status, R.plane_status, 4 * g}, {dst->cloud_counts, R.cloud_counts, 4 * g},
       {dst->cloud_offsets, R.cloud_offsets, 8 * g}, {dst->xyz, R.xyz, 12 * R.n_points},
       {dst->rgb, R.rgb, 3 * R.n_points}, {dst->labels, R.labels, n * px}, {dst->depth, R.depth, 4 * n * px}};
-  if (n > 0 && !R.status) return refuse("no successful run to download");
+  if (n > 0 && !R.status) return kSession.refuse("no successful run to download");
   if ((dst->rgb && !R.rgb) || (dst->labels && !R.labels) || (dst->depth && !R.depth))
-    return refuse("an optional output the config does not make was asked for");
+    return kSession.refuse("an optional output the config does not make was asked for");
   cudaError_t e = cudaSetDevice(S.device);
   for (const Copy& c : copies)
     if (e == cudaSuccess && c.d && c.bytes > 0) e = cudaMemcpyAsync(c.d, c.s, (size_t)c.bytes, cudaMemcpyDefault, S.st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(S.st);
-  if (e != cudaSuccess) return refuse(std::string("download: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return kSession.refuse(std::string("download: ") + cudaGetErrorString(e));
   return 0;
 }

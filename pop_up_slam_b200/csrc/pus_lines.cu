@@ -17,8 +17,6 @@
 #include "pus_stages.cuh"
 
 namespace pus {
-extern thread_local std::string g_err;
-
 namespace lines {
 
 __device__ __forceinline__ int refl(int p, int n) { return p < 0 ? -p : (p >= n ? 2 * n - 2 - p : p); }
@@ -261,6 +259,15 @@ Dims make_dims(int width, int height, int channels, int downsample) {
   return D;
 }
 
+const char* shape_error(int width, int height, int channels, int downsample) {
+  if (channels != 1 && channels != 3) return "channels must be 1 (grey) or 3 (BGR)";
+  if (downsample && ((width & 1) || (height & 1))) return "downsample needs even width and height";
+  const int w = downsample ? width / 2 : width, h = downsample ? height / 2 : height;
+  if (w < 3 || h < 3) return "the detection image (after the optional halving) must be at least 3 x 3";
+  if ((long long)width * height > PUS_POPUP_LINES_MAX_PIXELS) return "a frame has more than 2^28 pixels";
+  return nullptr;
+}
+
 #define WCHK(call)                        \
   do {                                    \
     const cudaError_t e__ = (call);       \
@@ -320,45 +327,29 @@ cudaError_t scatter(cudaStream_t st, int n_frames, const Dims& D, const Work& W,
 }  // namespace lines
 }  // namespace pus
 
-#define LCHK(call)                                                                                          \
-  do {                                                                                                      \
-    cudaError_t e__ = (call);                                                                               \
-    if (e__ != cudaSuccess) { g_err = std::string("pus_popup_lines: ") + #call + ": " + cudaGetErrorString(e__); return -1; } \
-  } while (0)
-
 extern "C" long long pus_popup_lines(int device, int n_frames, const unsigned char* images, int width, int height,
                                      int channels, int downsample, int* status, int* counts, float* lines,
                                      long long capacity) {
   using namespace pus;
   using namespace pus::lines;
-  auto refuse = [](const char* why) { g_err = std::string("pus_popup_lines: ") + why; return -1LL; };
-  if (n_frames < 0) return refuse("n_frames < 0");
-  if (!images && n_frames > 0) return refuse("images is NULL");
-  if (!status || !counts) return refuse("status and counts are required");
-  if (channels != 1 && channels != 3) return refuse("channels must be 1 (grey) or 3 (BGR)");
-  if (downsample && ((width & 1) || (height & 1))) return refuse("downsample needs even width and height");
-  const int w = downsample ? width / 2 : width, h = downsample ? height / 2 : height;
-  if (w < 3 || h < 3) return refuse("the detection image (after the optional halving) must be at least 3 x 3");
-  if ((long long)width * height > PUS_POPUP_LINES_MAX_PIXELS) return refuse("a frame has more than 2^28 pixels");
-  {
-    int ndev = 0;
-    cudaError_t de = cudaGetDeviceCount(&ndev);
-    if (de != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
-      return refuse("no CUDA device usable; libpopup_gpu has no CPU fallback");
-  }
+  const Call C{"pus_popup_lines"};
+  if (n_frames < 0) return C.refuse("n_frames < 0");
+  if (!images && n_frames > 0) return C.refuse("images is NULL");
+  if (!status || !counts) return C.refuse("status and counts are required");
+  if (const char* why = shape_error(width, height, channels, downsample)) return C.refuse(why);
+  if (C.check_device(device) < 0) return -1;
   if (n_frames == 0) return 0;
-  LCHK(cudaSetDevice(device));
+  PUS_CALL_OK(C, cudaSetDevice(device));
   const Dims D = make_dims(width, height, channels, downsample);
   const long long F = n_frames;
   TempAlloc A;
   Work W;
   unsigned char* d_img = nullptr;
-  LCHK(A.get(d_img, F * D.N * channels));
-  LCHK(cudaMemcpy(d_img, images, (size_t)(F * D.N * channels), cudaMemcpyHostToDevice));
-  LCHK(detect(0, A, n_frames, D, d_img, W));
+  PUS_CALL_OK(C, A.upload(d_img, images, (size_t)(F * D.N * channels)));
+  PUS_CALL_OK(C, detect(0, A, n_frames, D, d_img, W));
   std::vector<int> st(F), fc(F);
-  LCHK(cudaMemcpy(st.data(), W.st, F * sizeof(int), cudaMemcpyDeviceToHost));
-  LCHK(cudaMemcpy(fc.data(), W.fc, F * sizeof(int), cudaMemcpyDeviceToHost));
+  PUS_CALL_OK(C, download(st.data(), W.st, F));
+  PUS_CALL_OK(C, download(fc.data(), W.fc, F));
   std::vector<long long> ff(F);
   long long total = 0;
   for (int f = 0; f < n_frames; f++) {
@@ -368,14 +359,13 @@ extern "C" long long pus_popup_lines(int device, int n_frames, const unsigned ch
     total += counts[f];
   }
   if (!lines) return total;   // size query
-  if (capacity < total) return refuse("capacity is smaller than the number of lines");
+  if (capacity < total) return C.refuse("capacity is smaller than the number of lines");
   if (total == 0) return 0;
   long long* d_ff = nullptr;
   float* d_out = nullptr;
-  LCHK(A.get(d_ff, F));
-  LCHK(A.get(d_out, 4 * total));
-  LCHK(cudaMemcpy(d_ff, ff.data(), F * sizeof(long long), cudaMemcpyHostToDevice));
-  LCHK(scatter(0, n_frames, D, W, d_ff, d_out));
-  LCHK(cudaMemcpy(lines, d_out, 4 * total * sizeof(float), cudaMemcpyDeviceToHost));
+  PUS_CALL_OK(C, A.upload(d_ff, ff.data(), F));
+  PUS_CALL_OK(C, A.get(d_out, 4 * total));
+  PUS_CALL_OK(C, scatter(0, n_frames, D, W, d_ff, d_out));
+  PUS_CALL_OK(C, download(lines, d_out, 4 * total));
   return total;
 }

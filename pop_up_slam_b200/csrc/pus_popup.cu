@@ -23,8 +23,6 @@
 #include "pus_stages.cuh"
 
 namespace pus {
-extern thread_local std::string g_err;
-
 __device__ __forceinline__ float seg_dist(const float* b, const float* e, const float* q) {
   float dx = e[0] - b[0], dy = e[1] - b[1];
   float length = sqrtf(dx * dx + dy * dy);
@@ -190,62 +188,41 @@ cudaError_t launch_project(cudaStream_t st, int n, const int* d_plane_idx, const
 
 using namespace pus;
 
-#define PCHK(call)                                                                  \
-  do {                                                                              \
-    cudaError_t e__ = (call);                                                       \
-    if (e__ != cudaSuccess) { g_err = std::string(#call) + ": " + cudaGetErrorString(e__); rc = -1; goto done; } \
-  } while (0)
-
 extern "C" int pus_popup_fit_frames(int device, int n_frames, const int* seg_ptr, const float* segs, const float* invK,
                                     const float* Ts, float dist_thre, int mode, float* planes_world, float* planes_sensor,
                                     float* dist, int* good) {
-  int rc = 0;
+  const Call C{"pus_popup_fit_frames"};
   if (n_frames <= 0) return 0;
+  std::vector<int> rf;
+  if (const char* why = row_frames(n_frames, seg_ptr, rf)) return C.refuse(why);
   const int n_seg = seg_ptr[n_frames];
   const int n_rows = n_seg + n_frames;
+  if (C.check_device(device) < 0) return -1;
+  PUS_CALL_OK(C, cudaSetDevice(device));
+  TempAlloc A;
   int *d_ptr = nullptr, *d_rf = nullptr, *d_good = nullptr;
   float *d_segs = nullptr, *d_K = nullptr, *d_T = nullptr, *d_pw = nullptr, *d_ps = nullptr, *d_dist = nullptr;
-  int* rf = new int[n_rows];
-  for (int f = 0; f < n_frames; f++)
-    for (int r = seg_ptr[f] + f; r < seg_ptr[f + 1] + f + 1; r++) rf[r] = f;
-  {
-    int ndev = 0;
-    cudaError_t de = cudaGetDeviceCount(&ndev);
-    if (de != cudaSuccess || ndev <= 0 || device >= ndev) {
-      g_err = "pus_popup_fit_frames: no usable CUDA device; libpopup_gpu has no CPU fallback";
-      delete[] rf;
-      return -1;
-    }
-  }
-  PCHK(cudaSetDevice(device));
-  PCHK(cudaMalloc(&d_ptr, (n_frames + 1) * sizeof(int)));
-  PCHK(cudaMalloc(&d_rf, n_rows * sizeof(int)));
-  PCHK(cudaMalloc(&d_segs, (size_t)(n_seg > 0 ? n_seg : 1) * 4 * sizeof(float)));
-  PCHK(cudaMalloc(&d_K, 9 * sizeof(float)));
-  PCHK(cudaMalloc(&d_T, (size_t)n_frames * 16 * sizeof(float)));
-  PCHK(cudaMalloc(&d_pw, (size_t)n_rows * 4 * sizeof(float)));
-  PCHK(cudaMalloc(&d_ps, (size_t)n_rows * 4 * sizeof(float)));
-  PCHK(cudaMalloc(&d_dist, (size_t)n_rows * sizeof(float)));
-  PCHK(cudaMalloc(&d_good, (size_t)n_rows * sizeof(int)));
-  PCHK(cudaMemcpy(d_ptr, seg_ptr, (n_frames + 1) * sizeof(int), cudaMemcpyHostToDevice));
-  PCHK(cudaMemcpy(d_rf, rf, n_rows * sizeof(int), cudaMemcpyHostToDevice));
-  if (n_seg > 0) PCHK(cudaMemcpy(d_segs, segs, (size_t)n_seg * 4 * sizeof(float), cudaMemcpyHostToDevice));
-  PCHK(cudaMemcpy(d_K, invK, 9 * sizeof(float), cudaMemcpyHostToDevice));
-  PCHK(cudaMemcpy(d_T, Ts, (size_t)n_frames * 16 * sizeof(float), cudaMemcpyHostToDevice));
-  PCHK(cudaMemset(d_pw, 0, (size_t)n_rows * 4 * sizeof(float)));
-  PCHK(cudaMemset(d_ps, 0, (size_t)n_rows * 4 * sizeof(float)));
-  PCHK(cudaMemset(d_dist, 0, (size_t)n_rows * sizeof(float)));
-  PCHK(cudaMemset(d_good, 0, (size_t)n_rows * sizeof(int)));
-  PCHK(launch_fit(0, n_frames, d_ptr, d_rf, n_rows, d_segs, d_K, d_T, dist_thre, mode, d_pw, d_ps, d_dist, d_good, nullptr));
-  PCHK(cudaDeviceSynchronize());
-  if (planes_world) PCHK(cudaMemcpy(planes_world, d_pw, (size_t)n_rows * 4 * sizeof(float), cudaMemcpyDeviceToHost));
-  if (planes_sensor) PCHK(cudaMemcpy(planes_sensor, d_ps, (size_t)n_rows * 4 * sizeof(float), cudaMemcpyDeviceToHost));
-  if (dist) PCHK(cudaMemcpy(dist, d_dist, (size_t)n_rows * sizeof(float), cudaMemcpyDeviceToHost));
-  if (good) PCHK(cudaMemcpy(good, d_good, (size_t)n_rows * sizeof(int), cudaMemcpyDeviceToHost));
-done:
-  delete[] rf;
-  cudaFree(d_ptr); cudaFree(d_rf); cudaFree(d_segs); cudaFree(d_K); cudaFree(d_T); cudaFree(d_pw); cudaFree(d_ps); cudaFree(d_dist); cudaFree(d_good);
-  return rc;
+  PUS_CALL_OK(C, A.upload(d_ptr, seg_ptr, n_frames + 1));
+  PUS_CALL_OK(C, A.upload(d_rf, rf.data(), n_rows));
+  PUS_CALL_OK(C, A.upload(d_segs, segs, (size_t)n_seg * 4));
+  PUS_CALL_OK(C, A.upload(d_K, invK, 9));
+  PUS_CALL_OK(C, A.upload(d_T, Ts, (size_t)n_frames * 16));
+  PUS_CALL_OK(C, A.get(d_pw, (size_t)n_rows * 4));
+  PUS_CALL_OK(C, A.get(d_ps, (size_t)n_rows * 4));
+  PUS_CALL_OK(C, A.get(d_dist, n_rows));
+  PUS_CALL_OK(C, A.get(d_good, n_rows));
+  PUS_CALL_OK(C, cudaMemset(d_pw, 0, (size_t)n_rows * 4 * sizeof(float)));
+  PUS_CALL_OK(C, cudaMemset(d_ps, 0, (size_t)n_rows * 4 * sizeof(float)));
+  PUS_CALL_OK(C, cudaMemset(d_dist, 0, (size_t)n_rows * sizeof(float)));
+  PUS_CALL_OK(C, cudaMemset(d_good, 0, (size_t)n_rows * sizeof(int)));
+  PUS_CALL_OK(C, launch_fit(0, n_frames, d_ptr, d_rf, n_rows, d_segs, d_K, d_T, dist_thre, mode, d_pw, d_ps, d_dist, d_good,
+                            nullptr));
+  PUS_CALL_OK(C, cudaDeviceSynchronize());
+  if (planes_world) PUS_CALL_OK(C, download(planes_world, d_pw, (size_t)n_rows * 4));
+  if (planes_sensor) PUS_CALL_OK(C, download(planes_sensor, d_ps, (size_t)n_rows * 4));
+  if (dist) PUS_CALL_OK(C, download(dist, d_dist, n_rows));
+  if (good) PUS_CALL_OK(C, download(good, d_good, n_rows));
+  return 0;
 }
 
 // ---- dense plane clouds (pus_popup_clouds) ------------------------------------------------------------------------------
@@ -697,21 +674,14 @@ cudaError_t launch_depth(cudaStream_t st, int n_frames, int n_planes, const int*
 }  // namespace pus
 
 namespace {
-template <class T>
-struct DevBuf {   // a device allocation freed on every return path
-  T* p = nullptr;
-  ~DevBuf() { cudaFree(p); }
-  cudaError_t alloc(size_t n) { return cudaMalloc(&p, (n > 0 ? n : 1) * sizeof(T)); }
-};
-
 // The planes' polygon arguments of pus_popup_clouds and pus_popup_depth, checked, and per polygon matrix_to_points'
 // truncation, boundingRect and the box-shifted vertices (popup_plane.cpp:85-96).  Returns the number of box rows in all, or
-// -1 with g_err set (prefixed by who).
-long long plane_jobs(const char* who, int n_frames, const int* plane_ptr, const int* poly_ptr, const float* polys,
+// -1 refused through C.
+long long plane_jobs(const Call& C, int n_frames, const int* plane_ptr, const int* poly_ptr, const float* polys,
                      const float* planes_sensor, const float* Ts, const float* invK, int downsample,
                      std::vector<pus::cloud::Job>& jobs, std::vector<int2>& vtx) {
   using pus::cloud::Job;
-  auto refuse = [&](const char* why) { g_err = std::string(who) + why; return -1LL; };
+  auto refuse = [&](const char* why) { return (long long)C.refuse(why); };
   for (int f = 0; f < n_frames; f++)
     if (plane_ptr[f + 1] < plane_ptr[f]) return refuse("plane_ptr is not ascending");
   const int n_planes = plane_ptr[n_frames];
@@ -743,153 +713,110 @@ long long plane_jobs(const char* who, int n_frames, const int* plane_ptr, const 
 }
 }  // namespace
 
-#define CCHK(call)                                                                                        \
-  do {                                                                                                    \
-    cudaError_t e__ = (call);                                                                             \
-    if (e__ != cudaSuccess) { g_err = std::string("pus_popup_clouds: ") + #call + ": " + cudaGetErrorString(e__); return -1; } \
-  } while (0)
-
 extern "C" long long pus_popup_clouds(int device, int n_frames, const int* plane_ptr, const int* poly_ptr, const float* polys,
                                       const float* planes_sensor, const float* Ts, const float* invK,
                                       const unsigned char* images, int width, int height, int downsample, float depth_thre,
                                       float ceiling_threshold, int* counts, long long* offsets, float* xyz, unsigned char* rgb,
                                       long long capacity, unsigned char* labels) {
   using namespace pus::cloud;
-  auto refuse = [](const char* why) { g_err = std::string("pus_popup_clouds: ") + why; return -1LL; };
-  if (n_frames < 0) return refuse("n_frames < 0");
-  if (!plane_ptr || plane_ptr[0] != 0) return refuse("plane_ptr must be given and start at 0");
-  if (width <= 0 || height <= 0) return refuse("width and height must be positive");
-  if (labels && downsample && ((width | height) & 1)) return refuse("label images in downsample mode need an even width and height");
+  const Call C{"pus_popup_clouds"};
+  if (n_frames < 0) return C.refuse("n_frames < 0");
+  if (!plane_ptr || plane_ptr[0] != 0) return C.refuse("plane_ptr must be given and start at 0");
+  if (width <= 0 || height <= 0) return C.refuse("width and height must be positive");
+  if (labels && downsample && ((width | height) & 1)) return C.refuse("label images in downsample mode need an even width and height");
   std::vector<Job> jobs;
   std::vector<int2> vtx;
-  const long long rows = plane_jobs("pus_popup_clouds: ", n_frames, plane_ptr, poly_ptr, polys, planes_sensor, Ts, invK,
-                                    downsample, jobs, vtx);
+  const long long rows = plane_jobs(C, n_frames, plane_ptr, poly_ptr, polys, planes_sensor, Ts, invK, downsample, jobs, vtx);
   if (rows < 0) return -1;
   const int n_planes = (int)jobs.size(), n_vtx = (int)vtx.size();
-  {
-    int ndev = 0;
-    cudaError_t de = cudaGetDeviceCount(&ndev);
-    if (de != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
-      return refuse("no CUDA device usable; libpopup_gpu has no CPU fallback");
-  }
-  CCHK(cudaSetDevice(device));
-  DevBuf<Job> d_jobs;
-  DevBuf<int2> d_vtx, d_span;
-  DevBuf<float> d_planes, d_T, d_K, d_xyz;
-  DevBuf<unsigned char> d_img, d_rgb, d_lab;
-  DevBuf<int> d_rowcnt, d_cnt, d_ptr;
-  DevBuf<long long> d_rowoff, d_off;
+  if (C.check_device(device) < 0) return -1;
+  PUS_CALL_OK(C, cudaSetDevice(device));
+  TempAlloc A;
+  Job* d_jobs = nullptr;
+  int2 *d_vtx = nullptr, *d_span = nullptr;
+  float *d_planes = nullptr, *d_T = nullptr, *d_K = nullptr, *d_xyz = nullptr;
+  unsigned char *d_img = nullptr, *d_rgb = nullptr, *d_lab = nullptr;
+  int *d_rowcnt = nullptr, *d_cnt = nullptr, *d_ptr = nullptr;
+  long long *d_rowoff = nullptr, *d_off = nullptr;
   const size_t img_bytes = (size_t)n_frames * width * height * 3;
-  CCHK(d_jobs.alloc(n_planes));
-  CCHK(d_vtx.alloc(n_vtx));
-  CCHK(d_span.alloc(rows));
-  CCHK(d_planes.alloc((size_t)n_planes * 4));
-  CCHK(d_T.alloc((size_t)n_frames * 16));
-  CCHK(d_K.alloc(9));
-  CCHK(d_rowcnt.alloc(rows));
-  CCHK(d_rowoff.alloc(rows + 1));
-  CCHK(d_cnt.alloc(n_planes));
-  CCHK(d_off.alloc(n_planes));
-  if (n_planes > 0) {
-    CCHK(cudaMemcpy(d_jobs.p, jobs.data(), n_planes * sizeof(Job), cudaMemcpyHostToDevice));
-    CCHK(cudaMemcpy(d_planes.p, planes_sensor, (size_t)n_planes * 4 * sizeof(float), cudaMemcpyHostToDevice));
-  }
-  if (n_vtx > 0) CCHK(cudaMemcpy(d_vtx.p, vtx.data(), n_vtx * sizeof(int2), cudaMemcpyHostToDevice));
-  if (n_frames > 0) {
-    CCHK(cudaMemcpy(d_T.p, Ts, (size_t)n_frames * 16 * sizeof(float), cudaMemcpyHostToDevice));
-    CCHK(cudaMemcpy(d_K.p, invK, 9 * sizeof(float), cudaMemcpyHostToDevice));
-  }
-  if (images && rgb) {
-    CCHK(d_img.alloc(img_bytes));
-    CCHK(cudaMemcpy(d_img.p, images, img_bytes, cudaMemcpyHostToDevice));
-  }
-  Params P{d_jobs.p, d_vtx.p, d_planes.p, d_T.p, d_K.p, d_img.p, width, height, downsample ? 2 : 1, images && width == 960, depth_thre,
-           ceiling_threshold, d_span.p, d_rowcnt.p, d_rowoff.p, nullptr, nullptr};
-  CCHK(launch_count(0, n_planes, rows, P, d_rowoff.p, d_cnt.p, d_off.p));
+  PUS_CALL_OK(C, A.upload(d_jobs, jobs.data(), n_planes));
+  PUS_CALL_OK(C, A.upload(d_planes, planes_sensor, (size_t)n_planes * 4));
+  PUS_CALL_OK(C, A.upload(d_vtx, vtx.data(), n_vtx));
+  PUS_CALL_OK(C, A.upload(d_T, Ts, (size_t)n_frames * 16));
+  PUS_CALL_OK(C, A.upload(d_K, invK, n_frames > 0 ? 9 : 0));
+  PUS_CALL_OK(C, A.get(d_span, rows));
+  PUS_CALL_OK(C, A.get(d_rowcnt, rows));
+  PUS_CALL_OK(C, A.get(d_rowoff, rows + 1));
+  PUS_CALL_OK(C, A.get(d_cnt, n_planes));
+  PUS_CALL_OK(C, A.get(d_off, n_planes));
+  if (images && rgb) PUS_CALL_OK(C, A.upload(d_img, images, img_bytes));
+  Params P{d_jobs, d_vtx, d_planes, d_T, d_K, d_img, width, height, downsample ? 2 : 1, images && width == 960, depth_thre,
+           ceiling_threshold, d_span, d_rowcnt, d_rowoff, nullptr, nullptr};
+  PUS_CALL_OK(C, launch_count(0, n_planes, rows, P, d_rowoff, d_cnt, d_off));
   long long total = 0;
-  CCHK(cudaMemcpy(&total, d_rowoff.p + rows, sizeof(long long), cudaMemcpyDeviceToHost));
-  if (counts && n_planes > 0) CCHK(cudaMemcpy(counts, d_cnt.p, n_planes * sizeof(int), cudaMemcpyDeviceToHost));
-  if (offsets && n_planes > 0) CCHK(cudaMemcpy(offsets, d_off.p, n_planes * sizeof(long long), cudaMemcpyDeviceToHost));
-  if ((xyz || rgb) && capacity < total) return refuse("capacity is smaller than the number of points");
+  PUS_CALL_OK(C, download(&total, d_rowoff + rows, 1));
+  if (counts) PUS_CALL_OK(C, download(counts, d_cnt, n_planes));
+  if (offsets) PUS_CALL_OK(C, download(offsets, d_off, n_planes));
+  if ((xyz || rgb) && capacity < total) return C.refuse("capacity is smaller than the number of points");
   if ((xyz || rgb) && total > 0) {
-    if (xyz) CCHK(d_xyz.alloc((size_t)total * 3));
-    if (rgb) CCHK(d_rgb.alloc((size_t)total * 3));
-    P.xyz = d_xyz.p;
-    P.rgb = d_rgb.p;
-    CCHK(launch_write(0, n_planes, P));
-    if (xyz) CCHK(cudaMemcpy(xyz, d_xyz.p, (size_t)total * 3 * sizeof(float), cudaMemcpyDeviceToHost));
-    if (rgb) CCHK(cudaMemcpy(rgb, d_rgb.p, (size_t)total * 3, cudaMemcpyDeviceToHost));
+    if (xyz) PUS_CALL_OK(C, A.get(d_xyz, (size_t)total * 3));
+    if (rgb) PUS_CALL_OK(C, A.get(d_rgb, (size_t)total * 3));
+    P.xyz = d_xyz;
+    P.rgb = d_rgb;
+    PUS_CALL_OK(C, launch_write(0, n_planes, P));
+    if (xyz) PUS_CALL_OK(C, download(xyz, d_xyz, (size_t)total * 3));
+    if (rgb) PUS_CALL_OK(C, download(rgb, d_rgb, (size_t)total * 3));
   }
   if (labels && n_frames > 0) {
-    CCHK(d_lab.alloc((size_t)n_frames * width * height));
-    CCHK(d_ptr.alloc(n_frames + 1));
-    CCHK(cudaMemcpy(d_ptr.p, plane_ptr, (n_frames + 1) * sizeof(int), cudaMemcpyHostToDevice));
-    CCHK(cudaMemset(d_lab.p, 127, (size_t)n_frames * width * height));
-    CCHK(launch_labels(0, n_frames, d_ptr.p, P, d_lab.p));
-    CCHK(cudaMemcpy(labels, d_lab.p, (size_t)n_frames * width * height, cudaMemcpyDeviceToHost));
+    PUS_CALL_OK(C, A.get(d_lab, (size_t)n_frames * width * height));
+    PUS_CALL_OK(C, A.upload(d_ptr, plane_ptr, n_frames + 1));
+    PUS_CALL_OK(C, cudaMemset(d_lab, 127, (size_t)n_frames * width * height));
+    PUS_CALL_OK(C, launch_labels(0, n_frames, d_ptr, P, d_lab));
+    PUS_CALL_OK(C, download(labels, d_lab, (size_t)n_frames * width * height));
   }
-  CCHK(cudaDeviceSynchronize());
+  PUS_CALL_OK(C, cudaDeviceSynchronize());
   return total;
 }
-
-#define DCHK(call)                                                                                        \
-  do {                                                                                                    \
-    cudaError_t e__ = (call);                                                                             \
-    if (e__ != cudaSuccess) { g_err = std::string("pus_popup_depth: ") + #call + ": " + cudaGetErrorString(e__); return -1; } \
-  } while (0)
 
 extern "C" int pus_popup_depth(int device, int n_frames, const int* plane_ptr, const int* poly_ptr, const float* polys,
                                const float* planes_sensor, const float* Ts, const float* invK, int width, int height,
                                int downsample, float ceiling_threshold, float* depth) {
   using namespace pus::cloud;
-  auto refuse = [](const char* why) { g_err = std::string("pus_popup_depth: ") + why; return -1; };
-  if (n_frames < 0) return refuse("n_frames < 0");
-  if (!plane_ptr || plane_ptr[0] != 0) return refuse("plane_ptr must be given and start at 0");
-  if (width <= 0 || height <= 0) return refuse("width and height must be positive");
-  if (downsample && ((width | height) & 1)) return refuse("downsample mode needs an even width and height");
-  if (!depth) return refuse("depth must be given");
+  const Call C{"pus_popup_depth"};
+  if (n_frames < 0) return C.refuse("n_frames < 0");
+  if (!plane_ptr || plane_ptr[0] != 0) return C.refuse("plane_ptr must be given and start at 0");
+  if (width <= 0 || height <= 0) return C.refuse("width and height must be positive");
+  if (downsample && ((width | height) & 1)) return C.refuse("downsample mode needs an even width and height");
+  if (!depth) return C.refuse("depth must be given");
   std::vector<Job> jobs;
   std::vector<int2> vtx;
-  const long long rows = plane_jobs("pus_popup_depth: ", n_frames, plane_ptr, poly_ptr, polys, planes_sensor, Ts, invK,
-                                    downsample, jobs, vtx);
+  const long long rows = plane_jobs(C, n_frames, plane_ptr, poly_ptr, polys, planes_sensor, Ts, invK, downsample, jobs, vtx);
   if (rows < 0) return -1;
   const int n_planes = (int)jobs.size(), n_vtx = (int)vtx.size();
-  {
-    int ndev = 0;
-    cudaError_t de = cudaGetDeviceCount(&ndev);
-    if (de != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
-      return refuse("no CUDA device usable; libpopup_gpu has no CPU fallback");
-  }
+  if (C.check_device(device) < 0) return -1;
   if (n_frames == 0) return 0;
-  DCHK(cudaSetDevice(device));
+  PUS_CALL_OK(C, cudaSetDevice(device));
   const int scale = downsample ? 2 : 1, fw = width / scale, fh = height / scale;
   const size_t out_n = (size_t)n_frames * width * height, fill_n = (size_t)n_frames * fw * fh;
-  DevBuf<Job> d_jobs;
-  DevBuf<int2> d_vtx, d_span;
-  DevBuf<Edge> d_edges;
-  DevBuf<float> d_planes, d_T, d_K, d_fill, d_out;
-  DevBuf<int> d_ptr;
-  DCHK(d_jobs.alloc(n_planes));
-  DCHK(d_vtx.alloc(n_vtx));
-  DCHK(d_edges.alloc(n_vtx));
-  DCHK(d_span.alloc(rows));
-  DCHK(d_planes.alloc((size_t)n_planes * 4));
-  DCHK(d_T.alloc((size_t)n_frames * 16));
-  DCHK(d_K.alloc(9));
-  DCHK(d_ptr.alloc(n_frames + 1));
-  DCHK(d_fill.alloc(fill_n));
-  if (downsample) DCHK(d_out.alloc(out_n));
-  if (n_planes > 0) {
-    DCHK(cudaMemcpy(d_jobs.p, jobs.data(), n_planes * sizeof(Job), cudaMemcpyHostToDevice));
-    DCHK(cudaMemcpy(d_planes.p, planes_sensor, (size_t)n_planes * 4 * sizeof(float), cudaMemcpyHostToDevice));
-  }
-  if (n_vtx > 0) DCHK(cudaMemcpy(d_vtx.p, vtx.data(), n_vtx * sizeof(int2), cudaMemcpyHostToDevice));
-  DCHK(cudaMemcpy(d_T.p, Ts, (size_t)n_frames * 16 * sizeof(float), cudaMemcpyHostToDevice));
-  DCHK(cudaMemcpy(d_K.p, invK, 9 * sizeof(float), cudaMemcpyHostToDevice));
-  DCHK(cudaMemcpy(d_ptr.p, plane_ptr, (n_frames + 1) * sizeof(int), cudaMemcpyHostToDevice));
-  DCHK(launch_depth(0, n_frames, n_planes, d_ptr.p, d_jobs.p, d_vtx.p, d_edges.p, d_span.p, d_planes.p, d_T.p, d_K.p, width,
-                    height, downsample, ceiling_threshold, d_fill.p, d_out.p));
-  DCHK(cudaMemcpy(depth, downsample ? d_out.p : d_fill.p, out_n * sizeof(float), cudaMemcpyDeviceToHost));
+  TempAlloc A;
+  Job* d_jobs = nullptr;
+  int2 *d_vtx = nullptr, *d_span = nullptr;
+  Edge* d_edges = nullptr;
+  float *d_planes = nullptr, *d_T = nullptr, *d_K = nullptr, *d_fill = nullptr, *d_out = nullptr;
+  int* d_ptr = nullptr;
+  PUS_CALL_OK(C, A.upload(d_jobs, jobs.data(), n_planes));
+  PUS_CALL_OK(C, A.upload(d_planes, planes_sensor, (size_t)n_planes * 4));
+  PUS_CALL_OK(C, A.upload(d_vtx, vtx.data(), n_vtx));
+  PUS_CALL_OK(C, A.upload(d_T, Ts, (size_t)n_frames * 16));
+  PUS_CALL_OK(C, A.upload(d_K, invK, 9));
+  PUS_CALL_OK(C, A.upload(d_ptr, plane_ptr, n_frames + 1));
+  PUS_CALL_OK(C, A.get(d_edges, n_vtx));
+  PUS_CALL_OK(C, A.get(d_span, rows));
+  PUS_CALL_OK(C, A.get(d_fill, fill_n));
+  if (downsample) PUS_CALL_OK(C, A.get(d_out, out_n));
+  PUS_CALL_OK(C, launch_depth(0, n_frames, n_planes, d_ptr, d_jobs, d_vtx, d_edges, d_span, d_planes, d_T, d_K, width,
+                              height, downsample, ceiling_threshold, d_fill, d_out));
+  PUS_CALL_OK(C, download(depth, downsample ? d_out : d_fill, out_n));
   return 0;
 }
 
@@ -1334,81 +1261,58 @@ cudaError_t launch_pack(cudaStream_t st, const Params& P, const long long* d_off
 }  // namespace poly
 }  // namespace pus
 
-#define GCHK(call)                                                                                          \
-  do {                                                                                                      \
-    cudaError_t e__ = (call);                                                                               \
-    if (e__ != cudaSuccess) { g_err = std::string("pus_popup_polygons: ") + #call + ": " + cudaGetErrorString(e__); return -1; } \
-  } while (0)
-
 extern "C" int pus_popup_polygons(int device, int n_frames, const int* seg_ptr, const float* segs, const float* K,
                                   const float* invK, const float* Ts, int width, int height, float ceiling_threshold,
                                   float walllength_threshold, int* bound_counts, int* cut_counts, int* world_counts,
                                   float* bound2d, float* cut2d, float* world3d, long long bound_capacity,
                                   long long cut_capacity, long long world_capacity) {
   using namespace pus::poly;
-  auto refuse = [](const char* why) { g_err = std::string("pus_popup_polygons: ") + why; return -1; };
+  const Call C{"pus_popup_polygons"};
   auto finite = [](const float* a, size_t n) {
     for (size_t i = 0; i < n; i++)
       if (!std::isfinite(a[i])) return false;
     return true;
   };
-  if (n_frames < 0) return refuse("n_frames < 0");
-  if (!seg_ptr || seg_ptr[0] != 0) return refuse("seg_ptr must be given and start at 0");
-  for (int f = 0; f < n_frames; f++) {
-    const int n = seg_ptr[f + 1] - seg_ptr[f];
-    if (n < 0) return refuse("seg_ptr is not ascending");
-    if (n > PUS_POPUP_MAX_SEGMENTS) return refuse("a frame has more than PUS_POPUP_MAX_SEGMENTS segments");
-  }
-  if (width < 2 || height < 2) return refuse("width and height must be at least 2");
+  if (n_frames < 0) return C.refuse("n_frames < 0");
+  std::vector<int> rf;
+  if (const char* why = row_frames(n_frames, seg_ptr, rf, true)) return C.refuse(why);
+  if (width < 2 || height < 2) return C.refuse("width and height must be at least 2");
   const int n_seg = seg_ptr[n_frames];
   const int n_rows = n_seg + n_frames;
-  if (n_seg > 0 && !segs) return refuse("segs must be given");
+  if (n_seg > 0 && !segs) return C.refuse("segs must be given");
   for (long long i = 0; i < 4LL * n_seg; i++)
-    if (!(std::fabs(segs[i]) <= PUS_POPUP_MAX_COORD)) return refuse("a segment coordinate is not finite or exceeds PUS_POPUP_MAX_COORD");
-  if (!K || !invK || !finite(K, 9) || !finite(invK, 9)) return refuse("K and invK must be given and finite");
-  if (n_frames > 0 && (!Ts || !finite(Ts, (size_t)n_frames * 16))) return refuse("Ts must be given and finite");
-  if (!bound_counts || !cut_counts || !world_counts) return refuse("the count arrays must be given");
+    if (!(std::fabs(segs[i]) <= PUS_POPUP_MAX_COORD)) return C.refuse("a segment coordinate is not finite or exceeds PUS_POPUP_MAX_COORD");
+  if (!K || !invK || !finite(K, 9) || !finite(invK, 9)) return C.refuse("K and invK must be given and finite");
+  if (n_frames > 0 && (!Ts || !finite(Ts, (size_t)n_frames * 16))) return C.refuse("Ts must be given and finite");
+  if (!bound_counts || !cut_counts || !world_counts) return C.refuse("the count arrays must be given");
   if (n_frames == 0) return 0;
-  std::vector<int> rf(n_rows);
-  for (int f = 0; f < n_frames; f++)
-    for (int r = seg_ptr[f] + f; r < seg_ptr[f + 1] + f + 1; r++) rf[r] = f;
-  {
-    int ndev = 0;
-    cudaError_t de = cudaGetDeviceCount(&ndev);
-    if (de != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
-      return refuse("no CUDA device usable; libpopup_gpu has no CPU fallback");
-  }
-  GCHK(cudaSetDevice(device));
-  DevBuf<int> d_ptr, d_rf, d_cnt;
-  DevBuf<float> d_segs, d_K, d_iK, d_T, d_pl, d_ends, d_b, d_c, d_w, d_ob, d_oc, d_ow;
-  DevBuf<long long> d_off;
-  GCHK(d_ptr.alloc(n_frames + 1));
-  GCHK(d_rf.alloc(n_rows));
-  GCHK(d_segs.alloc((size_t)n_seg * 4));
-  GCHK(d_K.alloc(9));
-  GCHK(d_iK.alloc(9));
-  GCHK(d_T.alloc((size_t)n_frames * 16));
-  GCHK(d_pl.alloc((size_t)n_rows * 4));
-  GCHK(d_ends.alloc((size_t)n_rows * 6));
-  GCHK(d_b.alloc((size_t)n_rows * kBoundSlot * 2));
-  GCHK(d_c.alloc((size_t)n_rows * kCutSlot * 2));
-  GCHK(d_w.alloc((size_t)n_rows * kCutSlot * 3));
-  GCHK(d_cnt.alloc((size_t)n_rows * 3));
-  GCHK(d_off.alloc((size_t)n_rows * 3));
-  GCHK(cudaMemcpy(d_ptr.p, seg_ptr, (n_frames + 1) * sizeof(int), cudaMemcpyHostToDevice));
-  GCHK(cudaMemcpy(d_rf.p, rf.data(), n_rows * sizeof(int), cudaMemcpyHostToDevice));
-  if (n_seg > 0) GCHK(cudaMemcpy(d_segs.p, segs, (size_t)n_seg * 4 * sizeof(float), cudaMemcpyHostToDevice));
-  GCHK(cudaMemcpy(d_K.p, K, 9 * sizeof(float), cudaMemcpyHostToDevice));
-  GCHK(cudaMemcpy(d_iK.p, invK, 9 * sizeof(float), cudaMemcpyHostToDevice));
-  GCHK(cudaMemcpy(d_T.p, Ts, (size_t)n_frames * 16 * sizeof(float), cudaMemcpyHostToDevice));
+  if (C.check_device(device) < 0) return -1;
+  PUS_CALL_OK(C, cudaSetDevice(device));
+  TempAlloc A;
+  int *d_ptr = nullptr, *d_rf = nullptr, *d_cnt = nullptr;
+  float *d_segs = nullptr, *d_K = nullptr, *d_iK = nullptr, *d_T = nullptr, *d_pl = nullptr, *d_ends = nullptr, *d_b = nullptr,
+        *d_c = nullptr, *d_w = nullptr, *d_ob = nullptr, *d_oc = nullptr, *d_ow = nullptr;
+  long long* d_off = nullptr;
+  PUS_CALL_OK(C, A.upload(d_ptr, seg_ptr, n_frames + 1));
+  PUS_CALL_OK(C, A.upload(d_rf, rf.data(), n_rows));
+  PUS_CALL_OK(C, A.upload(d_segs, segs, (size_t)n_seg * 4));
+  PUS_CALL_OK(C, A.upload(d_K, K, 9));
+  PUS_CALL_OK(C, A.upload(d_iK, invK, 9));
+  PUS_CALL_OK(C, A.upload(d_T, Ts, (size_t)n_frames * 16));
+  PUS_CALL_OK(C, A.get(d_pl, (size_t)n_rows * 4));
+  PUS_CALL_OK(C, A.get(d_ends, (size_t)n_rows * 6));
+  PUS_CALL_OK(C, A.get(d_b, (size_t)n_rows * kBoundSlot * 2));
+  PUS_CALL_OK(C, A.get(d_c, (size_t)n_rows * kCutSlot * 2));
+  PUS_CALL_OK(C, A.get(d_w, (size_t)n_rows * kCutSlot * 3));
+  PUS_CALL_OK(C, A.get(d_cnt, (size_t)n_rows * 3));
   // the planes and the world ground endpoints: get_plane_equation, as pus_popup_fit_frames runs it (mode 0)
-  GCHK(launch_fit(0, n_frames, d_ptr.p, d_rf.p, n_rows, d_segs.p, d_iK.p, d_T.p, 0.f, 0, nullptr, d_pl.p, nullptr, nullptr,
-                  d_ends.p));
-  Params P{d_ptr.p, d_rf.p, n_rows, d_segs.p, d_K.p, d_iK.p, d_T.p, d_pl.p, d_ends.p, width, height, ceiling_threshold,
-           walllength_threshold, d_b.p, d_c.p, d_w.p, d_cnt.p};
-  GCHK(launch_rows(0, P));
+  PUS_CALL_OK(C, launch_fit(0, n_frames, d_ptr, d_rf, n_rows, d_segs, d_iK, d_T, 0.f, 0, nullptr, d_pl, nullptr, nullptr,
+                            d_ends));
+  Params P{d_ptr, d_rf, n_rows, d_segs, d_K, d_iK, d_T, d_pl, d_ends, width, height, ceiling_threshold,
+           walllength_threshold, d_b, d_c, d_w, d_cnt};
+  PUS_CALL_OK(C, launch_rows(0, P));
   std::vector<int> cnt((size_t)n_rows * 3);
-  GCHK(cudaMemcpy(cnt.data(), d_cnt.p, cnt.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  PUS_CALL_OK(C, download(cnt.data(), d_cnt, cnt.size()));
   std::memcpy(bound_counts, cnt.data(), n_rows * sizeof(int));
   std::memcpy(cut_counts, cnt.data() + n_rows, n_rows * sizeof(int));
   std::memcpy(world_counts, cnt.data() + 2 * (size_t)n_rows, n_rows * sizeof(int));
@@ -1421,17 +1325,17 @@ extern "C" int pus_popup_polygons(int device, int n_frames, const int* seg_ptr, 
       tot[k] += cnt[(size_t)k * n_rows + r];
     }
   if ((bound2d && bound_capacity < tot[0]) || (cut2d && cut_capacity < tot[1]) || (world3d && world_capacity < tot[2]))
-    return refuse("a capacity is smaller than its number of vertices");
+    return C.refuse("a capacity is smaller than its number of vertices");
   if (!bound2d && !cut2d && !world3d) return 0;   // size query
-  GCHK(cudaMemcpy(d_off.p, off.data(), off.size() * sizeof(long long), cudaMemcpyHostToDevice));
-  if (bound2d) GCHK(d_ob.alloc((size_t)tot[0] * 2));
-  if (cut2d) GCHK(d_oc.alloc((size_t)tot[1] * 2));
-  if (world3d) GCHK(d_ow.alloc((size_t)tot[2] * 3));
-  GCHK(launch_pack(0, P, d_off.p, d_ob.p, d_oc.p, d_ow.p));
-  if (bound2d && tot[0] > 0) GCHK(cudaMemcpy(bound2d, d_ob.p, (size_t)tot[0] * 2 * sizeof(float), cudaMemcpyDeviceToHost));
-  if (cut2d && tot[1] > 0) GCHK(cudaMemcpy(cut2d, d_oc.p, (size_t)tot[1] * 2 * sizeof(float), cudaMemcpyDeviceToHost));
-  if (world3d && tot[2] > 0) GCHK(cudaMemcpy(world3d, d_ow.p, (size_t)tot[2] * 3 * sizeof(float), cudaMemcpyDeviceToHost));
-  GCHK(cudaDeviceSynchronize());
+  PUS_CALL_OK(C, A.upload(d_off, off.data(), off.size()));
+  if (bound2d) PUS_CALL_OK(C, A.get(d_ob, (size_t)tot[0] * 2));
+  if (cut2d) PUS_CALL_OK(C, A.get(d_oc, (size_t)tot[1] * 2));
+  if (world3d) PUS_CALL_OK(C, A.get(d_ow, (size_t)tot[2] * 3));
+  PUS_CALL_OK(C, launch_pack(0, P, d_off, d_ob, d_oc, d_ow));
+  if (bound2d) PUS_CALL_OK(C, download(bound2d, d_ob, (size_t)tot[0] * 2));
+  if (cut2d) PUS_CALL_OK(C, download(cut2d, d_oc, (size_t)tot[1] * 2));
+  if (world3d) PUS_CALL_OK(C, download(world3d, d_ow, (size_t)tot[2] * 3));
+  PUS_CALL_OK(C, cudaDeviceSynchronize());
   return 0;
 }
 
@@ -1534,40 +1438,27 @@ cudaError_t select(cudaStream_t st, Alloc& A, int n_frames, const pus_edge_param
 }  // namespace edges
 }  // namespace pus
 
-#define ECHK(call)                                                                                          \
-  do {                                                                                                      \
-    cudaError_t e__ = (call);                                                                               \
-    if (e__ != cudaSuccess) { g_err = std::string("pus_popup_edges: ") + #call + ": " + cudaGetErrorString(e__); return -1; } \
-  } while (0)
-
 extern "C" int pus_popup_edges(int device, int n_frames, const unsigned char* labels, int width, int height,
                                const int* line_ptr, const float* lines, const pus_edge_params* params, int* status,
                                int* open_counts, int* connect_counts, float* open_segs, float* connect_segs,
                                int* open_in_connect, long long open_capacity, long long connect_capacity) {
   using namespace pus::edges;
-  auto refuse = [](const std::string& why) { g_err = "pus_popup_edges: " + why; return -1; };
+  const Call C{"pus_popup_edges"};
   const std::string why = args_error(n_frames, labels, width, height, line_ptr, lines, params, status, open_counts,
                                       connect_counts);
-  if (!why.empty()) return refuse(why);
-  {
-    int ndev = 0;
-    cudaError_t de = cudaGetDeviceCount(&ndev);
-    if (de != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
-      return refuse("no CUDA device usable; libpopup_gpu has no CPU fallback");
-  }
+  if (!why.empty()) return C.refuse(why);
+  if (C.check_device(device) < 0) return -1;
   if (n_frames == 0) return 0;
-  ECHK(cudaSetDevice(device));
+  PUS_CALL_OK(C, cudaSetDevice(device));
   const pus_edge_params P = *params;
   const long long n_lines = line_ptr[n_frames];
-  const size_t lab_n = (size_t)n_frames * width * height;
   TempAlloc A;
   unsigned char* d_lab = nullptr;
-  ECHK(A.get(d_lab, lab_n));
-  ECHK(cudaMemcpy(d_lab, labels, lab_n, cudaMemcpyHostToDevice));
+  PUS_CALL_OK(C, A.upload(d_lab, labels, (size_t)n_frames * width * height));
   Maps M;
-  ECHK(prep(0, A, n_frames, d_lab, width, height, P, M));
+  PUS_CALL_OK(C, prep(0, A, n_frames, d_lab, width, height, P, M));
   std::vector<int> cnt(n_frames);
-  ECHK(cudaMemcpy(cnt.data(), M.seg_count, n_frames * sizeof(int), cudaMemcpyDeviceToHost));
+  PUS_CALL_OK(C, download(cnt.data(), M.seg_count, n_frames));
   // scratch layout
   std::vector<Frame> fr(n_frames);
   long long tot[4] = {0, 0, 0, 0};
@@ -1576,17 +1467,15 @@ extern "C" int pus_popup_edges(int device, int n_frames, const unsigned char* la
   Frame* d_fr = nullptr;
   float *d_lines = nullptr, *d_open = nullptr, *d_conn = nullptr;
   int *d_inc = nullptr, *d_out = nullptr;
-  ECHK(A.get(d_fr, n_frames));
-  ECHK(A.get(d_lines, 4 * n_lines));
-  ECHK(A.get(d_open, 8 * n_lines));
-  ECHK(A.get(d_conn, 16 * n_lines));
-  ECHK(A.get(d_inc, 2 * n_lines));
-  ECHK(A.get(d_out, 4 * (size_t)n_frames));
-  ECHK(cudaMemcpy(d_fr, fr.data(), n_frames * sizeof(Frame), cudaMemcpyHostToDevice));
-  if (n_lines > 0) ECHK(cudaMemcpy(d_lines, lines, 4 * n_lines * sizeof(float), cudaMemcpyHostToDevice));
-  ECHK(select(0, A, n_frames, P, width, height, M, d_fr, tot, n_lines, d_lines, d_open, d_conn, d_inc, d_out));
+  PUS_CALL_OK(C, A.upload(d_fr, fr.data(), n_frames));
+  PUS_CALL_OK(C, A.upload(d_lines, lines, 4 * n_lines));
+  PUS_CALL_OK(C, A.get(d_open, 8 * n_lines));
+  PUS_CALL_OK(C, A.get(d_conn, 16 * n_lines));
+  PUS_CALL_OK(C, A.get(d_inc, 2 * n_lines));
+  PUS_CALL_OK(C, A.get(d_out, 4 * (size_t)n_frames));
+  PUS_CALL_OK(C, select(0, A, n_frames, P, width, height, M, d_fr, tot, n_lines, d_lines, d_open, d_conn, d_inc, d_out));
   std::vector<int> out(4 * (size_t)n_frames);
-  ECHK(cudaMemcpy(out.data(), d_out, out.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  PUS_CALL_OK(C, download(out.data(), d_out, out.size()));
   long long tot_open = 0, tot_conn = 0;
   int found = 0;
   for (int f = 0; f < n_frames; f++) {
@@ -1598,15 +1487,13 @@ extern "C" int pus_popup_edges(int device, int n_frames, const unsigned char* la
     found += status[f] == 0;
   }
   if ((open_segs && open_capacity < tot_open) || (connect_segs && connect_capacity < tot_conn))
-    return refuse("a capacity is smaller than its number of segments");
+    return C.refuse("a capacity is smaller than its number of segments");
   if (!open_segs && !connect_segs) return found;   // size query
   std::vector<float> os(8 * (size_t)n_lines), cs(16 * (size_t)n_lines);
   std::vector<int> inc(2 * (size_t)n_lines);
-  if (n_lines > 0) {
-    ECHK(cudaMemcpy(os.data(), d_open, os.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    ECHK(cudaMemcpy(cs.data(), d_conn, cs.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    ECHK(cudaMemcpy(inc.data(), d_inc, inc.size() * sizeof(int), cudaMemcpyDeviceToHost));
-  }
+  PUS_CALL_OK(C, download(os.data(), d_open, os.size()));
+  PUS_CALL_OK(C, download(cs.data(), d_conn, cs.size()));
+  PUS_CALL_OK(C, download(inc.data(), d_inc, inc.size()));
   long long po = 0, pc = 0;
   for (int f = 0; f < n_frames; f++) {
     const long long l0 = line_ptr[f];

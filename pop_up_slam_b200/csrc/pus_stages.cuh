@@ -1,14 +1,19 @@
 // pus_stages.cuh -- the pop-up stages' internal launchers: device pointers in, kernels enqueued on a stream.  The extern "C"
 // stage calls (pus_popup.cu, pus_lines.cu) and the pop-up session (pus_frames.cu) launch the same kernels through these.
 // Scratch comes from an Alloc: the stage calls free theirs on return (TempAlloc), the session keeps grow-only buffers.
+// Also the host side every stage call shares: its error messages and device check (Call), and the seg_ptr row table.
 #pragma once
 #include <cuda_runtime.h>
 
+#include <climits>
+#include <new>
+#include <string>
 #include <vector>
 
 #include "../../include/popup_gpu.h"
 
 namespace pus {
+extern thread_local std::string g_err;
 
 // device scratch for a launcher
 struct Alloc {
@@ -21,7 +26,18 @@ struct Alloc {
     p = (T*)v;
     return e;
   }
+  // get, then a synchronous copy of h [0, n) (none when n is 0)
+  template <class T>
+  cudaError_t upload(T*& d, const T* h, size_t n) {
+    const cudaError_t e = get(d, n);
+    return e != cudaSuccess || n == 0 ? e : cudaMemcpy(d, h, n * sizeof(T), cudaMemcpyHostToDevice);
+  }
 };
+// a synchronous copy of d [0, n) into h (none when n is 0)
+template <class T>
+cudaError_t download(T* h, const T* d, size_t n) {
+  return n == 0 ? cudaSuccess : cudaMemcpy(h, d, n * sizeof(T), cudaMemcpyDeviceToHost);
+}
 // cudaMalloc per request, everything freed on destruction
 struct TempAlloc : Alloc {
   std::vector<void*> ps;
@@ -35,6 +51,53 @@ struct TempAlloc : Alloc {
   }
 };
 
+// the messages of one extern "C" call: everything it refuses goes to g_err as "<name>: <why>"
+struct Call {
+  const char* name;
+  int refuse(const std::string& why) const {
+    g_err = std::string(name) + ": " + why;
+    return -1;
+  }
+  // 0, or -1 refused: the library has no CPU path to fall back to
+  int check_device(int device) const {
+    int n = 0;
+    if (cudaGetDeviceCount(&n) == cudaSuccess && device >= 0 && device < n) return 0;
+    return refuse("no CUDA device usable; libpopup_gpu has no CPU fallback");
+  }
+  // true, with "<name>: <what>: <CUDA error>" in g_err, when e is an error
+  bool failed(cudaError_t e, const char* what) const {
+    if (e != cudaSuccess) refuse(std::string(what) + ": " + cudaGetErrorString(e));
+    return e != cudaSuccess;
+  }
+};
+// return -1 from the calling function when `call` fails, reported through the Call C
+#define PUS_CALL_OK(C, call)                    \
+  do {                                          \
+    if ((C).failed((call), #call)) return -1;   \
+  } while (0)
+
+// Frame f of a CSR seg_ptr [n_frames + 1] owns the rows seg_ptr[f] + f .. seg_ptr[f + 1] + f: its ground row, then one row
+// per segment.  Checks all of seg_ptr before row_frame is written: given, starting at 0, and frame by frame non-decreasing
+// and, when capped, at most PUS_POPUP_MAX_SEGMENTS segments; the row count must fit an int.  Then sets each row's frame.
+// Returns NULL, or why seg_ptr is refused.  n_frames >= 0.
+inline const char* row_frames(int n_frames, const int* seg_ptr, std::vector<int>& row_frame, bool capped = false) {
+  if (!seg_ptr || seg_ptr[0] != 0) return "seg_ptr must be given and start at 0";
+  for (int f = 0; f < n_frames; f++) {
+    if (seg_ptr[f + 1] < seg_ptr[f]) return "seg_ptr is not ascending";
+    if (capped && seg_ptr[f + 1] - seg_ptr[f] > PUS_POPUP_MAX_SEGMENTS)
+      return "a frame has more than PUS_POPUP_MAX_SEGMENTS segments";
+  }
+  if (seg_ptr[n_frames] > INT_MAX - n_frames) return "seg_ptr has more rows than an int can count";
+  try {
+    row_frame.resize((size_t)seg_ptr[n_frames] + n_frames);
+  } catch (const std::bad_alloc&) {
+    return "seg_ptr has more rows than host memory holds";
+  }
+  for (int f = 0; f < n_frames; f++)
+    for (int r = seg_ptr[f] + f; r <= seg_ptr[f + 1] + f; r++) row_frame[r] = f;
+  return nullptr;
+}
+
 // ---- lines (pus_lines.cu) ----
 namespace lines {
 struct Dims {
@@ -43,6 +106,8 @@ struct Dims {
   int plim, clim, hcap, nslot;    // pix_limit, chain_limit, half_cap, line_slots of n
 };
 Dims make_dims(int width, int height, int channels, int downsample);
+// NULL when the detector takes frames of this shape, else why not
+const char* shape_error(int width, int height, int channels, int downsample);
 struct Work {   // the detector's buffers; st / fc are each frame's status and line count after detect()
   unsigned char *grey, *lut, *i8, *b8;
   unsigned short *h16, *rec;
