@@ -28,6 +28,8 @@
 #include <string>
 #include <vector>
 
+#include "popup_noise.hpp"
+
 #include "popup_gpu.h"
 
 #ifdef ISAM_FACADE_USE_EIGEN
@@ -107,31 +109,8 @@ inline int mrows(const MatrixXd& m) { return m.rows(); }
 
 namespace detail {
 inline void check(int rc) { if (rc < 0) throw std::runtime_error(std::string("libpopup_gpu: ") + pus_last_error()); }
-// in-place Cholesky A = U^T U of a small SPD matrix; returns U (upper), row-major n x n
-inline std::vector<double> chol_upper(std::vector<double> A, int n) {
-  std::vector<double> U((size_t)n * n, 0.0);
-  for (int i = 0; i < n; i++)
-    for (int j = i; j < n; j++) {
-      double s = A[(size_t)i * n + j];
-      for (int k = 0; k < i; k++) s -= U[(size_t)k * n + i] * U[(size_t)k * n + j];
-      if (i == j) { if (!(s > 0)) throw std::runtime_error("Noise: matrix not positive definite"); U[(size_t)i * n + i] = std::sqrt(s); }
-      else U[(size_t)i * n + j] = s / U[(size_t)i * n + i];
-    }
-  return U;
-}
-inline std::vector<double> inverse_spd(const std::vector<double>& A, int n) {
-  std::vector<double> M = A, I((size_t)n * n, 0.0);
-  for (int i = 0; i < n; i++) I[(size_t)i * n + i] = 1;
-  for (int k = 0; k < n; k++) {
-    double p = M[(size_t)k * n + k];
-    for (int j = 0; j < n; j++) { M[(size_t)k * n + j] /= p; I[(size_t)k * n + j] /= p; }
-    for (int i = 0; i < n; i++) if (i != k) {
-      double f = M[(size_t)i * n + k];
-      for (int j = 0; j < n; j++) { M[(size_t)i * n + j] -= f * M[(size_t)k * n + j]; I[(size_t)i * n + j] -= f * I[(size_t)k * n + j]; }
-    }
-  }
-  return I;
-}
+using pus_noise::chol_upper;    // include/popup_noise.hpp: shared with the plane map
+using pus_noise::inverse_spd;
 }  // namespace detail
 
 // ---------------------------------------------------------------------------------------------
@@ -141,7 +120,7 @@ class Noise {
  public:
   int n = 0;
   std::vector<double> _sqrtinf;  // n x n row-major, upper triangular
-  std::vector<double> packed() const { std::vector<double> p; for (int r = 0; r < n; r++) for (int c = r; c < n; c++) p.push_back(_sqrtinf[(size_t)r * n + c]); return p; }
+  std::vector<double> packed() const { return pus_noise::pack_upper(_sqrtinf, n); }
  protected:
   static std::vector<double> flat(const MatrixXd& m) { int k = mrows(m); std::vector<double> a((size_t)k * k); for (int i = 0; i < k; i++) for (int j = 0; j < k; j++) a[(size_t)i * k + j] = mget(m, i, j); return a; }
 };

@@ -39,6 +39,8 @@
  *   - the error / Jacobian export (pus_weighted_errors .. pus_local_chi2) evaluates at the estimate only (iSAM's default
  *     Selector ESTIMATE; LINPOINT is not provided) and writes caller-owned host arrays only.  Its indices are int32: a
  *     graph whose Jacobian has more than 2^31 - 1 nonzeros is refused with a message.
+ *   - the plane map (pus_map_*) covers Mapper_mono's path without loop closure (loopclose_merge, ORB bag of words); a
+ *     caller's own merge removes plane nodes with pus_remove_node.  The map owns its handle's resident refresh tables.
  */
 #ifndef POPUP_GPU_H
 #define POPUP_GPU_H
@@ -600,6 +602,92 @@ int pus_refresh_run(pus_handle h, double* new_meas);
  * applies it to every stored polygon vertex (Mapping.cpp:609-632): pts_out[i] = float(project(double(pts_in[i])))
  * onto the current device-resident estimate of plane node plane_of_point[i]. */
 int pus_project_to_planes(pus_handle h, int n_points, const int* plane_of_point, const float* pts_in, float* pts_out);
+
+/* ---- plane map: Mapper_mono::processFrame on the device (DESIGN.md section 5.11) ------------------------------------ */
+/* A map bound to one solver handle keeps pop_planar_slam's landmark table (Map_plane, PPS/src/Map_plane.h) on the device
+ * and maps each frame's good planes into the handle's graph as Mapper_mono::processFrame (PPS/src/Mapping.cpp:401-586) and
+ * main_3d's frame loop (PPS/src/main_3d.cpp:366-385, 464-504) do.  Single-threaded, like the handle; it works on the
+ * handle's stream.  The caller sets the handle's properties (Mapping.cpp:31-43: LM, mod_batch 1, epsilons x 0.1).
+ * There are no defaults: every field of the config is used (capi.PlaneMap has the plane_3d_tum_far.yaml and the
+ * Mapping.h:72-94 presets).  Refused at create: a NULL handle or config, a non-finite value, a sigma whose square or
+ * inverse square is not a positive finite number, a plane_sigma_dist_mul that makes a pose-plane sigma non-positive. */
+typedef void* pus_map;
+typedef struct pus_map_config {
+  double edge_asso_2ddist, edge_asso_proj, edge_asso_angle, edge_asso_planedist;   /* findClosestPlane's gates */
+  int assoc_near_frames;
+  double pose_sigmas[6];          /* x y z yaw pitch roll: the prior and odometry noise */
+  double plane_sigmas[3];         /* the ground prior's noise */
+  double plane_sigma_dist_mul;    /* pose-plane sigma = (clamp(dist, 3, 8) - 1) * mul + 5 */
+  double init_wTo[16];            /* the first frame's pose, row-major camera-to-world (main_3d.cpp:368-376) */
+  float invK[9];                  /* row-major, for the measurement refresh */
+} pus_map_config;
+/* one landmark (Map_plane): its plane node, whether that node was removed (pus_remove_node: deteted_by_merge, skipped
+ * and never re-projected), the latest observation's descriptor (copy_plane, Map_plane.cpp:11-29) and the first two
+ * vertices of its 2-D bound and 3-D world polygons, which are all the association reads (n_* of them stored) */
+typedef struct pus_map_landmark {
+  int node, deleted, frame_seq_id, frame_plane_indice, good_plane_indice, being_tracked_times;
+  double plane_dist_cam;
+  int n_bound2d, n_world3d;
+  float bound2d[2][2], world3d[2][3];
+} pus_map_landmark;
+/* One frame's good planes, in one of two forms.  session != NULL: frame `frame` of that pop-up session's last run, read in
+ * place on the device (its good rows, planes_sensor, dist, bound2d, world3d and open segments).  Otherwise n_planes planes
+ * in arrays, each host or device memory (told apart as the session does): planes_sensor [n][4], dist [n], plane_indice [n]
+ * (the plane's row in the frame: 0 ground, 1 + s wall of open segment s), bound_ptr [n + 1] / bound2d [..][2] and
+ * world_ptr [n + 1] / world3d [..][3] (CSR), and the frame's n_segs open segments segs [n_segs][4] for the refresh.
+ * odom7 (host, x y z qw qx qy qz) is the frame's odometry (temp_pose); NULL takes that of the last pus_map_predict_pose. */
+typedef struct pus_map_frame {
+  int seq_id;                       /* main_3d's counter */
+  const double* odom7;
+  pus_popup_session session;
+  int frame;
+  int n_planes;
+  const float *planes_sensor, *dist;
+  const int* plane_indice;
+  const int* bound_ptr; const float* bound2d;
+  const int* world_ptr; const float* world3d;
+  int n_segs; const float* segs;
+} pus_map_frame;
+/* Outputs of one frame; the per-plane arrays (caller-owned host memory, any may be NULL) hold `capacity` entries, in plane
+ * order.  landmark: its index; error: the reference's assoc_error (the match error, -1 for a ground match; 0 for a new
+ * landmark, and -1 for the plane that loses a dual match to a later one); status: 0 matched, 1 a wall whose bound or world
+ * polygon has fewer than two vertices (a new landmark, never matched later: the reference reads past .col(1)), 2 no
+ * candidate (new), 3 lost a dual match (new); factor: its pose-plane factor id.  Per frame: pose_node, n_new and the new
+ * plane nodes (new_nodes, landmark-index order, room for `capacity`), the solve's LM iteration count (pus_stats). */
+typedef struct pus_map_result {
+  int capacity;
+  int n_planes, pose_node, n_new, lm_iterations;
+  int *landmark, *status, *factor, *new_nodes;
+  double* error;
+} pus_map_result;
+int pus_map_create(pus_handle h, const pus_map_config* config, pus_map* out);
+/* destroy gives the handle's refresh tables up (unbound): a later map on the same handle starts them afresh */
+int pus_map_destroy(pus_map m);
+/* main_3d.cpp:366-385 from the handle's device-resident estimates, keyed on the number of MAPPED frames (main_3d keys it on
+ * its frame counter, which also counts frames without good planes, and reads all_frames.back() of an empty list there):
+ * none -> odometry = prediction = the config's initial pose; one -> zero odometry; more -> last.ominus(previous).  The
+ * prediction is last.oplus(odometry); T16 (host or device memory) receives its wTo() as row-major float, ready for
+ * pus_popup_session_run's Ts; odom7 (host, may be NULL) the odometry, which the next pus_map_process_frame takes when its
+ * odom7 is NULL. */
+int pus_map_predict_pose(pus_map m, float* T16, double* odom7);
+/* One frame, in main_3d's order: 1 association (findClosestPlane and the one-to-one rule, against the estimate
+ * last.oplus(odom), the identity on the first frame); 2 graph edits, ids in insertion order: the pose node, the prior at
+ * odom (first frame) or the odometry factor, the new plane nodes in landmark order (initialised at their measurement
+ * through the estimate's oTw), then per plane the ground prior (0,0,-1,0) for a new ground landmark and the pose-plane
+ * factor, noise as isam::Covariance forms it (include/popup_noise.hpp);  3 copy_plane;  4 pus_batch_optimize when
+ * seq_id % 5 == 0, else pus_update;  5 the landmarks' stored 3-D vertices projected onto their planes' new estimates
+ * (as pus_project_to_planes);  6 the measurement refresh (pus_refresh_run) over every mapped frame, whose tables the map
+ * appends to (the frame's open segments, its pose, its planes' factor and row) -- a pus_refresh_bind on the handle
+ * afterwards takes the tables away, and the map then refuses further frames.  A frame without planes changes nothing.
+ * Refused with a message before any edit, map and handle unchanged: NULL arguments, too small a capacity, a session frame
+ * out of range, a non-finite value among those read (planes, dist, the first two vertices, the segments), a
+ * plane_indice outside 0..n_segs, more than one ground plane, a frame with planes but no open segments (as
+ * pus_refresh_bind), malformed CSR offsets, no odometry, a removed last pose.  An edit that fails removes the nodes the
+ * frame added (with their factors) and leaves the map as it was; a failing solve leaves the edits in place.  Deterministic: repeated runs, the session and array forms, host and device
+ * inputs give the same bytes. */
+int pus_map_process_frame(pus_map m, const pus_map_frame* in, pus_map_result* out);
+/* the landmark table (capacity records; out = NULL is a size query); returns the number of landmarks */
+int pus_map_landmarks(pus_map m, int capacity, pus_map_landmark* out);
 
 /* ---- weighted errors and the stacked Jacobian at the current estimate ---------------------------- */
 /* Evaluated on the device, one thread per live factor, with the residual and Jacobian code the solver linearises with.

@@ -1016,3 +1016,170 @@ class PopupFrames:
             out[k] = a
         self._check(self.lib.pus_popup_session_download(self.h, C.byref(dst)))
         return out
+
+
+# ---- plane map (pus_map_*, include/popup_gpu.h) ------------------------------------------------------------------------
+class MapConfig(C.Structure):
+    """pus_map_config (include/popup_gpu.h)"""
+    _fields_ = [("edge_asso_2ddist", C.c_double), ("edge_asso_proj", C.c_double), ("edge_asso_angle", C.c_double),
+                ("edge_asso_planedist", C.c_double), ("assoc_near_frames", C.c_int), ("pose_sigmas", C.c_double * 6),
+                ("plane_sigmas", C.c_double * 3), ("plane_sigma_dist_mul", C.c_double), ("init_wTo", C.c_double * 16),
+                ("invK", C.c_float * 9)]
+
+
+class MapLandmark(C.Structure):
+    """pus_map_landmark (include/popup_gpu.h)"""
+    _fields_ = [(k, C.c_int) for k in ("node", "deleted", "frame_seq_id", "frame_plane_indice", "good_plane_indice",
+                                       "being_tracked_times")] + [
+        ("plane_dist_cam", C.c_double), ("n_bound2d", C.c_int), ("n_world3d", C.c_int),
+        ("bound2d", (C.c_float * 2) * 2), ("world3d", (C.c_float * 3) * 2)]
+
+
+class MapFrame(C.Structure):
+    """pus_map_frame (include/popup_gpu.h)"""
+    _fields_ = [("seq_id", C.c_int), ("odom7", C.c_void_p), ("session", C.c_void_p), ("frame", C.c_int), ("n_planes", C.c_int),
+                ("planes_sensor", C.c_void_p), ("dist", C.c_void_p), ("plane_indice", C.c_void_p), ("bound_ptr", C.c_void_p),
+                ("bound2d", C.c_void_p), ("world_ptr", C.c_void_p), ("world3d", C.c_void_p), ("n_segs", C.c_int),
+                ("segs", C.c_void_p)]
+
+
+class MapResult(C.Structure):
+    """pus_map_result (include/popup_gpu.h)"""
+    _fields_ = [("capacity", C.c_int), ("n_planes", C.c_int), ("pose_node", C.c_int), ("n_new", C.c_int),
+                ("lm_iterations", C.c_int)] + [(k, C.POINTER(C.c_int)) for k in ("landmark", "status", "factor", "new_nodes")] + [
+        ("error", C.POINTER(C.c_double))]
+
+
+# main_3d.cpp:368-376: the TUM fr3 "no texture far" first pose from ground truth (camera-to-world)
+TUM_FAR_INIT_WTO = [-0.4563, 0.2444, -0.8556, -1.2432, 0.8898, 0.1249, -0.4388, 1.9219, -0.0004, -0.9616, -0.2745, 1.0547,
+                    0, 0, 0, 1]
+# pop_planar_slam/params/plane_3d_tum_far.yaml: the covering and 2-D gates disabled
+MAP_PRESET_TUM_FAR = dict(edge_asso_2ddist=10000.0, edge_asso_proj=-1.0, edge_asso_angle=35.0, edge_asso_planedist=2.0,
+                          assoc_near_frames=1000, pose_sigmas=[2.0] * 6, plane_sigmas=[0.05] * 3, plane_sigma_dist_mul=2.0)
+# pop_planar_slam/src/Mapping.h:72-94: the in-class values, every gate enabled
+MAP_PRESET_MAPPING_H = dict(edge_asso_2ddist=50.0, edge_asso_proj=0.5, edge_asso_angle=60.0, edge_asso_planedist=4.0,
+                            assoc_near_frames=5, pose_sigmas=[0.001, 0.001, 0.001, 0.01, 0.01, 0.01], plane_sigmas=[0.001] * 3,
+                            plane_sigma_dist_mul=3.0)
+MAP_PRESETS = {"tum_far": MAP_PRESET_TUM_FAR, "mapping_h": MAP_PRESET_MAPPING_H}
+
+
+def map_config(preset, invK, init_wTo=TUM_FAR_INIT_WTO, **over):
+    """A pus_map_config from a preset name ("tum_far" or "mapping_h"), the camera's invK and the first pose; keyword
+    arguments replace preset values."""
+    v = dict(MAP_PRESETS[preset], **over)
+    c = MapConfig()
+    for k in ("edge_asso_2ddist", "edge_asso_proj", "edge_asso_angle", "edge_asso_planedist", "plane_sigma_dist_mul"):
+        setattr(c, k, float(v[k]))
+    c.assoc_near_frames = int(v["assoc_near_frames"])
+    c.pose_sigmas[:] = [float(x) for x in v["pose_sigmas"]]
+    c.plane_sigmas[:] = [float(x) for x in v["plane_sigmas"]]
+    c.init_wTo[:] = [float(x) for x in np.asarray(init_wTo, np.float64).reshape(16)]
+    c.invK[:] = [float(x) for x in np.asarray(invK, np.float32).reshape(9)]
+    return c
+
+
+class PlaneMap:
+    """A plane map (pus_map_*): Mapper_mono::processFrame on the device, bound to a GpuGraphAPI handle.
+
+    config: a MapConfig (map_config(preset, invK)).  predict_pose() -> (T [4, 4] float32, odom7); process_frame(seq_id,
+    planes=dict(planes_sensor [n, 4], dist [n], plane_indice [n], bound [list of [k, 2]], world [list of [k, 3]],
+    segs [m, 4]) or session=(PopupFrames, frame), odom7=None) -> dict of the per-plane and per-frame results;
+    landmarks() -> a numpy structured array of the table."""
+
+    def __init__(self, api, config):
+        self.api, self.lib = api, api.lib
+        self.lib.pus_map_create.argtypes = [C.c_void_p, C.POINTER(MapConfig), C.POINTER(C.c_void_p)]
+        self.lib.pus_map_destroy.argtypes = [C.c_void_p]
+        self.lib.pus_map_predict_pose.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        self.lib.pus_map_process_frame.argtypes = [C.c_void_p, C.POINTER(MapFrame), C.POINTER(MapResult)]
+        self.lib.pus_map_landmarks.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        self.config = config
+        h = C.c_void_p()
+        self._check(self.lib.pus_map_create(api.h, C.byref(config), C.byref(h)))
+        self.h = h
+
+    def _check(self, rc):
+        if rc < 0:
+            raise ApiError(self.lib.pus_last_error().decode())
+        return rc
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.pus_map_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def predict_pose(self, T_out=None):
+        """T_out: None (a host array is returned) or a torch CUDA tensor of 16 float32 written in place"""
+        odom = np.zeros(7)
+        if T_out is not None:
+            self._check(self.lib.pus_map_predict_pose(self.h, C.c_void_p(T_out.data_ptr()), odom.ctypes.data))
+            return T_out, odom
+        T = np.zeros(16, np.float32)
+        self._check(self.lib.pus_map_predict_pose(self.h, T.ctypes.data, odom.ctypes.data))
+        return T.reshape(4, 4), odom
+
+    @staticmethod
+    def _ptr(a):
+        if a is None:
+            return None
+        return a.data_ptr() if hasattr(a, "data_ptr") else a.ctypes.data
+
+    def process_frame(self, seq_id, planes=None, session=None, odom7=None, capacity=None):
+        f = MapFrame()
+        f.seq_id = int(seq_id)
+        keep = []
+        if odom7 is not None:
+            o = np.ascontiguousarray(odom7, np.float64)
+            keep.append(o)
+            f.odom7 = o.ctypes.data
+        if session is not None:
+            sess, frame = session
+            f.session, f.frame = sess.h, int(frame)
+            n_cap = capacity or 1024
+        else:
+            arrs = self._arrays(planes)
+            keep.append(arrs)
+            f.n_planes = int(len(arrs["planes_sensor"]))
+            f.n_segs = int(len(arrs["segs"]))
+            for k in ("planes_sensor", "dist", "plane_indice", "bound_ptr", "bound2d", "world_ptr", "world3d", "segs"):
+                setattr(f, k, self._ptr(arrs[k]))
+            n_cap = capacity or max(f.n_planes, 1)
+        out = {k: np.zeros(n_cap, np.int32) for k in ("landmark", "status", "factor", "new_nodes")}
+        out["error"] = np.zeros(n_cap)
+        r = MapResult()
+        r.capacity = n_cap
+        for k in ("landmark", "status", "factor", "new_nodes"):
+            setattr(r, k, out[k].ctypes.data_as(C.POINTER(C.c_int)))
+        r.error = out["error"].ctypes.data_as(C.POINTER(C.c_double))
+        self._check(self.lib.pus_map_process_frame(self.h, C.byref(f), C.byref(r)))
+        n = r.n_planes
+        res = {k: out[k][:n].copy() for k in ("landmark", "status", "factor", "error")}
+        res.update(new_nodes=out["new_nodes"][:r.n_new].copy(), n_planes=n, pose_node=r.pose_node, n_new=r.n_new,
+                   lm_iterations=r.lm_iterations)
+        return res
+
+    @staticmethod
+    def _arrays(p):
+        """numpy (host) or torch CUDA (device) arrays of one frame's planes, CSR-packed"""
+        if "bound_ptr" in p:
+            return p
+        lens = lambda polys: np.concatenate([[0], np.cumsum([len(x) for x in polys])]).astype(np.int32)
+        cat = lambda polys, d: (np.concatenate([np.asarray(x, np.float32).reshape(-1, d) for x in polys])
+                                if sum(len(x) for x in polys) else np.zeros((0, d), np.float32))
+        return dict(planes_sensor=np.ascontiguousarray(p["planes_sensor"], np.float32).reshape(-1, 4),
+                    dist=np.ascontiguousarray(p["dist"], np.float32), plane_indice=np.ascontiguousarray(p["plane_indice"], np.int32),
+                    bound_ptr=lens(p["bound"]), bound2d=np.ascontiguousarray(cat(p["bound"], 2)),
+                    world_ptr=lens(p["world"]), world3d=np.ascontiguousarray(cat(p["world"], 3)),
+                    segs=np.ascontiguousarray(p["segs"], np.float32).reshape(-1, 4))
+
+    def landmarks(self):
+        n = self._check(self.lib.pus_map_landmarks(self.h, 0, None))
+        buf = (MapLandmark * max(n, 1))()
+        self._check(self.lib.pus_map_landmarks(self.h, n, buf))
+        return np.ctypeslib.as_array(buf)[:n].copy()

@@ -87,6 +87,8 @@ struct Solver {
   struct RefreshTables {
     bool bound = false;
     int n_frames = 0, n_seg = 0, n_rows = 0, n_map = 0;
+    int cap_frames = 0, cap_seg = 0, cap_map = 0;  // room of the carved sections (a plane map appends into them)
+    const void* owner = nullptr;                  // the plane map that appends to these tables; nullptr after pus_refresh_bind
     std::vector<int> frame_node, map_fid, mrow;   // host copies: pose node id per frame, factor id and plane row per map entry
     uint64_t slot_topo = 0;                       // layout version the device slot / pose-index tables were built for
     void* mem = nullptr; size_t bytes = 0;        // one allocation carved into the pointers below
@@ -1212,6 +1214,7 @@ static int refresh_slots(Solver* s) {   // (re)build the layout-dependent tables
   }
   for (int m = 0; m < t.n_map; m++) {
     const int fid = t.map_fid[m];
+    if (t.owner && !s->g.ok_factor(fid)) { mslot[m] = -1; continue; }   // a plane map's landmark removed by its caller: skipped
     if (!s->g.ok_factor(fid) || s->g.factors[fid].kind != F_POSE_PLANE || s->fid2slot[fid] < 0) {
       g_err = "pus_refresh_run: map entry " + std::to_string(m) + " is no longer a pose-plane factor; bind again";
       return -1;
@@ -1223,6 +1226,27 @@ static int refresh_slots(Solver* s) {   // (re)build the layout-dependent tables
   CUDA_OK(cudaStreamSynchronize(s->stream));   // (the staging vectors go out of scope)
   t.slot_topo = s->compiled_topo;
   return 0;
+}
+
+// the resident tables' sections, carved from one allocation for room of cap_frames frames, cap_seg segments and cap_map
+// map entries (one row per segment plus a ground row per frame)
+static size_t refresh_bytes(int cap_frames, int cap_seg, int cap_map) {
+  auto al = [](size_t b) { return (b + 255) / 256 * 256; };
+  const size_t rows = (size_t)cap_seg + cap_frames, m = (size_t)std::max(cap_map, 1);
+  return al(4 * (size_t)cap_frames) + al(4 * (size_t)(cap_frames + 1)) + al(4 * rows) + 2 * al(4 * m) + al(16 * (size_t)std::max(cap_seg, 1)) +
+         al(36) + al(64 * (size_t)cap_frames) + al(16 * rows) + al(32 * m);
+}
+static void refresh_carve(Solver::RefreshTables& t, void* mem, int cap_frames, int cap_seg, int cap_map) {
+  auto al = [](size_t b) { return (b + 255) / 256 * 256; };
+  char* base = static_cast<char*>(mem);
+  size_t off = 0;
+  auto carve = [&](size_t b) { void* p = base + off; off += al(b); return p; };
+  const size_t rows = (size_t)cap_seg + cap_frames, m = (size_t)std::max(cap_map, 1);
+  t.d_fpose = (int*)carve(4 * (size_t)cap_frames); t.d_ptr = (int*)carve(4 * (size_t)(cap_frames + 1)); t.d_rf = (int*)carve(4 * rows);
+  t.d_mrow = (int*)carve(4 * m); t.d_mslot = (int*)carve(4 * m);
+  t.d_segs = (float*)carve(16 * (size_t)std::max(cap_seg, 1)); t.d_K = (float*)carve(36); t.d_T = (float*)carve(64 * (size_t)cap_frames);
+  t.d_ps = (float*)carve(16 * rows); t.d_out = (double*)carve(32 * m);
+  t.cap_frames = cap_frames; t.cap_seg = cap_seg; t.cap_map = cap_map;
 }
 
 int pus_refresh_bind(pus_handle h, int n_frames, const int* frame_pose, const int* seg_ptr, const float* segs, const float* invK,
@@ -1249,22 +1273,15 @@ int pus_refresh_bind(pus_handle h, int n_frames, const int* frame_pose, const in
     if (!s->g.ok_factor(map_fid[m]) || s->g.factors[map_fid[m]].kind != F_POSE_PLANE) { g_err = "map_fid is not a pose-plane factor"; return -1; }
     t.mrow[m] = seg_ptr[f] + f + map_row[m];
   }
-  auto al = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t need = al(4 * (size_t)n_frames) + al(4 * (size_t)(n_frames + 1)) + al(4 * (size_t)n_rows) + 2 * al(4 * (size_t)std::max(n_map, 1)) +
-                      al(16 * (size_t)std::max(n_seg, 1)) + al(36) + al(64 * (size_t)n_frames) + al(16 * (size_t)n_rows) + al(32 * (size_t)std::max(n_map, 1));
+  const size_t need = refresh_bytes(n_frames, n_seg, n_map);
   CUDA_OK(cudaSetDevice(s->device));
   if (need > t.bytes) {
     if (t.mem) { cudaStreamSynchronize(s->stream); cudaFree(t.mem); t.mem = nullptr; t.bytes = 0; }
     CUDA_OK(cudaMalloc(&t.mem, need + need / 2));
     t.bytes = need + need / 2;
   }
-  char* base = static_cast<char*>(t.mem);
-  size_t off = 0;
-  auto carve = [&](size_t b) { void* p = base + off; off += al(b); return p; };
-  t.d_fpose = (int*)carve(4 * (size_t)n_frames); t.d_ptr = (int*)carve(4 * (size_t)(n_frames + 1)); t.d_rf = (int*)carve(4 * (size_t)n_rows);
-  t.d_mrow = (int*)carve(4 * (size_t)std::max(n_map, 1)); t.d_mslot = (int*)carve(4 * (size_t)std::max(n_map, 1));
-  t.d_segs = (float*)carve(16 * (size_t)std::max(n_seg, 1)); t.d_K = (float*)carve(36); t.d_T = (float*)carve(64 * (size_t)n_frames);
-  t.d_ps = (float*)carve(16 * (size_t)n_rows); t.d_out = (double*)carve(32 * (size_t)std::max(n_map, 1));
+  t.owner = nullptr;
+  refresh_carve(t, t.mem, n_frames, n_seg, n_map);
   cudaStream_t st = s->stream;
   CUDA_OK(cudaMemcpyAsync(t.d_ptr, seg_ptr, 4 * (size_t)(n_frames + 1), cudaMemcpyHostToDevice, st));
   CUDA_OK(cudaMemcpyAsync(t.d_rf, row_frame.data(), 4 * (size_t)n_rows, cudaMemcpyHostToDevice, st));
@@ -1343,6 +1360,104 @@ int pus_project_to_planes(pus_handle h, int n_points, const int* plane_of_point,
 }
 
 // ---- weighted errors / stacked Jacobian at the current estimate (pus_export.cu) ----
+}  // extern "C"
+
+// ---- what a plane map (pus_map.cu) needs from its handle ----
+namespace pus {
+// the device estimates current: upload when the topology, the host values or the measurements changed
+int engine_sync(pus_handle h) {
+  NEED(h);
+  Solver* s = SV(h);
+  if (s->g.nodes.empty()) { if (ensure_device(s) < 0) return -1; CUDA_OK(cudaSetDevice(s->device)); return 0; }
+  if (!s->uploaded || s->compiled_topo != s->g.topo_version || s->values_dirty || s->meas_dirty) return upload(s);
+  if (ensure_device(s) < 0) return -1;
+  CUDA_OK(cudaSetDevice(s->device));
+  return 0;
+}
+int engine_device(pus_handle h) { return SV(h)->device; }
+cudaStream_t engine_stream(pus_handle h) { return SV(h)->stream; }
+// the resident estimates of the last upload / solve, indexed by engine_node_index
+const double* engine_pose_lin(pus_handle h) { return SV(h)->hd.pose_lin; }
+const double* engine_plane_lin(pus_handle h) { return SV(h)->hd.plane_lin; }
+// a live node's index into those arrays, or -1 (removed, or not of that kind: 0 pose, 1 plane); valid after engine_sync
+int engine_node_index(pus_handle h, int id, int kind) {
+  const Solver* s = SV(h);
+  if (!s->g.ok_node(id, kind ? NODE_PLANE : NODE_POSE)) return -1;
+  return s->c.node_idx[id];
+}
+bool engine_node_alive(pus_handle h, int id, int kind) { return SV(h)->g.ok_node(id, kind ? NODE_PLANE : NODE_POSE); }
+int engine_iterations(pus_handle h) { return SV(h)->stats.lm_iterations; }
+// Append one frame to the resident refresh tables owned by `owner`: its pose node, its n_segs segments (device pointer,
+// copied on the device) and n_map (factor, plane row) entries.  The first append of an owner starts the tables afresh;
+// the sections grow by half their size and only the new rows are written.  Refused when the caller rebound the tables.
+int engine_refresh_append(pus_handle h, const void* owner, int pose_node, int n_segs, const float* d_segs, const float* invK,
+                          int n_map, const int* fids, const int* rows) {
+  NEED(h);
+  Solver* s = SV(h);
+  Solver::RefreshTables& t = s->rt;
+  const bool fresh = t.owner != owner;
+  const int nf = fresh ? 0 : t.n_frames, ns = fresh ? 0 : t.n_seg, nm = fresh ? 0 : t.n_map;
+  const int need_f = nf + 1, need_s = ns + n_segs, need_m = nm + n_map;
+  cudaStream_t st = s->stream;
+  CUDA_OK(cudaSetDevice(s->device));
+  if (fresh || need_f > t.cap_frames || need_s > t.cap_seg || need_m > t.cap_map) {
+    const int cf = std::max(need_f, fresh ? 16 : t.cap_frames + t.cap_frames / 2);
+    const int cs = std::max(need_s, fresh ? 256 : t.cap_seg + t.cap_seg / 2);
+    const int cm = std::max(need_m, fresh ? 128 : t.cap_map + t.cap_map / 2);
+    const size_t bytes = refresh_bytes(cf, cs, cm);
+    void* mem = nullptr;
+    CUDA_OK(cudaMalloc(&mem, bytes));
+    Solver::RefreshTables old = t;
+    refresh_carve(t, mem, cf, cs, cm);
+    if (!fresh) {
+      CUDA_OK(cudaMemcpyAsync(t.d_ptr, old.d_ptr, 4 * (size_t)(nf + 1), cudaMemcpyDeviceToDevice, st));
+      CUDA_OK(cudaMemcpyAsync(t.d_rf, old.d_rf, 4 * (size_t)(ns + nf), cudaMemcpyDeviceToDevice, st));
+      if (nm) CUDA_OK(cudaMemcpyAsync(t.d_mrow, old.d_mrow, 4 * (size_t)nm, cudaMemcpyDeviceToDevice, st));
+      if (ns) CUDA_OK(cudaMemcpyAsync(t.d_segs, old.d_segs, 16 * (size_t)ns, cudaMemcpyDeviceToDevice, st));
+      CUDA_OK(cudaMemcpyAsync(t.d_ps, old.d_ps, 16 * (size_t)(ns + nf), cudaMemcpyDeviceToDevice, st));
+    }
+    if (old.mem) { CUDA_OK(cudaStreamSynchronize(st)); cudaFree(old.mem); }
+    t.mem = mem; t.bytes = bytes;
+    CUDA_OK(cudaMemcpyAsync(t.d_K, invK, 36, cudaMemcpyHostToDevice, st));   // (every new allocation)
+  }
+  if (fresh) {
+    const int zero = 0;
+    CUDA_OK(cudaMemcpyAsync(t.d_ptr, &zero, 4, cudaMemcpyHostToDevice, st));
+    t.frame_node.clear(); t.map_fid.clear(); t.mrow.clear();
+    t.owner = owner;
+  }
+  const int end = need_s;
+  std::vector<int> rf(n_segs + 1, nf), mrow(n_map);
+  for (int m = 0; m < n_map; m++) mrow[m] = ns + nf + rows[m];
+  CUDA_OK(cudaMemcpyAsync(t.d_ptr + nf + 1, &end, 4, cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaMemcpyAsync(t.d_rf + ns + nf, rf.data(), 4 * (size_t)(n_segs + 1), cudaMemcpyHostToDevice, st));
+  if (n_segs) CUDA_OK(cudaMemcpyAsync(t.d_segs + 4 * (size_t)ns, d_segs, 16 * (size_t)n_segs, cudaMemcpyDeviceToDevice, st));
+  CUDA_OK(cudaMemsetAsync(t.d_ps + 4 * (size_t)(ns + nf), 0, 16 * (size_t)(n_segs + 1), st));
+  if (n_map) CUDA_OK(cudaMemcpyAsync(t.d_mrow + nm, mrow.data(), 4 * (size_t)n_map, cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaStreamSynchronize(st));   // (the staging vectors go out of scope)
+  t.frame_node.push_back(pose_node);
+  t.map_fid.insert(t.map_fid.end(), fids, fids + n_map);
+  t.mrow.insert(t.mrow.end(), mrow.begin(), mrow.end());
+  t.n_frames = need_f; t.n_seg = need_s; t.n_rows = need_s + need_f; t.n_map = need_m;
+  t.slot_topo = 0;
+  t.bound = true;
+  return 0;
+}
+// whether `owner` still owns the handle's refresh tables (false once the caller rebound them)
+bool engine_refresh_owned(pus_handle h, const void* owner) { return SV(h)->rt.owner == owner; }
+// a destroyed map gives its tables up: they are unbound, and the next map's first append starts afresh
+void engine_refresh_release(pus_handle h, const void* owner) {
+  Solver::RefreshTables& t = SV(h)->rt;
+  if (!owner || t.owner != owner) return;
+  t.owner = nullptr;
+  t.bound = false;
+  t.n_frames = t.n_seg = t.n_rows = t.n_map = 0;
+  t.frame_node.clear(); t.map_fid.clear(); t.mrow.clear();
+}
+}  // namespace pus
+
+extern "C" {
+
 // Every export starts as pus_project_to_planes does: re-upload when the topology, the host values or the measurements changed,
 // otherwise only bind the device (the estimate on the device is then the one a resident solve left there).  The per-record
 // table is rebuilt after a layout rebuild: one pass over the nodes (column of every live node) and one over the factors (first

@@ -211,6 +211,15 @@ __global__ void __launch_bounds__(kScan) job_scan_kernel(int n, const int* good_
 }
 }  // namespace frames
 
+bool on_device(const void* p) {
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+
 namespace {
 struct Slot {
   void* p = nullptr;
@@ -259,15 +268,6 @@ struct Arena : pus::Alloc {
   explicit Arena(Session& s) : S(s) {}
   cudaError_t raw(void** p, size_t bytes) override { return S.slot(S.dev, S.cursor, false, p, bytes); }
 };
-
-bool on_device(const void* p) {
-  cudaPointerAttributes a{};
-  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-    cudaGetLastError();
-    return false;
-  }
-  return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
 
 bool finite9(const float* a) {
   for (int i = 0; i < 9; i++)

@@ -142,8 +142,10 @@ __global__ void store_meas_kernel(int n_map, const int* __restrict__ map_row, co
     const double n = sqrt(z);
     v[0] /= n; v[1] /= n; v[2] /= n; v[3] /= n;
   }
+  for (int i = 0; i < 4; i++) out[(size_t)m * 4 + i] = v[i];
+  if (map_slot[m] < 0) return;   // (a plane map's entry whose factor the caller removed)
   double* dst = pp_meas + (size_t)map_slot[m] * 4;
-  for (int i = 0; i < 4; i++) { dst[i] = v[i]; out[(size_t)m * 4 + i] = v[i]; }
+  for (int i = 0; i < 4; i++) dst[i] = v[i];
 }
 
 // Plane3d::project_to_plane (isam_plane3d.h:172-177): normal() = abc/|abc|, d() = -d/|abc|

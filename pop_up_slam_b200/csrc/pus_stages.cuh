@@ -15,6 +15,9 @@
 namespace pus {
 extern thread_local std::string g_err;
 
+// whether p is device (or managed) memory; anything else is taken as host memory (pus_frames.cu)
+bool on_device(const void* p);
+
 // device scratch for a launcher
 struct Alloc {
   virtual ~Alloc() = default;
